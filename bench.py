@@ -1,16 +1,18 @@
 #!/usr/bin/env python
 """bench.py -- layouts/sec of the LayoutDM denoising loop (BASELINE.json metric) on N GPUs of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 A "step" is one full pass of the hot path over one batch: `sample()` of B=1024 layouts per GPU through all T=100
 denoising iterations (BASELINE.json configs[1]: rico25 unconditional, T=100, batch 1024, random sampling).
 Prints ONE JSON line (rank 0).  `value` = layouts/s with everything device-resident; `e2e` = the same metric through
 the host-buffer C-ABI entry (ldm_sample_host: pinned-host inputs -> H2D -> loop -> D2H of the ids);
-`roofline` = the dominant kernel against the measured bf16 tensor peak; `cpu_baseline` = the unmodified reference's
+`roofline` = the dominant kernel against the H100 SXM data-sheet dense 16-bit tensor peak; `cpu_baseline` = the unmodified reference's
 `LayoutDM.sample` on the host cores (bounded sample; packaged by oracle/make_ref.py), `gpu_eager_baseline` = the same
 reference run eagerly on the GPU.  `--impl reference` times the CPU reference alone.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (rank 0's ids) as DIR/ids.npy (float64);
+the inputs (weights, seeds) depend only on the arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -54,7 +56,7 @@ BYTES = {"embed_adaln": 237_568 + 118_784, "qkv_gemm": 118_784 + 393_216, "atten
 
 
 def load_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed ncu --set full capture (profiles/ncu_traffic.json)"""
+    """DRAM bytes per launch of `kernel` from a local ncu capture (tools/ncu_summary.py --traffic), None without one"""
     try:
         d = json.load(open(os.path.join(REPO, "profiles", "ncu_traffic.json")))
         return float(d["dram_bytes_per_launch"][kernel]), d["source"]
@@ -79,24 +81,10 @@ def kernel_record(k, v, B, tot_ms, peaks):
     return r
 
 
-def load_precision():
-    """logit error of the 16-bit operand path vs the fp32 oracle at weight scales 1 / 2 / 3, measured on the GPU box by
-    tools/precision_report.py and committed under profiles/ (bench.py itself must not run the oracle outside the CPU legs)"""
-    try:
-        d = json.load(open(os.path.join(REPO, "profiles", "r02c_precision.json")))
-        return {"source": "profiles/r02c_precision.json (tools/precision_report.py: max-abs logit error vs the fp32 oracle, B=32, t in {0, 42, 99})",
-                "rows": [{k: r[k] for k in ("operand_dtype", "weight_scale", "max_abs_logit", "logit_err_vs_fp32", "logit_err_vs_same_rounding", "fp16_headroom_x", "nonfinite")}
-                         for r in d["rows"]]}
-    except Exception:
-        return None
-
-
 def load_peaks():
-    p = os.path.join(REPO, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(burst=d["bf16_tflops"], sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), hbm=d["hbm_gbs"], src="measured (MEASURED_PEAKS.json)")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    """NVIDIA's H100 SXM data sheet (700 W card): dense 16-bit tensor rate and HBM3 bandwidth.  Upper bounds, not measured
+    here; a card with a lower power limit runs below them (`clocks` in the result line shows what the timed run saw)."""
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, src="H100 SXM data sheet (dense BF16/FP16, 700 W)")
 
 
 class ClockSampler:
@@ -174,12 +162,12 @@ def max_over_ranks(x: float, world, device):
 
 # --------------------------------------------------------------------------------------------------------------
 # Reference arm: the UNMODIFIED reference `LayoutDM.sample` (layoutdm.py:77-88 -> base.py:293-371) from the archive
-# oracle/make_ref.py packaged (oracle/_ref/trainer_ref.zip; /root/reference does not exist on the GPU box), on the host
+# oracle/make_ref.py packaged (oracle/_ref/trainer_ref.zip), on the host
 # cores.  Falls back to the oracle port (kind "port") only if the archive is missing.
 # --------------------------------------------------------------------------------------------------------------
 REF_B, REF_NT = 64, 100      # fixed bounded sample: one step = sample() of 64 layouts through the FULL T=100 loop (no extrapolation in T;
                              # B=64 is the reference's most efficient CPU batch per layout: measured 64 / 256 / 512 -> 1.96 / 1.28 / 1.12
-                             # layouts/s on 8 cores).  ~3.6 s per step on the 64 physical cores of the GPU box (r02b: 17.7 layouts/s)
+                             # layouts/s on 8 cores)
 
 
 def physical_cores(cap=64):
@@ -379,6 +367,10 @@ def run_b200_arm(args, world, rank, local):
     value = total / (ms_step * 1e-3)
     clocks = cs.summary()
     assert int(out.max()) < vocab.mask_id, "MASK token survived the loop"
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "ids.npy"), out.cpu().numpy().astype(np.float64))   # [global batch][S] token ids
 
     # ---- end to end through the host-buffer entry (pinned host buffers, H2D + D2H inside the timed region) ----
     init = torch.full((B, vocab.S), vocab.mask_id, dtype=torch.int64).pin_memory()
@@ -406,7 +398,7 @@ def run_b200_arm(args, world, rank, local):
     traffic, traffic_src = load_traffic(dom) if B == 1024 else (None, None)
     roofline = {"bound": "tensor", "kernel": dom, "achieved": achieved, "peak": peaks["sustained"], "unit": "TFLOP/s",
                 "frac": achieved / peaks["sustained"], "traffic": traffic, "traffic_unit": "bytes/launch", "traffic_source": traffic_src,
-                "algorithmic_flops_per_launch": FLOPS[dom] * B, "peak_source": peaks["src"] + ", sustained bf16 (kernel timed inside a long step)",
+                "algorithmic_flops_per_launch": FLOPS[dom] * B, "peak_source": peaks["src"],
                 "share_of_step": dom_ms / tot_prof,
                 "kernels": {k: kernel_record(k, v, B, tot_prof, peaks) for k, v in prof.items() if v[1]},
                 "hbm_peak_gbs": peaks["hbm"],
@@ -438,9 +430,9 @@ def run_b200_arm(args, world, rank, local):
                 "dtype": args.dtype, "data": "synthetic",
                 "config": {"workload": f"rico25 unconditional, T=100, batch={B} per GPU, N=25 (S=125 tokens, C=155), sampling=random, random-init weights",
                            "global_batch": total, "parallelism": f"dp{world} (batch-sharded replicas, one all-gather of ids)" if world > 1 else "single GPU",
-                           "l2": "per-step activation working set (1.9 GB at B=1024) >> 126 MB L2, no explicit flush needed",
+                           "l2": "per-step activation working set (1.9 GB at B=1024) >> 50 MB L2, no explicit flush needed",
                            "operands": f"{args.dtype} tensor-core operands, fp32 accumulate / LayerNorm / softmax / posterior"},
-                "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "cpu_baseline": cpu, "gpu_eager_baseline": gpu_eager, "configs": configs, "precision": load_precision()}
+                "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "cpu_baseline": cpu, "gpu_eager_baseline": gpu_eager, "configs": configs}
         emit(json.dumps(line))
 
 
@@ -455,6 +447,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the sub-records of BASELINE.json configs 0 / 2 / 3")
     ap.add_argument("--total-batch", type=int, default=0, help="strong scaling: this many layouts in total, split over the ranks")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's output ids to DIR/ids.npy (float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))

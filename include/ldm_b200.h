@@ -1,5 +1,5 @@
 /*
- * ldm_b200 -- C ABI of the B200-native LayoutDM sampling path (discrete-diffusion denoising loop).
+ * ldm_b200 -- C ABI of the H100-native LayoutDM sampling path (discrete-diffusion denoising loop).
  *
  * The reference (CyberAgentAILab/layout-dm) is pure Python: it has NO plugin / FFI boundary.  The seam this
  * library sits behind is the Python class API
@@ -29,7 +29,7 @@ extern "C" {
 #define LDM_OK 0
 #define LDM_ERR_INVALID (-1)      /* bad argument (the Python mirror raises AssertionError / NotImplementedError like the reference) */
 #define LDM_ERR_CUDA (-2)         /* CUDA runtime / driver error */
-#define LDM_ERR_UNSUPPORTED (-3)  /* model shape outside what the sm_100a kernels are built for */
+#define LDM_ERR_UNSUPPORTED (-3)  /* model shape outside what the sm_90a kernels are built for */
 
 typedef struct LdmHandle LdmHandle;
 

@@ -1,4 +1,4 @@
-"""layoutdm_b200 -- B200-native (sm_100a) implementation of LayoutDM's discrete-diffusion sampling loop.
+"""layoutdm_b200 -- H100-native (sm_90a) implementation of LayoutDM's discrete-diffusion sampling loop.
 
 Host-side mirror of the reference's class API (LayoutDM.sample / BaseMaskAndReplaceDiffusion.sample /
 _sample_single_step) on top of the C ABI in include/ldm_b200.h.  See DESIGN.md and INTEGRATION.md."""

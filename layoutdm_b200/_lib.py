@@ -81,7 +81,7 @@ def load() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
-                f"{LIB_PATH} is missing: the sm_100a CUDA library has not been built (run __graft_entry__.build()). "
+                f"{LIB_PATH} is missing: the sm_90a CUDA library has not been built (run __graft_entry__.build()). "
                 "layoutdm_b200 has no CPU or PyTorch fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():

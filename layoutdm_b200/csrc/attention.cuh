@@ -1,4 +1,4 @@
-// Per-(layout, head) self-attention of the LayoutDM denoiser on tcgen05: O = softmax(Q K^T) V, 125 keys, head_dim 58.
+// Per-(layout, head) self-attention of the LayoutDM denoiser on wgmma: O = softmax(Q K^T) V, 125 keys, head_dim 58.
 // (nn.MultiheadAttention inside Block._sa_block, T/models/transformer_utils.py:140-142,191-205; no masks.)
 //
 // Input  qkv [M][1536] 16-bit, per-head column blocks padded 58 -> 64 with zeros:
@@ -7,245 +7,124 @@
 // Output att [M][512] 16-bit, head h in cols [h*64, h*64+64) (col 58 of every head is 1 = the normalised ones column, cols
 //        59..63 are zeros; the out-projection weight is packed with zero columns there) = A operand of the out-projection.
 //
-// Persistent CTAs (two per SM, 320 threads) walk the (layout, head) work items, 128 query rows x 128 keys each, with the
-// Q / K / V tiles double-buffered so the next item's loads are in flight during the current item's math:
-//   warp 0 (one thread) : TMA loads of the Q / K / V head tiles (128B swizzle) two items ahead, and the TMA store of O
-//   warp 1 (one thread) : tcgen05.mma issue:
-//                           S[128x128] = Q K^T      A = Q (K-major), B = K (K-major), 4 MMAs of k=16, fp32 in TMEM cols 0..127
-//                           O[128x64]  = P V        A = P (K-major, written by the softmax warps), B = V as loaded
-//                                                   ([key][d] rows = MN-major operand), 8 MMAs of k=16, TMEM cols 128..191
-//                         S of item i+1 is issued right behind PV of item i.
-//   warps 2..9          : two threads per query row (64 keys each; row max / sum combined through shared memory).  Exact
-//                         softmax from TMEM (max pass, then exp2 / sum in registers), the normalised probabilities are rounded
-//                         to the operand dtype and written as the P operand tile (over the dead Q | K tiles); later O is read
-//                         back from TMEM, packed into the same buffer (P is dead by then) and handed to warp 0 for the store.
+// One CTA per (layout, head) work item, 256 threads = two warpgroups of 64 query rows each; several CTAs per SM overlap
+// one item's loads with another's math.  Thread 0 issues the TMA loads of the Q / K / V head tiles (128 x 64, 128B swizzle).
+//   S[64x128] = Q K^T   wgmma, A = Q rows of the warpgroup, B = K (both K-major, shared memory), fp32 in registers
+//   exact softmax in registers (a row lives in the quad of lanes that shares it); the probabilities stay un-normalised,
+//   are rounded to the operand dtype and become the register A operand of
+//   O[64x64]  = P V     wgmma, B = V as loaded ([key][d] rows = MN-major operand)
+//   O is normalised by its ones column (the row sum of the rounded P) and stored.
 #pragma once
 #include "common.cuh"
 
 namespace ldm {
 
-constexpr int kAttThreads = 320;                    // producer warp + MMA warp + 8 softmax / output warps
+constexpr int kAttThreads = 256;
 constexpr int kAttTile = 128 * 128;                 // one 128 x 64 16-bit tile = 16 KB
-// smem: 2 buffers of Q | K | V (Q | K later overwritten by the 2 k-blocks of P, then Q by the O staging tile) | barriers | stats
-// 96 KB + TMEM 256 columns per CTA; two CTAs (20 warps) per SM
-constexpr int kAttBuf = 3 * kAttTile;
-constexpr int kAttOffQ = 0, kAttOffK = kAttTile, kAttOffP = 0, kAttOffV = 2 * kAttTile, kAttOffO = 0;   // within a buffer
-constexpr int kAttOffBar = 2 * kAttBuf;
-constexpr int kAttOffStat = kAttOffBar + 128;              // float [2 items][2 halves][128 rows] partial row maxima
-constexpr int kAttSmemBytes = kAttOffStat + 2048 + 1024;   // + alignment slack
-constexpr uint32_t kAttTmemCols = 256;              // S: cols 0..127, O: cols 128..191
-
-// MN-major (rows = K index, 64 contiguous 16-bit elements = N) operand tile with 128-byte swizzle, 8-row groups 1024 B apart
-LDM_DEVINL uint64_t make_smem_desc_mn_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;               // LBO: single 64-element atom along N, unused
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;       // SBO: stride between groups of 8 K-rows
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
+constexpr int kAttOffQ = 0, kAttOffK = kAttTile, kAttOffV = 2 * kAttTile, kAttOffBar = 3 * kAttTile;
+constexpr int kAttSmemBytes = kAttOffBar + 64 + 1024;   // + alignment slack
+constexpr int kAttOnesCol = 58;                     // head_dim: V column that holds 1.0
+constexpr int kAttOut = 8 * 64;                     // att row length
 
 template <bool BF16>
 __global__ void __launch_bounds__(kAttThreads, 2)
-attention_kernel(const __grid_constant__ CUtensorMap map_qkv /*[M][1536], box 64 x 128*/,
-                 const __grid_constant__ CUtensorMap map_att /*[M][512], box 64 x 128*/, int n_valid /*125*/, int n_heads /*8*/,
-                 int n_layouts, int ones_col /*58: V column that holds 1.0*/, int rev /*1: walk the items from the last to the first (L2 reuse, see GemmParams::rev)*/,
-                 int store_evict_last /*bit 0: L2 evict_last hint on the O stores (the out-projection reads them next); bit 1: evict_first on the Q / K / V loads (dead afterwards)*/) {
+attention_kernel(const __grid_constant__ CUtensorMap map_qkv /*[M][1536], box 64 x 128*/, void* att /*[M][512]*/,
+                 int n_valid /*125*/, int n_heads /*8*/, int n_layouts,
+                 int rev /*1: walk the items from the last to the first (L2 reuse, see GemmParams::rev)*/) {
   using O = OpT<BF16>;
   extern __shared__ uint8_t att_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kAttOffBar);
-  uint64_t* qkv_full = bars + 0;  // [2] tx: Q + K + V tiles of a buffer
-  uint64_t* s_full = bars + 2;    // commit: S ready (and Q, K smem dead)
-  uint64_t* p_ready = bars + 3;   // 256 arrivals: P tile written, S consumed
-  uint64_t* o_full = bars + 4;    // commit: O ready (and P, V smem dead)
-  uint64_t* o_done = bars + 5;    // 256 arrivals: O read out of TMEM
-  uint64_t* o_staged = bars + 6;  // 256 arrivals: O staging tile written
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 7);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kAttOffBar);
 
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // shuffle: provably warp-uniform (uniform-register control warps)
   const int n_items = n_layouts * n_heads;                     // item = layout * n_heads + head
-  const int step = gridDim.x;
+  const int item = rev ? n_items - 1 - static_cast<int>(blockIdx.x) : static_cast<int>(blockIdx.x);
+  const int h = item % n_heads, row0 = (item / n_heads) * 128;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_qkv);
-    tma_prefetch_desc(&map_att);
-    mbar_init(&qkv_full[0], 1); mbar_init(&qkv_full[1], 1); mbar_init(s_full, 1); mbar_init(o_full, 1);
-    mbar_init(p_ready, 256); mbar_init(o_done, 256); mbar_init(o_staged, 256);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kAttTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t tS = tmem_base, tO = tmem_base + 128;
   pdl_sync();
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(bar, 3 * kAttTile);
+    tma_load_2d(smem + kAttOffQ, &map_qkv, bar, h * 64, row0);
+    tma_load_2d(smem + kAttOffK, &map_qkv, bar, n_heads * 64 + h * 64, row0);
+    tma_load_2d(smem + kAttOffV, &map_qkv, bar, 2 * n_heads * 64 + h * 64, row0);
+  }
+  mbar_wait(bar, 0);
 
-  if (warp == 0) {
-    // ===================== producer: loads two items ahead, stores O (whole warp loops, one elected lane issues) =====================
-    {
-      auto load = [&](int item, int b) {
-        const int pit = rev ? n_items - 1 - item : item;
-        const int h = pit % n_heads, row0 = (pit / n_heads) * 128;
-        uint8_t* buf = smem + b * kAttBuf;
-        mbar_arrive_expect_tx(&qkv_full[b], 3 * kAttTile);
-        if (store_evict_last & 2) {
-          const uint64_t pol = l2_policy_evict_first();
-          tma_load_2d_hint(buf + kAttOffQ, &map_qkv, &qkv_full[b], h * 64, row0, pol);
-          tma_load_2d_hint(buf + kAttOffK, &map_qkv, &qkv_full[b], n_heads * 64 + h * 64, row0, pol);
-          tma_load_2d_hint(buf + kAttOffV, &map_qkv, &qkv_full[b], 2 * n_heads * 64 + h * 64, row0, pol);
-        } else {
-          tma_load_2d(buf + kAttOffQ, &map_qkv, &qkv_full[b], h * 64, row0);
-          tma_load_2d(buf + kAttOffK, &map_qkv, &qkv_full[b], n_heads * 64 + h * 64, row0);
-          tma_load_2d(buf + kAttOffV, &map_qkv, &qkv_full[b], 2 * n_heads * 64 + h * 64, row0);
-        }
-      };
-      const int first = blockIdx.x;
-      if (elect_one()) {
-        if (first < n_items) load(first, 0);
-        if (first + step < n_items) load(first + step, 1);
-      }
-      __syncwarp();
-      int hi = 0;
-      for (int item = first; item < n_items; item += step, ++hi) {
-        const int b = hi & 1;
-        const int pit = rev ? n_items - 1 - item : item;
-        const int h = pit % n_heads, row0 = (pit / n_heads) * 128;
-        mbar_wait(o_staged, hi & 1);
-        if (elect_one()) {
-          if (store_evict_last & 1) tma_store_2d_hint(&map_att, smem_u32(smem + b * kAttBuf + kAttOffO), h * 64, row0, l2_policy_evict_last());
-          else tma_store_2d(&map_att, smem_u32(smem + b * kAttBuf + kAttOffO), h * 64, row0);
-          bulk_commit();
-          if (item + 2 * step < n_items) {
-            bulk_wait_read0();                                   // the store has read the staging tile: the buffer is free
-            load(item + 2 * step, b);
-          }
-        }
-        __syncwarp();
-      }
-      bulk_wait_read0();                                       // the staging tiles have been read; the writes complete with the grid
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    {
-      constexpr uint32_t idesc_s = make_idesc_f16(128, 128, BF16 ? 1 : 0);                 // A, B K-major
-      constexpr uint32_t idesc_o = make_idesc_f16(128, 64, BF16 ? 1 : 0) | (1u << 16);     // B (= V) MN-major
-      int hi = 0;
-      for (int item = blockIdx.x; item < n_items; item += step, ++hi) {
-        const uint32_t ph = hi & 1;
-        const int b = hi & 1;
-        const uint32_t sbuf = smem_u32(smem + b * kAttBuf);
-        // ---- S = Q K^T (S of the previous item was consumed before its p_ready) ----
-        mbar_wait(&qkv_full[b], (hi >> 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da = make_smem_desc_sw128(sbuf + kAttOffQ), db = make_smem_desc_sw128(sbuf + kAttOffK);
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const uint32_t sbase = smem_u32(smem);
+  // ---- S = Q K^T ----
+  float s[64];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tS, da + 2 * k, db + 2 * k, idesc_s, k != 0);
-          umma_commit(s_full);
-        }
-        __syncwarp();
-        // ---- O = P V ----
-        mbar_wait(p_ready, ph);                                  // P written (and S fully read)
-        if (hi > 0) mbar_wait(o_done, (hi - 1) & 1);             // previous O has been read out of TMEM
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da = make_smem_desc_sw128(sbuf + kAttOffP), db = make_smem_desc_mn_sw128(sbuf + kAttOffV);
+  for (int i = 0; i < 64; ++i) s[i] = 0.0f;
+  {
+    const uint64_t da = make_smem_desc_sw128(sbase + kAttOffQ + wg * 64 * 128), db = make_smem_desc_sw128(sbase + kAttOffK);
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 8; ++k)                            // 16 keys per MMA: P advances 32 B inside a k-block / 16 KB
-            umma_f16(tO, da + (k >> 2) * (kAttTile >> 4) + 2 * (k & 3), db + k * (2048 >> 4), idesc_o, k != 0);   // V: 16 rows
-          umma_commit(o_full);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== softmax / output warps: two threads per query row =====================
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;                            // keys [64*half, 64*half + 64) ; output columns [32*half, +32)
-    const int r = quad * 32 + lane;                              // row of the 128-row tile
-    const uint32_t tl = static_cast<uint32_t>(quad * 32) << 16;
-    float* sstat = reinterpret_cast<float*>(smem + kAttOffStat);
-    constexpr float kLog2e = 1.4426950408889634f;
-    int hi = 0;
-    for (int item = blockIdx.x; item < n_items; item += step, ++hi) {
-      const uint32_t ph = hi & 1;
-      const uint32_t sP = smem_u32(smem + (hi & 1) * kAttBuf + kAttOffP), sO = smem_u32(smem + (hi & 1) * kAttBuf + kAttOffO);
-      mbar_wait(s_full, ph);
-      tc_fence_after();
-      // pass 1: maximum over this thread's valid keys (only the last 32-key chunk of the row holds padding keys), combined
-      // with the other half of the row
-      float mx = -INFINITY;
+    for (int k = 0; k < 4; ++k) wgmma_ss_n128<BF16>(s, da + 2 * k, db + 2 * k, k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(s);
+  }
+  // ---- softmax over the valid keys: rows r0 (s[4j], s[4j+1]) and r0 + 8 (s[4j+2], s[4j+3]), keys 8j + 2(lane%4) + {0,1} ----
+  constexpr float kLog2e = 1.4426950408889634f;
+  const int kq = 2 * (lane & 3);
+  float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld<32>(tS + tl + half * 64 + c * 32, v);
-        tmem_wait_ld();
-        if (half == 1 && c == 1) {
+  for (int j = 0; j < 16; ++j) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) if (96 + j < n_valid) mx = fmaxf(mx, __uint_as_float(v[j]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-        }
-      }
-      sstat[(hi & 1) * 256 + half * 128 + r] = mx;
-      named_bar_sync(1, 256);
-      mx = fmaxf(mx, sstat[(hi & 1) * 256 + (half ^ 1) * 128 + r]);
-      // pass 2: e = 2^((s - max) log2 e) in (0, 1], rounded to the operand dtype straight into k-block `half` of the K-major
-      // P tile (128B swizzle).  P stays un-normalised: V carries a column of ones (column `ones_col` of every head, see the
-      // QKV bias packing), so the PV MMA also produces the row sums of the rounded P and O is normalised on the way out.
-      const float mb = mx * kLog2e;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld<32>(tS + tl + half * 64 + c * 32, v);
-        tmem_wait_ld();
-        float e[32];
-        if (half == 1 && c == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) e[j] = (96 + j < n_valid) ? ex2_approx(fmaf(__uint_as_float(v[j]), kLog2e, -mb)) : 0.0f;
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) e[j] = ex2_approx(fmaf(__uint_as_float(v[j]), kLog2e, -mb));
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 pk = make_uint4(O::pack(e[8 * q], e[8 * q + 1]), O::pack(e[8 * q + 2], e[8 * q + 3]),
-                                      O::pack(e[8 * q + 4], e[8 * q + 5]), O::pack(e[8 * q + 6], e[8 * q + 7]));
-          sts_u4(sP + half * kAttTile + r * 128 + (((c * 4 + q) ^ (r & 7)) << 4), pk);
-        }
-      }
-      fence_proxy_async();                                       // generic-proxy writes -> visible to the tensor core
-      tc_fence_before();
-      mbar_arrive(p_ready);
-      // ---- output: this thread's 32 of the 64 head columns ----
-      mbar_wait(o_full, ph);                                     // PV retired: P (and V) of this buffer are dead
-      tc_fence_after();
-      uint32_t o0[32];
-      tmem_ld<32>(tO + tl + half * 32, o0);
-      const uint32_t den = tmem_ld1(tO + tl + ones_col);        // the ones column: row sum of the rounded P
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive(o_done);                                       // TMEM O may be overwritten by the next item
-      const float inv = 1.0f / __uint_as_float(den);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const uint32_t* sv = o0 + 8 * c;
-        const uint4 pk = make_uint4(O::pack(__uint_as_float(sv[0]) * inv, __uint_as_float(sv[1]) * inv), O::pack(__uint_as_float(sv[2]) * inv, __uint_as_float(sv[3]) * inv),
-                                    O::pack(__uint_as_float(sv[4]) * inv, __uint_as_float(sv[5]) * inv), O::pack(__uint_as_float(sv[6]) * inv, __uint_as_float(sv[7]) * inv));
-        sts_u4(sO + r * 128 + (((half * 4 + c) ^ (r & 7)) << 4), pk);
-      }
-      fence_proxy_async();
-      mbar_arrive(o_staged);                                     // warp 0 stores the tile and recycles the buffer
+    for (int e = 0; e < 2; ++e) {
+      if (8 * j + kq + e < n_valid) { mx0 = fmaxf(mx0, s[4 * j + e]); mx1 = fmaxf(mx1, s[4 * j + 2 + e]); }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kAttTmemCols); }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, o));
+  }
+  // e = 2^((s - max) log2 e) in (0, 1], rounded to the operand dtype; V carries a column of ones, so the PV MMA also
+  // produces the row sums of the rounded P and O is normalised on the way out
+  const float mb0 = mx0 * kLog2e, mb1 = mx1 * kLog2e;
+  uint32_t pa[8][4];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    float e[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const bool ok = 8 * j + kq + (q & 1) < n_valid;
+      e[q] = ok ? ex2_approx(fmaf(s[4 * j + q], kLog2e, (q < 2) ? -mb0 : -mb1)) : 0.0f;
+    }
+    // A fragment of k-step j/2: {row r0 keys +0..1, row r0+8 keys +0..1, row r0 keys +8..9, row r0+8 keys +8..9}
+    pa[j >> 1][(j & 1) * 2 + 0] = O::pack(e[0], e[1]);
+    pa[j >> 1][(j & 1) * 2 + 1] = O::pack(e[2], e[3]);
+  }
+  // ---- O = P V ----
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.0f;
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 8; ++k)                                    // 16 keys per MMA: V advances 16 rows = 2 KB
+    wgmma_rs_n64_tb<BF16>(o, pa[k], make_smem_desc_sw128(sbase + kAttOffV + k * 2048), k != 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  fence_acc(o);
+  // the ones column (head dim kAttOnesCol) sits in n8 block kAttOnesCol / 8 of the lane with 2 (lane % 4) = kAttOnesCol % 8
+  constexpr int jd = kAttOnesCol / 8, ld = (kAttOnesCol % 8) / 2, ed = kAttOnesCol % 2;
+  const float inv0 = 1.0f / __shfl_sync(0xffffffffu, o[4 * jd + ed], (lane & ~3) | ld);
+  const float inv1 = 1.0f / __shfl_sync(0xffffffffu, o[4 * jd + 2 + ed], (lane & ~3) | ld);
+  typename O::T* out = static_cast<typename O::T*>(att);
+  const size_t r0 = static_cast<size_t>(row0 + wg * 64 + warp * 16 + (lane >> 2));
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = h * 64 + 8 * j + kq;
+    *reinterpret_cast<uint32_t*>(out + r0 * kAttOut + c) = O::pack(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+    *reinterpret_cast<uint32_t*>(out + (r0 + 8) * kAttOut + c) = O::pack(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+  }
 }
 
 }  // namespace ldm

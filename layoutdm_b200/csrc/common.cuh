@@ -1,5 +1,5 @@
-// Shared device helpers for the LayoutDM sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers, Philox, misc.
-// Everything here is plain inline PTX for sm_100a (B200); no CUTLASS dependency.
+// Shared device helpers for the LayoutDM sm_90a kernels: mbarrier / TMA / wgmma PTX wrappers, Philox, misc.
+// Everything here is plain inline PTX for sm_90a (H100); no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -14,23 +14,13 @@ namespace ldm {
 constexpr float kLogEps = -69.07755278982137f;  // log(1e-30), T/models/categorical_diffusion/util.py:7-8
 
 // ------------------------------------------------------------------------------------------------------------
-// shared-memory addressing, elect
+// shared-memory addressing
 // ------------------------------------------------------------------------------------------------------------
 LDM_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-LDM_DEVINL bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // programmatic dependent launch (every kernel of the step is launched with programmatic stream serialization): the
-// prologue (barrier init, TMEM allocation, descriptor prefetch, parameter loads from constant tables) runs while the
+// prologue (barrier init, descriptor prefetch, parameter loads from constant tables) runs while the
 // previous kernel drains; pdl_wait() returns once the previous grid has completed and its writes are visible.  No global
 // access that depends on (or could overwrite the inputs of) the previous kernel may precede it.
 // ------------------------------------------------------------------------------------------------------------
@@ -45,7 +35,6 @@ LDM_DEVINL void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 LDM_DEVINL void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-LDM_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 LDM_DEVINL void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -64,7 +53,7 @@ LDM_DEVINL bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded spin: a protocol bug must not hang the GPU box (a hang is a strike).  ~2^28 polls >> any legal wait.
+// Bounded spin: a protocol bug traps instead of hanging the GPU.  ~2^28 polls >> any legal wait.
 LDM_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -84,267 +73,120 @@ LDM_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* ba
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-
-// TMA store of a staged tile (shared -> global), tracked by the issuing thread's bulk async-group
-LDM_DEVINL void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
-}
-// L2 eviction-priority hints (experiments, GemmParams::dbg bits 32 / 64 / 128)
-LDM_DEVINL uint64_t l2_policy_evict_first() { uint64_t p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p; }
-LDM_DEVINL uint64_t l2_policy_evict_last() { uint64_t p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p; }
-LDM_DEVINL void tma_store_2d_hint(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1, uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1), "l"(policy) : "memory");
-}
-LDM_DEVINL void tma_load_2d_2cta_hint(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int32_t c0, int32_t c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-LDM_DEVINL void tma_load_2d_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0, int32_t c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-LDM_DEVINL void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-LDM_DEVINL void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // staged sources reusable
-// all but the `pending` most recent bulk groups of this thread have finished reading their shared-memory source
-LDM_DEVINL void bulk_wait_read_pending(int pending) {
-  if (pending <= 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-  else if (pending == 1) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-  else if (pending == 2) asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory");
-  else asm volatile("cp.async.bulk.wait_group.read 3;" ::: "memory");
-}
-LDM_DEVINL void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }          // stores complete
-
-// multicast variant: the tile lands at the same smem offset (and signals the same-offset mbarrier) in every CTA of `mask`
-LDM_DEVINL void tma_load_2d_mc(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0, int32_t c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-// 2-CTA (cta_group::2) flavour: the completion bytes are credited to an mbarrier that may live in the peer CTA
-LDM_DEVINL void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-// shared::cluster address of the same smem offset in CTA `rank` of this cluster
-LDM_DEVINL uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-LDM_DEVINL void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  // default semantics (.release.cta) like CUTLASS ClusterBarrier::arrive: a .release.cluster here costs MEMBAR.ALL.GPU per arrive
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-// no memory ordering: for hand-offs whose data lives in TMEM (ordered by tcgen05.fence), saves the MEMBAR of a release
-LDM_DEVINL void mbar_arrive_cluster_relaxed(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-LDM_DEVINL void mbar_arrive_expect_tx_cluster(uint32_t bar_cluster_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(bar_cluster_addr), "r"(bytes) : "memory");
-}
-LDM_DEVINL uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-LDM_DEVINL void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
+// named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
+LDM_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads/stores, fences
+// wgmma (Hopper warpgroup MMA): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp32 accumulators in registers.
+// Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): n8 block j holds
+//   d[4j + 0], d[4j + 1] = row 16w + l/4,     columns 8j + 2(l%4) + {0, 1}
+//   d[4j + 2], d[4j + 3] = row 16w + l/4 + 8, same columns
 // ------------------------------------------------------------------------------------------------------------
-LDM_DEVINL void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-LDM_DEVINL void tmem_dealloc(uint32_t addr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-LDM_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-LDM_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-LDM_DEVINL void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-LDM_DEVINL void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers fp16 and bf16 operands, fp32 accumulate.
-LDM_DEVINL void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive once all previously issued tcgen05 async ops of this thread are complete
-LDM_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+LDM_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+LDM_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+LDM_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int N>
+LDM_DEVINL void fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// same, arriving on the same-offset mbarrier of every CTA in `mask` (cluster multicast pipelines)
-LDM_DEVINL void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-
-// cta_group::2: one MMA over the CTA pair (M = 256: 128 rows from each CTA's A tile; B's N rows split between the
-// two CTAs' shared memory; each CTA's TMEM receives its own 128 accumulator rows).  Issued by the leader CTA only.
-LDM_DEVINL void umma_f16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-LDM_DEVINL void umma_commit_2cta_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-LDM_DEVINL void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {  // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-LDM_DEVINL void tmem_dealloc_2cta(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand tile stored as rows of 64 x 16-bit (128 B) with the
-// 128-byte swizzle (what TMA SWIZZLE_128B writes): 8-row groups are 1024 B apart (SBO), LBO unused (=1).
-// Bit layout (PTX ISA "tcgen05 shared memory descriptor"): [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4,
-// [46,48) version=1, [61,64) layout type (2 = SWIZZLE_128B).
+// Shared-memory matrix descriptor of a 128-byte-swizzled operand tile (what TMA SWIZZLE_128B writes; tile base 1024-B
+// aligned).  K-major: rows of 64 x 16-bit (128 B), 8-row groups 1024 B apart (SBO); a k-step of 16 advances the start
+// address by 32 B.  MN-major (64 contiguous N elements per 128-B row, one row per K index): 8-K-row groups 1024 B apart.
+// Bit layout (PTX ISA "matrix descriptor" for wgmma): [0,14) addr>>4, [16,30) LBO>>4 (unused here), [32,46) SBO>>4,
+// [62,64) swizzle mode (1 = 128B).
 LDM_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// K-major operand tile whose rows hold only 16 elements (32 B) with the 32-byte swizzle (TMA SWIZZLE_32B):
-// 8-row groups are 256 B apart (SBO), layout type 6 = SWIZZLE_32B.  Used for the K tail of the A-resident block.
-LDM_DEVINL uint64_t make_smem_desc_sw32(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(256 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(6) << 61;
-  return d;
+// both operands from shared memory, both K-major
+// operand lists of the wrappers below: LDM_ACCn = "{%0, ..., %(n-1)}", LDM_OUTn = the matching "+f" constraints
+#define LDM_F(i) "+f"(d[i])
+#define LDM_ACC128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define LDM_OUT128 LDM_F(0), LDM_F(1), LDM_F(2), LDM_F(3), LDM_F(4), LDM_F(5), LDM_F(6), LDM_F(7), LDM_F(8), LDM_F(9), LDM_F(10), LDM_F(11), LDM_F(12), LDM_F(13), LDM_F(14), LDM_F(15), LDM_F(16), LDM_F(17), LDM_F(18), LDM_F(19), LDM_F(20), LDM_F(21), LDM_F(22), LDM_F(23), LDM_F(24), LDM_F(25), LDM_F(26), LDM_F(27), LDM_F(28), LDM_F(29), LDM_F(30), LDM_F(31), LDM_F(32), LDM_F(33), LDM_F(34), LDM_F(35), LDM_F(36), LDM_F(37), LDM_F(38), LDM_F(39), LDM_F(40), LDM_F(41), LDM_F(42), LDM_F(43), LDM_F(44), LDM_F(45), LDM_F(46), LDM_F(47), LDM_F(48), LDM_F(49), LDM_F(50), LDM_F(51), LDM_F(52), LDM_F(53), LDM_F(54), LDM_F(55), LDM_F(56), LDM_F(57), LDM_F(58), LDM_F(59), LDM_F(60), LDM_F(61), LDM_F(62), LDM_F(63), LDM_F(64), LDM_F(65), LDM_F(66), LDM_F(67), LDM_F(68), LDM_F(69), LDM_F(70), LDM_F(71), LDM_F(72), LDM_F(73), LDM_F(74), LDM_F(75), LDM_F(76), LDM_F(77), LDM_F(78), LDM_F(79), LDM_F(80), LDM_F(81), LDM_F(82), LDM_F(83), LDM_F(84), LDM_F(85), LDM_F(86), LDM_F(87), LDM_F(88), LDM_F(89), LDM_F(90), LDM_F(91), LDM_F(92), LDM_F(93), LDM_F(94), LDM_F(95), LDM_F(96), LDM_F(97), LDM_F(98), LDM_F(99), LDM_F(100), LDM_F(101), LDM_F(102), LDM_F(103), LDM_F(104), LDM_F(105), LDM_F(106), LDM_F(107), LDM_F(108), LDM_F(109), LDM_F(110), LDM_F(111), LDM_F(112), LDM_F(113), LDM_F(114), LDM_F(115), LDM_F(116), LDM_F(117), LDM_F(118), LDM_F(119), LDM_F(120), LDM_F(121), LDM_F(122), LDM_F(123), LDM_F(124), LDM_F(125), LDM_F(126), LDM_F(127)
+#define LDM_ACC116 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115}"
+#define LDM_OUT116 LDM_F(0), LDM_F(1), LDM_F(2), LDM_F(3), LDM_F(4), LDM_F(5), LDM_F(6), LDM_F(7), LDM_F(8), LDM_F(9), LDM_F(10), LDM_F(11), LDM_F(12), LDM_F(13), LDM_F(14), LDM_F(15), LDM_F(16), LDM_F(17), LDM_F(18), LDM_F(19), LDM_F(20), LDM_F(21), LDM_F(22), LDM_F(23), LDM_F(24), LDM_F(25), LDM_F(26), LDM_F(27), LDM_F(28), LDM_F(29), LDM_F(30), LDM_F(31), LDM_F(32), LDM_F(33), LDM_F(34), LDM_F(35), LDM_F(36), LDM_F(37), LDM_F(38), LDM_F(39), LDM_F(40), LDM_F(41), LDM_F(42), LDM_F(43), LDM_F(44), LDM_F(45), LDM_F(46), LDM_F(47), LDM_F(48), LDM_F(49), LDM_F(50), LDM_F(51), LDM_F(52), LDM_F(53), LDM_F(54), LDM_F(55), LDM_F(56), LDM_F(57), LDM_F(58), LDM_F(59), LDM_F(60), LDM_F(61), LDM_F(62), LDM_F(63), LDM_F(64), LDM_F(65), LDM_F(66), LDM_F(67), LDM_F(68), LDM_F(69), LDM_F(70), LDM_F(71), LDM_F(72), LDM_F(73), LDM_F(74), LDM_F(75), LDM_F(76), LDM_F(77), LDM_F(78), LDM_F(79), LDM_F(80), LDM_F(81), LDM_F(82), LDM_F(83), LDM_F(84), LDM_F(85), LDM_F(86), LDM_F(87), LDM_F(88), LDM_F(89), LDM_F(90), LDM_F(91), LDM_F(92), LDM_F(93), LDM_F(94), LDM_F(95), LDM_F(96), LDM_F(97), LDM_F(98), LDM_F(99), LDM_F(100), LDM_F(101), LDM_F(102), LDM_F(103), LDM_F(104), LDM_F(105), LDM_F(106), LDM_F(107), LDM_F(108), LDM_F(109), LDM_F(110), LDM_F(111), LDM_F(112), LDM_F(113), LDM_F(114), LDM_F(115)
+#define LDM_ACC80 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}"
+#define LDM_OUT80 LDM_F(0), LDM_F(1), LDM_F(2), LDM_F(3), LDM_F(4), LDM_F(5), LDM_F(6), LDM_F(7), LDM_F(8), LDM_F(9), LDM_F(10), LDM_F(11), LDM_F(12), LDM_F(13), LDM_F(14), LDM_F(15), LDM_F(16), LDM_F(17), LDM_F(18), LDM_F(19), LDM_F(20), LDM_F(21), LDM_F(22), LDM_F(23), LDM_F(24), LDM_F(25), LDM_F(26), LDM_F(27), LDM_F(28), LDM_F(29), LDM_F(30), LDM_F(31), LDM_F(32), LDM_F(33), LDM_F(34), LDM_F(35), LDM_F(36), LDM_F(37), LDM_F(38), LDM_F(39), LDM_F(40), LDM_F(41), LDM_F(42), LDM_F(43), LDM_F(44), LDM_F(45), LDM_F(46), LDM_F(47), LDM_F(48), LDM_F(49), LDM_F(50), LDM_F(51), LDM_F(52), LDM_F(53), LDM_F(54), LDM_F(55), LDM_F(56), LDM_F(57), LDM_F(58), LDM_F(59), LDM_F(60), LDM_F(61), LDM_F(62), LDM_F(63), LDM_F(64), LDM_F(65), LDM_F(66), LDM_F(67), LDM_F(68), LDM_F(69), LDM_F(70), LDM_F(71), LDM_F(72), LDM_F(73), LDM_F(74), LDM_F(75), LDM_F(76), LDM_F(77), LDM_F(78), LDM_F(79)
+#define LDM_ACC64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define LDM_OUT64 LDM_F(0), LDM_F(1), LDM_F(2), LDM_F(3), LDM_F(4), LDM_F(5), LDM_F(6), LDM_F(7), LDM_F(8), LDM_F(9), LDM_F(10), LDM_F(11), LDM_F(12), LDM_F(13), LDM_F(14), LDM_F(15), LDM_F(16), LDM_F(17), LDM_F(18), LDM_F(19), LDM_F(20), LDM_F(21), LDM_F(22), LDM_F(23), LDM_F(24), LDM_F(25), LDM_F(26), LDM_F(27), LDM_F(28), LDM_F(29), LDM_F(30), LDM_F(31), LDM_F(32), LDM_F(33), LDM_F(34), LDM_F(35), LDM_F(36), LDM_F(37), LDM_F(38), LDM_F(39), LDM_F(40), LDM_F(41), LDM_F(42), LDM_F(43), LDM_F(44), LDM_F(45), LDM_F(46), LDM_F(47), LDM_F(48), LDM_F(49), LDM_F(50), LDM_F(51), LDM_F(52), LDM_F(53), LDM_F(54), LDM_F(55), LDM_F(56), LDM_F(57), LDM_F(58), LDM_F(59), LDM_F(60), LDM_F(61), LDM_F(62), LDM_F(63)
+#define LDM_ACC32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define LDM_OUT32 LDM_F(0), LDM_F(1), LDM_F(2), LDM_F(3), LDM_F(4), LDM_F(5), LDM_F(6), LDM_F(7), LDM_F(8), LDM_F(9), LDM_F(10), LDM_F(11), LDM_F(12), LDM_F(13), LDM_F(14), LDM_F(15), LDM_F(16), LDM_F(17), LDM_F(18), LDM_F(19), LDM_F(20), LDM_F(21), LDM_F(22), LDM_F(23), LDM_F(24), LDM_F(25), LDM_F(26), LDM_F(27), LDM_F(28), LDM_F(29), LDM_F(30), LDM_F(31)
+template <bool BF16>
+LDM_DEVINL void wgmma_ss_n256(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " LDM_ACC128 ", %128, %129, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT128 : "l"(da), "l"(db), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " LDM_ACC128 ", %128, %129, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT128 : "l"(da), "l"(db), "r"(accumulate));
 }
-
-// Instruction descriptor for kind::f16: D=f32, A/B = f16 (0) or bf16 (1), both K-major, M x N.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int ab_format) {
-  return (1u << 4) | (static_cast<uint32_t>(ab_format) << 7) | (static_cast<uint32_t>(ab_format) << 10) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+template <bool BF16>
+LDM_DEVINL void wgmma_ss_n232(float (&d)[116], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %118, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n232k16.f32.bf16.bf16 " LDM_ACC116 ", %116, %117, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT116 : "l"(da), "l"(db), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %118, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n232k16.f32.f16.f16 " LDM_ACC116 ", %116, %117, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT116 : "l"(da), "l"(db), "r"(accumulate));
 }
-
-// TMEM -> registers: this warp's 32 lanes x N consecutive 32-bit columns (thread i gets lane i's row).
-LDM_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+template <bool BF16>
+LDM_DEVINL void wgmma_ss_n160(float (&d)[80], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 " LDM_ACC80 ", %80, %81, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT80 : "l"(da), "l"(db), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 " LDM_ACC80 ", %80, %81, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT80 : "l"(da), "l"(db), "r"(accumulate));
 }
-LDM_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+template <bool BF16>
+LDM_DEVINL void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " LDM_ACC64 ", %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT64 : "l"(da), "l"(db), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " LDM_ACC64 ", %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+                 : LDM_OUT64 : "l"(da), "l"(db), "r"(accumulate));
 }
-LDM_DEVINL void tmem_ld8(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
+// A from registers (four 16-bit pairs per thread, accumulator fragment order), B MN-major (transposed) from shared memory
+template <bool BF16>
+LDM_DEVINL void wgmma_rs_n64_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  if constexpr (BF16)
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " LDM_ACC32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+                 : LDM_OUT32 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+  else
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " LDM_ACC32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+                 : LDM_OUT32 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
-LDM_DEVINL uint32_t tmem_ld1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-// load `n` (8, 16 or 32; compile-time after unrolling) columns
-template <int N>
-LDM_DEVINL void tmem_ld(uint32_t taddr, uint32_t (&r)[32]) {
-  static_assert(N == 8 || N == 16 || N == 32, "unsupported tcgen05.ld width");
-  if constexpr (N == 32) tmem_ld32(taddr, r);
-  else if constexpr (N == 16) tmem_ld16(taddr, r);
-  else tmem_ld8(taddr, r);
-}
-// registers -> TMEM
-LDM_DEVINL void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-LDM_DEVINL void tmem_st16(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-LDM_DEVINL void tmem_st8(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-      : "memory");
-}
-template <int N>
-LDM_DEVINL void tmem_st(uint32_t taddr, const uint32_t (&r)[32]) {
-  static_assert(N == 8 || N == 16 || N == 32, "unsupported tcgen05.st width");
-  if constexpr (N == 32) tmem_st32(taddr, r);
-  else if constexpr (N == 16) tmem_st16(taddr, r);
-  else tmem_st8(taddr, r);
-}
-// named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
-// global-memory flag hand-off between co-resident CTAs
-LDM_DEVINL void st_release_gpu_u32(unsigned* p, unsigned v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-LDM_DEVINL unsigned ld_acquire_gpu_u32(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-// 8-byte {fp32 payload, 32-bit epoch} words: payload and flag travel in one single-copy-atomic access (no fences needed)
-LDM_DEVINL void st_ll_word(unsigned long long* p, float v, unsigned epoch) {
-  const unsigned long long w = (static_cast<unsigned long long>(epoch) << 32) | __float_as_uint(v);
-  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
-}
-LDM_DEVINL unsigned long long ld_ll_word(const unsigned long long* p) {
-  unsigned long long w;
-  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(w) : "l"(p) : "memory");
-  return w;
-}
-LDM_DEVINL float2 ld_cg_f2(const float2* p) {
-  float2 v;
-  asm volatile("ld.global.cg.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p) : "memory");
-  return v;
-}
-LDM_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+#undef LDM_ACC128
+#undef LDM_OUT128
+#undef LDM_ACC116
+#undef LDM_OUT116
+#undef LDM_ACC80
+#undef LDM_OUT80
+#undef LDM_ACC64
+#undef LDM_OUT64
+#undef LDM_ACC32
+#undef LDM_OUT32
+#undef LDM_F
 
 // ------------------------------------------------------------------------------------------------------------
 // operand dtype helpers (fp16 or bf16 tensor-core operands; accumulation is always fp32)
@@ -383,22 +225,6 @@ LDM_DEVINL float ex2_approx(float x) {
 }
 
 LDM_DEVINL float u01_from_bits(uint32_t w) { return (static_cast<float>(w >> 9) + 0.5f) * 1.1920928955078125e-07f; }
-
-// explicit shared-space vector accesses (keeps them on the LDS/STS pipe; pointer arithmetic on the dynamic-smem base
-// otherwise degrades to generic LD/ST, which queue behind global traffic)
-LDM_DEVINL float4 lds_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-LDM_DEVINL uint4 lds_u4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-LDM_DEVINL void sts_u4(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 
 LDM_DEVINL float warp_max(float v) {
 #pragma unroll

@@ -1,553 +1,238 @@
-// tcgen05 (5th-gen tensor core) GEMMs of the LayoutDM denoiser, C[M,N] = A[M,K] * W[N,K]^T (+ fused epilogue).
+// wgmma (Hopper warpgroup MMA) GEMMs of the LayoutDM denoiser, C[M,N] = A[M,K] * W[N,K]^T (+ fused epilogue).
 //
-//   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 * n_layouts (one 128-row tile = one layout)
+//   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 * n_layouts (one 128-row block = one layout)
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
 //
-// One kernel template, launched as thread-block clusters of 2 CTAs (cta_group::2), 320 threads per CTA:
-//   warp 0     : TMA producer  (cp.async.bulk.tensor 2-D tiles, 128-byte swizzle, mbarrier complete_tx); the warp loops
-//                warp-uniformly and one elected lane issues
-//   warp 1     : TMEM allocation; in the leader CTA it issues tcgen05.mma for the pair (fp32 accumulators in TMEM, two
-//                accumulators so the epilogue of tile i overlaps the main loop of tile i+1); warp-uniform loop, elected lane
-//   warps 2..9 : epilogue; warp w owns TMEM lanes 32*(w%4)..+31 (thread = one output row) and one half of the tile's
-//                columns.  All global traffic of the epilogue goes through TMA: every warp stages 32 x 32 blocks in
-//                its own swizzled shared-memory buffers (conflict-free 16-byte accesses along its rows) and a single
-//                lane issues the tensor store / load.  A 1-CTA/SM kernel with ~220 KB of smem has no L1 and only
-//                8 epilogue warps: per-thread global loads/stores made the epilogue 3-10x slower than the MMAs (profiles
-//                r01a..r01i).
-//
-// Operand feed:  ARES (QKV, FF1; K = 464): the CTA's 128 x K activation block is resident (7 k-block tiles + a 32B-swizzled
-//                16-column tail), loaded once per row block, and only weight half-tiles stream through the ring;
-//                otherwise (out-projection, FF2, head) A tile + weight half-tile per stage.
-// Epilogues:  QKV (bias, q-scale, 16-bit) | FF1 (bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
-//             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused; work unit =
-//                  (row block, column tile) with the row statistics exchanged between neighbouring CTA pairs -- see the
-//                  comment at the LN branch).
+// One kernel template, one output tile per CTA, 288 threads:
+//   warps 0..7 : two consumer warpgroups.  Each issues m64 x BN_WG x k16 wgmmas from the shared-memory ring (fp32
+//                accumulators in registers) and runs the epilogue on its own accumulator fragment.
+//   warp 8     : TMA producer (one lane): cp.async.bulk.tensor 2-D tiles with the 128-byte swizzle into a STAGES-deep
+//                ring, completion on mbarriers (full: TMA bytes landed, empty: both warpgroups' MMAs have read the stage).
+// Tile shapes:
+//   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (QKV, FF1: 256 columns; vocabulary head: 160)
+//   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the LN epilogue: 2 x 232 = 464 =
+//              d_model, so a CTA holds whole rows and the LayerNorm row statistics are combined in shared memory.
+// Epilogues:  QKV (bias, q-scale, 16-bit) | RELU (FF1: bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
+//             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused).
 //
 // Reference ops replaced: nn.Linear / nn.MultiheadAttention projections / nn.LayerNorm / AdaLayerNorm in
 // T/models/transformer_utils.py:79-83,165-210 and T/models/common/nn_lib.py:187-189,235.
 #pragma once
-#include <type_traits>
-
 #include "common.cuh"
 
 namespace ldm {
 
-constexpr int kBM = 128;       // rows per M tile (= one layout: 125 tokens + 3 pad rows)
+constexpr int kBM = 128;       // rows of one layout tile (125 tokens + 3 pad rows)
 constexpr int kBK = 64;        // K elements per smem stage (= 128 B = one swizzle row)
-constexpr int kUmmaK = 16;     // K per tcgen05.mma (16-bit operands)
-constexpr int kGemmThreads = 320;
-constexpr int kEpiThreads = 256;   // warps 2..9
-constexpr int kATileBytes = kBM * kBK * 2;   // 16 KB
+constexpr int kWgK = 16;       // K per wgmma (16-bit operands)
+constexpr int kGemmThreads = 288;
+constexpr int kGemmConsumers = 256;
 
 enum : int { EPI_QKV = 0, EPI_RELU = 1, EPI_F32 = 2, EPI_LN = 3 };
 
 struct GemmParams {
-  int M, N, K;            // M multiple of 256; N = n_tiles * BN_STORE, or (non-LN) a narrower last tile: N % BN_STORE a multiple of 32
+  int M, N, K;            // M multiple of the tile rows; N <= n_tiles * tile columns (columns past N are computed on zero weights, not stored)
   int n_tiles;
   const float* bias;      // [N] or nullptr
-  void* out;              // output tensor (informational: every store goes through the tensor maps)
+  void* out;              // [M][ldo] 16-bit (EPI_F32: fp32)
   int ldo;
   float qscale;           // EPI_QKV: columns < qcols are scaled by qscale after the bias
   int qcols;
-  // EPI_LN (N = 464 = column tiles of 224 + 240): y = acc + bias + resid ; out = LayerNorm(y) * gamma + beta  (gamma = 1 + scale_t for AdaLN)
+  // EPI_LN (N = 464): y = acc + bias + resid ; out = LayerNorm(y) * gamma + beta  (gamma = 1 + scale_t for AdaLN)
   const float* resid;     // fp32 [M][N] residual stream
   float* y_out;           // fp32 [M][N] pre-norm sum (the next residual) or nullptr
   const float* ln_scale;  // [N]
   const float* ln_shift;  // [N]
   int adaln;
   float* out32;           // fp32 [M][N] normalised output (next residual, AdaLN case) or nullptr
-  // EPI_LN row statistics exchanged between the two CTA pairs that hold the two column tiles of a row block
-  unsigned long long* ln_stats;   // [n_units * 2 CTAs][128 rows][2] {fp32 partial, launch epoch} words: sum and sum of squares over a unit's columns
-  unsigned ln_epoch;
   const int* t_layout;    // EPI_LN + adaln: per-layout timesteps (training-side calls): ln_scale then points at the layer's whole [T][2N]
-  int n_layouts;          //   AdaLN table and every (row block, CTA) = layout reloads its (scale, shift) row; nullptr: one timestep for all
-  int store_evict_last;   // 1: the epilogue's TMA stores carry an L2 evict_last hint (QKV / FF1: the freshly written qkv16 / hid16 rows stay in L2 for the
-                          // consumer that -- with alternating sweep directions -- reads them first; measured FF1 198 -> 187 us, QKV 160 -> 156, attention 95 -> 92)
-  int load_evict_first;   // bit 0: the A operand tiles, bit 1: the LN residual blocks are loaded with an L2 evict_first hint (read once, dead afterwards);
-                          // bit 2: the weight tiles are loaded with an evict_last hint
-  int rev;                // 1: walk the row blocks from the last to the first.  Consecutive kernels alternate the direction, so a consumer starts with
-                          // the rows its producer wrote last -- the part of the intermediate that is still in the 126 MB L2
-  int tile_sched;         // 1: spread single (row block, N tile) tiles over the CTA pairs (small batches); 0: a pair walks all N tiles of a row block
-  int dbg;                // bring-up probe (env LDM_GEMM_DEBUG), bit mask: 1 = skip the MMAs, 2 = skip the TMA operand loads, 4 = skip the epilogue body,
-                          // 8 = every epilogue store is issued out of bounds (the TMA engine reads the staging tile but writes nothing),
-                          // 16 = every epilogue store lands in the first 8192 rows (an L2-resident window: no HBM write stream); results are garbage.
-                          // L2 eviction-priority experiments (results stay correct): 32 = epilogue stores evict_first, 128 = epilogue stores evict_last,
-                          // 64 = weight tiles evict_last
+  int n_layouts;          //   AdaLN table and every layout reloads its (scale, shift) row; nullptr: one timestep for all
+  int rev;                // 1: walk the row blocks from the last to the first.  Consecutive kernels alternate the direction, so a consumer starts
+                          // with the rows its producer wrote last -- the part of the intermediate that is still in L2
 };
 
-#ifndef LDM_ARES_STORE_BUFS
-#define LDM_ARES_STORE_BUFS 1      // 2: two alternating store blocks per epilogue warp at the price of one weight stage -- measured SLOWER
-#endif                             // (QKV 158 -> 176 us, FF1 196 -> 221 us): the stores do not wait on their staging block, they slow the operand loads
-constexpr int kAResSlots = 8;   // A-resident mode: K <= 512, the row block's whole A operand (8 k-blocks) stays in smem
-
-// ARES: the 128 x K activation block of the CTA is loaded ONCE per row block and reused by all N tiles; only the weight
-// half-tiles stream through the ring (the K=464 GEMMs are bound by the bytes each SM pulls out of L2: -42 %).
-template <int UMMA_N, int STAGES, int EPI, bool ARES = false>
+template <int BN_WG, int WG_M, int STAGES>
 struct GemmSmem {
-  static constexpr int kBHalfBytes = (UMMA_N / 2) * kBK * 2;     // each CTA of the pair holds half of the weight tile
-  static constexpr int kStageBytes = ARES ? kBHalfBytes : kATileBytes + kBHalfBytes;
-  // the K = 464 block = 7 full k-blocks + a 16-column tail, kept as a 128 x 32 B tile (32-byte swizzle, its own tensor map)
-  static constexpr int kATailBytes = kBM * kUmmaK * 2;
-  static constexpr int kAResBytes = ARES ? (kAResSlots - 1) * kATileBytes + kATailBytes : 0;
-  static_assert(kBHalfBytes % 1024 == 0, "half weight tile must keep 1024-B (swizzle atom) alignment");
-  // per-epilogue-warp staging: [0,4K) 32x32 fp32 store block (128B swizzle) / 16-bit store block (64B swizzle);
-  // LN: [4K,6K) 16-bit store block, [6K,10K) residual load block (128B swizzle)
-  // LN with a short ring (out-projection, K = 512): the spare shared memory holds a second private residual block [10K,14K)
-  static constexpr bool kLnExtraBuf = EPI == EPI_LN && STAGES <= 3;
-  // LN with a long ring (FF2, K = 1856): compact staging, the 16-bit store block [4K,6K) shares the residual block [4K,8K)
-  static constexpr bool kLnCompact = EPI == EPI_LN && STAGES >= 5;
-  // plain 16-bit epilogues (ARES: QKV / FF1): kStoreBufs alternating 2 KB store blocks per warp (experiment, see LDM_ARES_STORE_BUFS)
-  static constexpr int kStoreBufs = (EPI != EPI_LN && ARES) ? LDM_ARES_STORE_BUFS : 1;
-  static constexpr int kWarpStage = EPI == EPI_LN ? (kLnExtraBuf ? 14336 : (kLnCompact ? 8192 : 10240)) : (ARES ? 2048 * kStoreBufs : 4096);
-  static constexpr int kStagingBytes = 8 * kWarpStage;
-  static constexpr int kBarBytes = 512;
-  // bias vector of the layer; LN: bias / gamma / beta of the CTA's own column tile (a pair keeps its tile), 256 floats each
-  static constexpr int kBiasBytes = EPI == EPI_LN ? 3 * 256 * 4 : 1856 * 4;
-  static constexpr int kStatBytes = EPI == EPI_LN ? 4 * kBM * 8 : 0;  // LN: per-row (sum, sumsq) partials of the two column halves, per accumulator
-  static constexpr int kOffRing = kAResBytes;                      // [A-resident slots][ring stages]...
-  static constexpr int kOffStaging = kOffRing + STAGES * kStageBytes;
-  static constexpr int kOffBars = kOffStaging + kStagingBytes;
-  static constexpr int kOffBias = kOffBars + kBarBytes;
-  static constexpr int kOffStat = kOffBias + kBiasBytes;
-  static constexpr int kBytes = kOffStat + kStatBytes + (kLnCompact ? 0 : 1024) /*align slack; compact: the base must be 1024-aligned (checked)*/;
+  static constexpr int kWgN = 3 - WG_M;                          // warpgroups along N
+  static constexpr int kABytes = 64 * WG_M * kBK * 2;
+  static constexpr int kBBytes = BN_WG * kBK * 2;                // one warpgroup's weight rows
+  static constexpr int kStageBytes = kABytes + kWgN * kBBytes;
+  static_assert(kBBytes % 1024 == 0, "weight block must keep 1024-B (swizzle atom) alignment");
+  static constexpr int kOffBars = STAGES * kStageBytes;
+  static constexpr int kOffStat = kOffBars + 256;                // LN: per-row (sum, sumsq) of each warpgroup's columns
+  static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
+  static_assert(2 * STAGES * 8 <= 256, "barrier block overflow");
   static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
 };
 
-// CTA pairs (thread-block cluster of 2, cta_group::2): the pair computes a 256 x UMMA_N tile per step with ONE
-// tcgen05.mma issued by the leader CTA (rank 0): A = 128 rows from each CTA's own smem, B = UMMA_N/2 weight rows from each
-// CTA's smem, D = 128 accumulator rows in each CTA's TMEM.  A pair walks all N tiles of its 256-row block back to back
-// (A tiles stay L2-hot, and the LN epilogue sees complete rows).
-template <int BN_STORE, int UMMA_N, int STAGES, int EPI, bool BF16, bool ARES = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_out,     // main output: 32x32 blocks (16-bit: 64B swizzle, fp32: 128B swizzle)
-               const __grid_constant__ CUtensorMap map_resid,   // LN: fp32 residual (load)
-               const __grid_constant__ CUtensorMap map_yout,    // LN: fp32 pre-norm sum (store) when p.y_out
-               const __grid_constant__ CUtensorMap map_out32,   // LN: fp32 normalised output (store) when p.out32; ARES: the A operand's K tail (16 x 128 box, 32B swizzle)
+template <bool BF16, int N>
+LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 256) wgmma_ss_n256<BF16>(d, da, db, accumulate);
+  else if constexpr (N == 232) wgmma_ss_n232<BF16>(d, da, db, accumulate);
+  else if constexpr (N == 160) wgmma_ss_n160<BF16>(d, da, db, accumulate);
+  else { static_assert(N == 128, "unsupported wgmma width"); wgmma_ss_n128<BF16>(d, da, db, accumulate); }
+}
+
+// grid: (n_tiles, M / (64 WG_M))
+template <int BN_WG, int WG_M, int STAGES, int EPI, bool BF16>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows*/, const __grid_constant__ CUtensorMap map_b /*box 64 x BN_WG rows*/,
                const GemmParams p) {
-  using SM = GemmSmem<UMMA_N, STAGES, EPI, ARES>;
+  using SM = GemmSmem<BN_WG, WG_M, STAGES>;
   using O = OpT<BF16>;
-  static_assert(!ARES || EPI == EPI_QKV || EPI == EPI_RELU, "A-resident mode: 16-bit plain epilogues only");
-  static_assert(UMMA_N % 16 == 0 && UMMA_N <= 256 && BN_STORE <= UMMA_N, "invalid UMMA shape");
-  constexpr int kAccStride = 256;            // TMEM columns between the two accumulators
-  constexpr uint32_t kTmemCols = 512;
-  constexpr int kFull = BN_STORE / 32;
-  constexpr int kSplit = (kFull + 1) / 2;    // half 0: 32-col chunks [0, kSplit), half 1: [kSplit, kFull)
-  static_assert(BN_STORE % 32 == 0, "tile widths are whole 32-column chunks (every chunk leaves through TMA)");
-  static_assert(EPI != EPI_LN || (BN_STORE == 224 && UMMA_N == 240), "LN epilogue is laid out for 464 = 224 + 240 columns");
-  static_assert(EPI == EPI_LN || BN_STORE == UMMA_N, "plain epilogues store whole UMMA tiles");
+  constexpr int kBMt = 64 * WG_M, kAcc = BN_WG / 2;
+  static_assert(EPI != EPI_LN || (WG_M == 1 && BN_WG == 232), "LN epilogue is laid out for 464 = 2 x 232 columns");
+  static_assert(EPI == EPI_LN || WG_M == 2, "plain epilogues use 128-row tiles");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
-  uint64_t* full = bars;                     // leader's copy is the live one: 2 producer arrivals + both CTAs' TMA bytes
-  uint64_t* empty = bars + STAGES;           // per CTA: released by the leader's multicast tcgen05.commit
-  uint64_t* tfull = bars + 2 * STAGES;       // per CTA: accumulator ready (multicast commit)
-  uint64_t* tempty = bars + 2 * STAGES + 2;  // leader's copy: 16 warp arrivals (8 epilogue warps x 2 CTAs)
-  uint64_t* lbars = bars + 2 * STAGES + 4;   // LN: two residual-load barriers per epilogue warp
-  uint64_t* afull = bars + 2 * STAGES + 20;  // ARES: leader's copy live (A k-block of this row block landed in both CTAs)
-  uint64_t* aempty = afull + kAResSlots;     // ARES: per CTA, the last N tile's MMAs are done with the A k-block
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 20 + 2 * kAResSlots);
-  float* sbias = reinterpret_cast<float*>(smem + SM::kOffBias);
-  static_assert((2 * STAGES + 20 + 2 * kAResSlots) * 8 + 4 <= SM::kBarBytes, "barrier block overflow");
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
+  uint64_t* empty = full + STAGES;
 
-  // warp index through a shuffle: the compiler then knows it is warp-uniform and keeps the producer / MMA loops (addresses,
-  // descriptors, barrier phases) in uniform registers -- with a per-lane index every tcgen05.mma paid ~25 instructions of
-  // R2UR.BROADCAST / ELECT glue and the tensor pipe idled half the time (profiles r01q)
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int num_kb = (p.K + kBK - 1) / kBK;
-  const uint32_t cta_rank = cluster_ctarank();               // 0 = leader
-  const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-  const int n_super = p.M / (2 * kBM);                       // 256-row blocks
-  // work units per pair: whole row blocks (inner loop over the N tiles) or, for small batches, single tiles
-  const int n_outer = p.tile_sched ? n_super * p.n_tiles : n_super, n_inner = p.tile_sched ? 1 : p.n_tiles;
-  if constexpr (EPI == EPI_LN) {
-    if (SM::kLnCompact && (smem_u32(smem_raw) & 1023u) != 0) { if (threadIdx.x == 0) printf("dynamic shared memory base is not 1024-byte aligned\n"); __trap(); }
-    // units o = pair + k * n_pairs with an even pair count: this pair always works on column tile (pair & 1)
-    const int tile0 = (pair & 1) * BN_STORE;
-    for (int i = threadIdx.x; i < 256; i += kGemmThreads) {
-      const int c = tile0 + i;
-      const bool ok = c < p.N;
-      sbias[i] = (ok && p.bias != nullptr) ? __ldg(p.bias + c) : 0.0f;
-      if (p.t_layout != nullptr) continue;                     // per-layout AdaLN rows are loaded per unit in the epilogue
-      sbias[256 + i] = ok ? __ldg(p.ln_scale + c) + (p.adaln ? 1.0f : 0.0f) : 0.0f;
-      sbias[512 + i] = ok ? __ldg(p.ln_shift + c) : 0.0f;
-    }
-  } else {
-    for (int i = threadIdx.x; i < p.N; i += kGemmThreads) sbias[i] = p.bias != nullptr ? __ldg(p.bias + i) : 0.0f;
-  }
+  const int n_mblk = p.M / kBMt;
+  const int m_blk = p.rev ? n_mblk - 1 - static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.y);
+  const int m0 = m_blk * kBMt, n0 = static_cast<int>(blockIdx.x) * BN_WG * SM::kWgN;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kGemmConsumers) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    tma_prefetch_desc(&map_out);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 2); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 16); }
-    for (int i = 0; i < 16; ++i) mbar_init(&lbars[i], 1);
-    for (int i = 0; i < kAResSlots; ++i) { mbar_init(&afull[i], 2); mbar_init(&aempty[i], 1); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc_2cta(tmem_ptr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                                        // both CTAs' barriers and TMEM are ready
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_sync();                                                // everything above overlapped the previous kernel's tail
 
-  if (warp == 0) {
-    // ===================== TMA producer (whole warp loops, one elected lane issues) =====================
-    {
-      int stage = 0; uint32_t phase = 0, a_phase = 0;
-      for (int o = pair; o < n_outer; o += n_pairs) {
-      for (int i = 0; i < n_inner; ++i) {
-        const int sup0 = p.tile_sched ? o / p.n_tiles : o, n_blk = p.tile_sched ? o % p.n_tiles : i;
-        const int sup = p.rev ? n_super - 1 - sup0 : sup0;
-        const int m_blk = 2 * sup + static_cast<int>(cta_rank);
-        // weight rows per CTA (the TMA box stays UMMA_N / 2 rows: rows past b_half are unused)
-        const int b_half = (EPI == EPI_LN ? (n_blk == 0 ? BN_STORE : UMMA_N) : min(UMMA_N, p.N - n_blk * BN_STORE)) / 2;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          if constexpr (ARES) {
-            if (i == 0) {                                      // this row block's A k-block: loaded once, reused by every N tile
-              mbar_wait(&aempty[kb], a_phase ^ 1);
-              const uint32_t lead_afull = mapa_shared(smem_u32(&afull[kb]), 0);
-              if (elect_one()) {
-                if (p.dbg & 2) { mbar_arrive_cluster(lead_afull); }
-                else {
-                  const bool tail = (kb == num_kb - 1) && (p.K & (kBK - 1)) != 0;   // K % 64 == 16 (checked by the host)
-                  mbar_arrive_expect_tx_cluster(lead_afull, tail ? SM::kATailBytes : kATileBytes);
-                  if (p.load_evict_first & 1) tma_load_2d_2cta_hint(smem + kb * kATileBytes, tail ? &map_out32 : &map_a, lead_afull, kb * kBK, m_blk * kBM, l2_policy_evict_first());
-                  else tma_load_2d_2cta(smem + kb * kATileBytes, tail ? &map_out32 : &map_a, lead_afull, kb * kBK, m_blk * kBM);
-                }
-              }
-              __syncwarp();
-            }
-          }
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sa = smem + SM::kOffRing + stage * SM::kStageBytes;
-          const uint32_t lead_full = mapa_shared(smem_u32(&full[stage]), 0);
-          if (elect_one()) {
-            if (p.dbg & 2) { mbar_arrive_cluster(lead_full); }
-            else {
-              mbar_arrive_expect_tx_cluster(lead_full, SM::kStageBytes);
-              if constexpr (!ARES) {
-                if (p.load_evict_first & 1) tma_load_2d_2cta_hint(sa, &map_a, lead_full, kb * kBK, m_blk * kBM, l2_policy_evict_first());
-                else if (p.load_evict_first & 8) tma_load_2d_2cta_hint(sa, &map_a, lead_full, kb * kBK, m_blk * kBM, l2_policy_evict_last());   // read again by the partner pair
-                else tma_load_2d_2cta(sa, &map_a, lead_full, kb * kBK, m_blk * kBM);
-              }
-              if ((p.dbg & 64) || (p.load_evict_first & 4)) tma_load_2d_2cta_hint(sa + (ARES ? 0 : kATileBytes), &map_b, lead_full, kb * kBK, n_blk * BN_STORE + static_cast<int>(cta_rank) * b_half, l2_policy_evict_last());
-              else tma_load_2d_2cta(sa + (ARES ? 0 : kATileBytes), &map_b, lead_full, kb * kBK, n_blk * BN_STORE + static_cast<int>(cta_rank) * b_half);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-      a_phase ^= 1;
+  if (warp == kGemmConsumers / 32) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
+        uint8_t* st = smem + s * SM::kStageBytes;
+        mbar_arrive_expect_tx(&full[s], SM::kStageBytes);    // out-of-bounds box parts are zero-filled and still counted
+        tma_load_2d(st, &map_a, &full[s], kb * kBK, m0);
+#pragma unroll
+        for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b, &full[s], kb * kBK, n0 + wn * BN_WG);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp 1 of the leader CTA loops, one elected lane issues) =====================
-    if (cta_rank == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(2 * kBM, UMMA_N, BF16 ? 1 : 0);
-      int stage = 0; uint32_t phase = 0, a_phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int o = pair; o < n_outer; o += n_pairs) {
-      for (int i = 0; i < n_inner; ++i) {
-        const int n_blk_mma = p.tile_sched ? o % p.n_tiles : i;
-        const int nw = EPI == EPI_LN ? (n_blk_mma == 0 ? BN_STORE : UMMA_N) : min(UMMA_N, p.N - n_blk_mma * BN_STORE);   // last tile may be narrower
-        const uint32_t idesc_t = nw == UMMA_N ? idesc : make_idesc_f16(2 * kBM, nw, BF16 ? 1 : 0);
-        mbar_wait(&tempty[acc], acc_phase ^ 1);              // both CTAs drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * kAccStride;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          if constexpr (ARES) { if (i == 0) mbar_wait(&afull[kb], a_phase); }   // this row block's A k-block is in place
-          mbar_wait(&full[stage], phase);                    // both CTAs' operand tiles have landed
-          tc_fence_after();
-          const uint32_t sr = smem_u32(smem + SM::kOffRing + stage * SM::kStageBytes);
-          const bool a_tail = ARES && (kb == num_kb - 1) && (p.K & (kBK - 1)) != 0;
-          const uint64_t da = a_tail ? make_smem_desc_sw32(smem_u32(smem + kb * kATileBytes))
-                                     : make_smem_desc_sw128(ARES ? smem_u32(smem + kb * kATileBytes) : sr);
-          const uint64_t db = make_smem_desc_sw128(ARES ? sr : sr + kATileBytes);
-          const int nk = min(kBK, p.K - kb * kBK) / kUmmaK;     // K tail: TMA zero-fills, skip the zero k-steps
-          if (elect_one()) {
-            if (!(p.dbg & 1)) {
-              if (nk == kBK / kUmmaK) {
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int wm = WG_M == 2 ? wg : 0, wn = WG_M == 2 ? 0 : wg;
+  float acc[kAcc];
 #pragma unroll
-                for (int k = 0; k < kBK / kUmmaK; ++k)
-                  umma_f16_2cta(tmem_d, da + 2 * k, db + 2 * k, idesc_t, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
-              } else {
-                for (int k = 0; k < nk; ++k) umma_f16_2cta(tmem_d, da + 2 * k, db + 2 * k, idesc_t, (kb | k) != 0);
-              }
-            }
-            umma_commit_2cta_mc(&empty[stage], static_cast<uint16_t>(0b11));       // free the stage in both CTAs
-            if constexpr (ARES) { if (i == n_inner - 1) umma_commit_2cta_mc(&aempty[kb], static_cast<uint16_t>(0b11)); }
-            if (kb == num_kb - 1) umma_commit_2cta_mc(&tfull[acc], static_cast<uint16_t>(0b11));   // accumulator ready in both CTAs
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+  for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    mbar_wait(&full[s], (kb / STAGES) & 1);
+    const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
+    const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
+    const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
+    wgmma_fence();
+    if (kb * kBK + kBK <= p.K) {
+#pragma unroll
+      for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
+    } else {                                                // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
+      wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
+    }
+    wgmma_commit();
+    // keep this k-block's MMAs in flight; once the previous k-block's have retired its stage goes back to the producer
+    if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[(kb - 1) % STAGES]); }
+  }
+  wgmma_wait<0>();
+  fence_acc(acc);
+
+  const int rw = (warp & 3) * 16 + (lane >> 2);             // fragment rows rw and rw + 8 of the warpgroup's 64
+  const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
+  const int col0 = n0 + wn * BN_WG + 2 * (lane & 3);        // + 8 j: columns col, col + 1 of n8 block j
+
+  if constexpr (EPI != EPI_LN) {
+    float scale = 1.0f;
+    if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
+      const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
+      float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if constexpr (EPI == EPI_QKV) v[e] *= scale;
+        if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
       }
-      a_phase ^= 1;
+      if constexpr (EPI == EPI_F32) {
+        float* o = static_cast<float*>(p.out);
+        *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
+        *reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * p.ldo + c) = make_float2(v[2], v[3]);
+      } else {
+        uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
+        uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
+        *o0 = O::pack(v[0], v[1]);
+        *o1 = O::pack(v[2], v[3]);
       }
     }
   } else {
-    // ===================== epilogue warps =====================
-    const int we = warp - 2;                   // 0..7
-    const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int half = we >> 2;                  // which half of the tile's columns
-    const int row_in_tile = quad * 32 + lane;
-    const uint32_t sbias_addr = smem_u32(sbias);
-    const uint32_t wbuf = smem_u32(smem + SM::kOffStaging) + we * SM::kWarpStage;
-    const uint32_t s32 = wbuf;                                              // fp32 store block, rows of 128 B
-    const uint32_t s16 = EPI == EPI_LN ? wbuf + 4096 : wbuf;                // 16-bit store block, rows of 64 B
-    const int c_begin = half == 0 ? 0 : kSplit, c_end = half == 0 ? kSplit : kFull;
-    const uint32_t tlane = static_cast<uint32_t>(quad * 32) << 16;
-
-    // stage one 32 x 32 block (this warp's rows, 32 columns) and hand it to the TMA engine
-    const int st_or = (p.dbg & 8) ? 0x40000000 : 0, st_and = (p.dbg & 16) ? 8191 : 0x7fffffff;   // store-stream probes (see GemmParams::dbg)
-    // Staging blocks are recycled per block, not per warp: every TMA store is its own bulk group, groups retire in order, so before a
-    // block is rewritten only the groups up to its previous store have to have left shared memory -- the newer ones stay in flight.
-    const bool st_hint16 = (p.dbg & (32 | 128)) != 0 || (p.store_evict_last & 1) != 0;     // bit 0: 16-bit stores, bit 1: fp32 stores
-    const bool st_hint32 = (p.dbg & (32 | 128)) != 0 || (p.store_evict_last & 2) != 0;
-    const uint64_t st_policy = (p.dbg & 32) ? l2_policy_evict_first() : l2_policy_evict_last();
-    int n_groups = 0, last_g16[2] = {-1000, -1000}, last_g32 = -1000;
-    uint32_t buf16 = 0;                        // which of the kStoreBufs 16-bit blocks the next store uses
-    // stage one 32 x 32 block (this warp's rows, 32 columns) and hand it to the TMA engine
-    auto store_f32 = [&](const CUtensorMap* m, const float* v, int col, int row0) {
-      row0 = (row0 & st_and) | st_or;
-      if (lane == 0) bulk_wait_read_pending(n_groups - 1 - last_g32);
-      __syncwarp();
+    // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
+    //   y = acc + bias + resid (-> y_out), row statistics over the thread's columns, the quad of lanes that shares a row,
+    //   then the other warpgroup (other 232 columns) through shared memory; normalise, 16-bit (+ fp32) outputs.
+    float2* sstat = reinterpret_cast<float2*>(smem + SM::kOffStat);
+    const int N = p.N;
+    float s0 = 0.0f, q0 = 0.0f, s1 = 0.0f, q1 = 0.0f;
+    const float* r0p = p.resid + static_cast<size_t>(row0) * N;
+    const float* r1p = p.resid + static_cast<size_t>(row1) * N;
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        sts_u4(s32 + lane * 128 + ((j ^ (lane & 7)) << 4),
-               make_uint4(__float_as_uint(v[4 * j]), __float_as_uint(v[4 * j + 1]), __float_as_uint(v[4 * j + 2]), __float_as_uint(v[4 * j + 3])));
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) { if (st_hint32) tma_store_2d_hint(m, s32, col, row0, st_policy); else tma_store_2d(m, s32, col, row0); bulk_commit(); }
-      last_g32 = n_groups++;
-    };
-    auto store_16 = [&](const CUtensorMap* m, const float* v, int col, int row0) {
-      row0 = (row0 & st_and) | st_or;
-      const uint32_t sb = s16 + (SM::kStoreBufs > 1 ? buf16 * 2048u : 0u);
-      if (lane == 0) bulk_wait_read_pending(n_groups - 1 - last_g16[buf16]);
-      __syncwarp();
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        sts_u4(sb + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4),
-               make_uint4(O::pack(v[8 * c], v[8 * c + 1]), O::pack(v[8 * c + 2], v[8 * c + 3]),
-                          O::pack(v[8 * c + 4], v[8 * c + 5]), O::pack(v[8 * c + 6], v[8 * c + 7])));
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) { if (st_hint16) tma_store_2d_hint(m, sb, col, row0, st_policy); else tma_store_2d(m, sb, col, row0); bulk_commit(); }
-      last_g16[buf16] = n_groups++;
-      if (SM::kStoreBufs > 1) buf16 ^= 1u;
-    };
-
-    int acc = 0; uint32_t acc_phase = 0;
-    if constexpr (EPI != EPI_LN) {
-      for (int o = pair; o < n_outer; o += n_pairs)
-      for (int i = 0; i < n_inner; ++i) {
-        const int sup0 = p.tile_sched ? o / p.n_tiles : o, n_blk = p.tile_sched ? o % p.n_tiles : i;
-        const int sup = p.rev ? n_super - 1 - sup0 : sup0;
-        const int m_blk = 2 * sup + static_cast<int>(cta_rank);
-        const int n0 = n_blk * BN_STORE;
-        const int wrow0 = m_blk * kBM + quad * 32;
-        float tile_scale = 1.0f;
-        if constexpr (EPI == EPI_QKV) tile_scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + tlane + acc * kAccStride;
-        int cb = c_begin, ce = c_end;
-        if (n0 + BN_STORE > p.N) {                   // narrower last tile: split its 32-column chunks over the two halves
-          const int nc = (p.N - n0) / 32;
-          cb = half == 0 ? 0 : nc / 2; ce = half == 0 ? nc / 2 : nc;
-        }
-        if (p.dbg & 4) ce = cb;
-#pragma unroll 1
-        for (int c = cb; c < ce; ++c) {
-          const int c0 = c * 32;
-          uint32_t r[32];
-          tmem_ld<32>(taddr + c0, r);
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {            // LDS broadcast reads overlap the TMEM load
-            const float4 b4 = lds_f4(sbias_addr + (n0 + c0 + 4 * j) * 4);
-            v[4 * j] = b4.x; v[4 * j + 1] = b4.y; v[4 * j + 2] = b4.z; v[4 * j + 3] = b4.w;
-          }
-          tmem_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float x = __uint_as_float(r[j]) + v[j];
-            if constexpr (EPI == EPI_QKV) x *= tile_scale;
-            if constexpr (EPI == EPI_RELU) x = fmaxf(x, 0.0f);
-            v[j] = x;
-          }
-          if constexpr (EPI == EPI_F32) store_f32(&map_out, v, n0 + c0, wrow0);
-          else store_16(&map_out, v, n0 + c0, wrow0);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster_relaxed(mapa_shared(smem_u32(&tempty[acc]), 0));   // leader's barrier: 8 warps x 2 CTAs
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    } else {
-      // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
-      // Work unit = (256-row block, column tile): tile 0 = columns [0, 224), tile 1 = [224, 464).  The two tiles of a row
-      // block run at the same time on two neighbouring CTA pairs (units o and o ^ 1; the launch keeps every pair resident
-      // and the pair count even), so a CTA holds 128 rows x <= 240 accumulator columns, the accumulators are double
-      // buffered and this epilogue overlaps the MMAs of the pair's next unit.  LayerNorm needs whole rows: each CTA
-      // publishes per-row (sum, sum of squares) partials of its tile through global memory and picks up its partner's.
-      //   phase A  y = acc + bias + resid -> back into TMEM (+ y_out), row partials
-      //   exchange with the partner CTA (same rows, other tile)
-      //   phase B  normalise from TMEM, 16-bit (+ fp32) outputs; release the accumulator
-      // Every 32-column chunk goes through TMA (the last chunk of tile 1 covers columns 448..479: the TMA load zero-fills
-      // and the TMA stores clip the 16 columns past N, the statistics mask them).
-      float2* sstat = reinterpret_cast<float2*>(smem + SM::kOffStat);
-      const uint32_t sgamma_addr = sbias_addr + 256 * 4, sbeta_addr = sbias_addr + 512 * 4;   // indexed by the column within the tile
-      // residual blocks (rows of 128 B, 128B swizzle): buffer 0 is private; without a y_out stream (FF2) the fp32 store
-      // staging block is idle during phase A and serves as a second buffer, i.e. the loads run two chunks ahead
-      const int n_lbuf = (SM::kLnExtraBuf || p.y_out == nullptr) ? 2 : 1;
-      const uint32_t lbuf_off[2] = {SM::kLnCompact ? 4096u : 6144u, SM::kLnExtraBuf ? 10240u : 0u};
-      uint8_t* const wbuf_ptr = smem + SM::kOffStaging + we * SM::kWarpStage;
-      uint64_t* lbar = &lbars[2 * we];
-      uint32_t lphase = 0;                                   // one phase bit per buffer
-      const float inv_n = 1.0f / static_cast<float>(p.N);
-      for (int o = pair; o < n_outer; o += n_pairs) {
-        const int sup = p.rev ? n_super - 1 - (o >> 1) : (o >> 1), n_blk = o & 1;
-        const int m_blk = 2 * sup + static_cast<int>(cta_rank);
-        const int wrow0 = m_blk * kBM + quad * 32;            // first row of this warp
-        const int n0 = n_blk * BN_STORE;
-        const int ce = (p.dbg & 4) ? c_begin : (half == 0 ? kSplit : kFull + n_blk);   // tile 1 has one more (half-valid) chunk
-        const uint32_t taddr = tmem_base + tlane + acc * kAccStride;
-        float sum = 0.0f, sq = 0.0f;
-        if (p.t_layout != nullptr) {
-          // per-layout timesteps: this CTA's layout (= its 128-row block) picks its own AdaLN (scale, shift) row.  Phase B of the
-          // previous unit must be through with gamma / beta before they are replaced; phase A does not read them and the
-          // statistics barrier below orders the new values before phase B.
-          named_bar_sync(1, kEpiThreads);
-          const int tl = m_blk < p.n_layouts ? __ldg(p.t_layout + m_blk) : 0;
-          const float* tab = p.ln_scale + static_cast<size_t>(tl) * 2 * p.N;
-          const int i = static_cast<int>(threadIdx.x) - 64, c = n0 + i;
-          const bool ok = c < p.N;
-          sbias[256 + i] = ok ? __ldg(tab + c) + 1.0f : 0.0f;
-          sbias[512 + i] = ok ? __ldg(tab + p.N + c) : 0.0f;
-        }
-        // ---------------- phase A ----------------
-        {
-          auto issue_resid = [&](int c) {                     // async: 32 rows x 32 fp32 of the residual -> buffer (c - c_begin) % n_lbuf
-            if (lane == 0 && c < ce) {
-              const int b = (c - c_begin) % n_lbuf;
-              mbar_arrive_expect_tx(&lbar[b], 4096);
-              if (p.load_evict_first & 2) tma_load_2d_hint(wbuf_ptr + lbuf_off[b], &map_resid, &lbar[b], n0 + c * 32, wrow0, l2_policy_evict_first());
-              else tma_load_2d(wbuf_ptr + lbuf_off[b], &map_resid, &lbar[b], n0 + c * 32, wrow0);
-            }
-          };
-          if ((SM::kLnCompact || (!SM::kLnExtraBuf && n_lbuf == 2)) && lane == 0) bulk_wait_read0();   // the previous unit's stores have left the staging blocks the loads reuse
-          for (int c = c_begin; c < c_begin + n_lbuf; ++c) issue_resid(c);   // in flight while the MMAs of this unit still run
-          mbar_wait(&tfull[acc], acc_phase);
-          tc_fence_after();
-#pragma unroll 1
-          for (int c = c_begin; c < ce; ++c) {
-            const int c0 = c * 32;
-            const int n_ok = p.N - (n0 + c0);                 // >= 32 except for the last chunk of the row (16)
-            uint32_t r[32];
-            tmem_ld<32>(taddr + c0, r);
-            const int lb = (c - c_begin) % n_lbuf;
-            mbar_wait(&lbar[lb], (lphase >> lb) & 1); lphase ^= 1u << lb;   // residual block has landed
-            const uint32_t lbuf = wbuf + lbuf_off[lb];
-            float y[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 rs = lds_f4(lbuf + lane * 128 + ((j ^ (lane & 7)) << 4));
-              const float4 b4 = lds_f4(sbias_addr + (c0 + 4 * j) * 4);
-              y[4 * j] = rs.x + b4.x; y[4 * j + 1] = rs.y + b4.y; y[4 * j + 2] = rs.z + b4.z; y[4 * j + 3] = rs.w + b4.w;
-            }
-            __syncwarp();                                     // every lane is done reading lbuf
-            issue_resid(c + n_lbuf);                          // refill this buffer: streams in during the math / stores below
-            tmem_wait_ld();
-            if (n_ok >= 32) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                y[j] += __uint_as_float(r[j]);
-                sum += y[j];
-                sq = fmaf(y[j], y[j], sq);
-                r[j] = __float_as_uint(y[j]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                y[j] = j < n_ok ? y[j] + __uint_as_float(r[j]) : 0.0f;
-                sum += y[j];
-                sq = fmaf(y[j], y[j], sq);
-                r[j] = __float_as_uint(y[j]);
-              }
-            }
-            tmem_st<32>(taddr + c0, r);
-            if (p.y_out != nullptr) store_f32(&map_yout, y, n0 + c0, wrow0);
-          }
-        }
-        // ---------------- row statistics: the two column halves of this CTA, then the partner's tile ----------------
-        sstat[(acc * 2 + half) * kBM + row_in_tile] = make_float2(sum, sq);
-        tmem_wait_st();
-        named_bar_sync(1, kEpiThreads);
-        const float2 other = sstat[(acc * 2 + (half ^ 1)) * kBM + row_in_tile];
-        sum += other.x; sq += other.y;
-        // {value, epoch} words: row r of CTA slot s lives at ln_stats[(s * 128 + r) * 2 + {0: sum, 1: sum of squares}]
-        unsigned long long* my_w = p.ln_stats + ((static_cast<size_t>(o) * 2 + cta_rank) * kBM + row_in_tile) * 2;
-        const unsigned long long* peer_w = p.ln_stats + ((static_cast<size_t>(o ^ 1) * 2 + cta_rank) * kBM + row_in_tile) * 2;
-        if (half == 0) { st_ll_word(my_w, sum, p.ln_epoch); st_ll_word(my_w + 1, sq, p.ln_epoch); }
-        float2 peer;
-        {
-          unsigned long long w0, w1;
-          uint32_t spins = 0;
-          do {
-            if (spins) __nanosleep(64);                        // the partner is a few hundred ns behind at most: poll gently
-            w0 = ld_ll_word(peer_w); w1 = ld_ll_word(peer_w + 1);
-            if (++spins > (1u << 24)) { printf("LN statistics exchange timed out (unit %d)\n", o); __trap(); }
-          } while (static_cast<unsigned>(w0 >> 32) != p.ln_epoch || static_cast<unsigned>(w1 >> 32) != p.ln_epoch);
-          peer = make_float2(__uint_as_float(static_cast<unsigned>(w0)), __uint_as_float(static_cast<unsigned>(w1)));
-        }
-        const float mean = (sum + peer.x) * inv_n;
-        const float var = fmaxf((sq + peer.y) * inv_n - mean * mean, 0.0f);
-        const float rstd = 1.0f / sqrtf(var + 1e-5f);
-        // ---------------- phase B ----------------
-        {
-          auto norm4 = [&](const uint32_t* rr4, int col, float* ov) {
-            const float4 g4 = lds_f4(sgamma_addr + col * 4), h4 = lds_f4(sbeta_addr + col * 4);
-            ov[0] = (__uint_as_float(rr4[0]) - mean) * rstd * g4.x + h4.x;
-            ov[1] = (__uint_as_float(rr4[1]) - mean) * rstd * g4.y + h4.y;
-            ov[2] = (__uint_as_float(rr4[2]) - mean) * rstd * g4.z + h4.z;
-            ov[3] = (__uint_as_float(rr4[3]) - mean) * rstd * g4.w + h4.w;
-          };
-#pragma unroll 1
-          for (int c = c_begin; c < ce; ++c) {
-            const int c0 = c * 32;
-            uint32_t r[32];
-            tmem_ld<32>(taddr + c0, r);
-            tmem_wait_ld();
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) norm4(r + 4 * j, c0 + 4 * j, v + 4 * j);
-            store_16(&map_out, v, n0 + c0, wrow0);
-            if (p.out32 != nullptr) store_f32(&map_out32, v, n0 + c0, wrow0);
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster_relaxed(mapa_shared(smem_u32(&tempty[acc]), 0));   // release this accumulator
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
+      acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
+      acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
+      s0 += acc[4 * j] + acc[4 * j + 1]; q0 = fmaf(acc[4 * j], acc[4 * j], fmaf(acc[4 * j + 1], acc[4 * j + 1], q0));
+      s1 += acc[4 * j + 2] + acc[4 * j + 3]; q1 = fmaf(acc[4 * j + 2], acc[4 * j + 2], fmaf(acc[4 * j + 3], acc[4 * j + 3], q1));
+      if (p.y_out != nullptr) {
+        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
     }
-    if (lane == 0) bulk_wait_read0();          // this warp's TMA stores have read their staging blocks before the CTA retires (the writes
-                                               // themselves complete with the grid: a dependent kernel's griddepcontrol.wait covers them)
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o); q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+    }
+    if ((lane & 3) == 0) { sstat[wn * 64 + rw] = make_float2(s0, q0); sstat[wn * 64 + rw + 8] = make_float2(s1, q1); }
+    named_bar_sync(1, kGemmConsumers);
+    const float2 o0 = sstat[(wn ^ 1) * 64 + rw], o1 = sstat[(wn ^ 1) * 64 + rw + 8];
+    const float inv_n = 1.0f / static_cast<float>(N);
+    const float mean0 = (s0 + o0.x) * inv_n, mean1 = (s1 + o1.x) * inv_n;
+    const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + o0.y) * inv_n - mean0 * mean0, 0.0f) + 1e-5f);
+    const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + o1.y) * inv_n - mean1 * mean1, 0.0f) + 1e-5f);
+    const float* gam = p.ln_scale;
+    const float* bet = p.ln_shift;
+    float gadd = p.adaln ? 1.0f : 0.0f;
+    if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
+      const int layout = m0 / kBM;
+      const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
+      gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
+    }
+    typename O::T* out16 = static_cast<typename O::T*>(p.out);
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      const float2 g = __ldg(reinterpret_cast<const float2*>(gam + c)), h = __ldg(reinterpret_cast<const float2*>(bet + c));
+      const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + gadd) + h.y;
+      const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + gadd) + h.y;
+      *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
+      *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
+      if (p.out32 != nullptr) {
+        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
+        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);
+      }
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                        // nobody exits while the peer may still arrive here / read our smem
-  if (warp == 1) { tc_fence_after(); tmem_dealloc_2cta(tmem_base, kTmemCols); }
 }
 
 }  // namespace ldm

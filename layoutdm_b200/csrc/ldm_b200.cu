@@ -39,10 +39,20 @@ constexpr int kMaxLayers = 16;
 constexpr int kHeadPad = 64;        // per-head width after padding 58 -> 64
 constexpr int kQkvN = 3 * 8 * kHeadPad;   // 1536
 constexpr int kAttN = 8 * kHeadPad;        // 512: attention output, heads padded like Q/K/V
+constexpr int kMaxLayouts = 32767;  // layouts per call
 constexpr int kLogitLd = 160;       // padded logits row (C <= 160)
 constexpr int kDModel = 464;        // the kernels are laid out for the paper's backbone: d = 464 (LN tiles 224 + 240), ff = 4 d
-// A-resident GEMMs (QKV, FF1): weight-ring depth.  Two alternating store blocks per epilogue warp cost the shared memory of one stage.
-constexpr int kAresStages = LDM_ARES_STORE_BUFS >= 2 ? 4 : 5;
+// GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, bf16>
+constexpr int kPlainBN = 256, kPlainStages = 4;   // QKV / FF1: 128 x 256 tiles
+constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
+constexpr int kLnBN = 232, kLnStages = 3;         // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue)
+template <bool BF16> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_QKV, BF16>;
+template <bool BF16> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_RELU, BF16>;
+template <bool BF16> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, BF16>;
+template <bool BF16> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, BF16>;
+constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages>::kBytes;
+constexpr int kHeadSmem = GemmSmem<kHeadBN, 2, kHeadStages>::kBytes;
+constexpr int kLnSmem = GemmSmem<kLnBN, 1, kLnStages>::kBytes;
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -59,7 +69,7 @@ int load_encode() {
   return LDM_OK;
 }
 
-// 2-D row-major [rows][cols] 16-bit tensor, box = box_rows x 64 columns, 128-byte swizzle, zero OOB fill.
+// 2-D row-major [rows][cols] 16-bit tensor, box = box_rows x 64 columns, 128-byte swizzle, zero OOB fill (TMA operand loads).
 int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16) {
   const cuuint64_t dims[2] = {cols, rows};
   const cuuint64_t strides[1] = {cols * 2};
@@ -70,37 +80,6 @@ int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uin
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu box_rows=%u", (int)r,
                                      (unsigned long long)rows, (unsigned long long)cols, box_rows);
-  return LDM_OK;
-}
-
-// 32 x 32-element block of a row-major [rows][cols] tensor as the GEMM epilogue stages it: 16-bit -> 64-byte rows
-// (64B swizzle), fp32 -> 128-byte rows (128B swizzle)
-int make_block_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, int elem_bytes, bool bf16) {
-  const cuuint64_t dims[2] = {cols, rows};
-  const cuuint64_t strides[1] = {cols * elem_bytes};
-  const cuuint32_t box[2] = {32, 32};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                                 : (bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
-  CUresult r = g_encode(m, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        elem_bytes == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled (block map) failed (%d) rows=%llu cols=%llu", (int)r,
-                                     (unsigned long long)rows, (unsigned long long)cols);
-  return LDM_OK;
-}
-
-// K tail of an activation operand for the A-resident GEMMs: 16 columns x 128 rows starting at any column, 32-byte swizzle
-int make_tail_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, bool bf16) {
-  const cuuint64_t dims[2] = {cols, rows};
-  const cuuint64_t strides[1] = {cols * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kUmmaK), static_cast<cuuint32_t>(kBM)};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims,
-                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled (tail map) failed (%d) rows=%llu cols=%llu", (int)r,
-                                     (unsigned long long)rows, (unsigned long long)cols);
   return LDM_OK;
 }
 
@@ -129,11 +108,9 @@ struct LdmHandle {
   LdmModelDesc desc;
   int C = 0, S = 0, L = 0, T = 0, G = 0;
   bool bf16 = false;
-  int num_sms = 148;
   int64_t launches = 0;
-  int gemm_dbg = 0;           // env LDM_GEMM_DEBUG (bring-up probe, see GemmParams::dbg)
   int debug_generic_posterior = 0;   // env LDM_GENERIC_POSTERIOR=1: always take the all-classes posterior / sampling kernel (tests)
-  int pdl = 1;                // env LDM_PDL=0: no programmatic dependent launch (LN GEMMs launched cooperatively instead)
+  int pdl = 1;                // env LDM_PDL=0: no programmatic dependent launch
   int debug_stop_after = 0;   // test tap: stop the denoiser after this many launches (0 = run everything)
   bool prof = false;          // per-kernel CUDA-event timing (ldm_profile_begin/end)
   struct ProfRec { int cat; cudaEvent_t a, b; };
@@ -149,19 +126,16 @@ struct LdmHandle {
   void *x16 = nullptr, *qkv16 = nullptr, *att16 = nullptr, *z16 = nullptr, *hid16 = nullptr;
   float *x32 = nullptr, *y32 = nullptr, *logits = nullptr;
   float* rel_lp = nullptr;      // [cap][S][C] log-probabilities between the posterior and the draw (cond = relation)
-  unsigned long long* ln_stats = nullptr; unsigned ln_epoch = 0;   // LN statistics exchange between CTA pairs (gemm_tc.cuh)
   long long* ids[2] = {nullptr, nullptr};
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
-  CUtensorMap m_x16, m_att16, m_z16, m_hid16, m_qkv16;                       // A operands (128 x 64 boxes)
-  CUtensorMap t_x16, t_z16;                                                  // K tails of the A-resident operands (128 x 16 boxes)
-  CUtensorMap b_qkv16, b_hid16, b_z16, b_x16, b_x32, b_y32, b_logits;  // epilogue 32 x 32 blocks
+  CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
+  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
   std::vector<void*> owned;
   // CUDA graph of the whole T-step loop (ldm_sample_loop): captured once per (batch, plan, sampling, conditioning kind) and
   // replayed; everything that changes from call to call lives in device memory (noise key block, staged cond / start ids)
   int use_graph = 1;           // env LDM_GRAPH=0: plain stream launches
   int sweep = 1;               // env LDM_SWEEP=0: every kernel walks its row blocks in ascending order (no alternating directions)
-  int l2_hint = 1;             // env LDM_L2_HINT bit mask: L2 evict_last hint on the 16-bit stores of 1 = QKV / FF1, 2 = attention, 4 = out-projection (z16), 8 = FF2 (x16 / z16); evict_first hint on loads of data that is dead afterwards: 16 = A operands of QKV / FF1 / out-projection, 32 = fp32 residual blocks, 64 = attention's Q / K / V; 128 = evict_last on the weight tiles; 0 = none
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
@@ -259,20 +233,15 @@ struct ProfScope {   // counts the launch; when profiling is on, brackets it wit
 
 // Launch of one kernel of the step.  Default: programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization):
 // the kernel's CTAs may start while the previous kernel of the stream drains; every kernel calls pdl_sync() (griddepcontrol.wait
-// + launch_dependents) after its prologue and before its first dependent global access, so barrier init / TMEM allocation /
-// descriptor prefetch / parameter loads overlap the predecessor's tail and the launch latency disappears.
-// The LN GEMMs exchange row statistics between neighbouring CTA pairs while both run, i.e. all their CTAs must be resident
-// together.  With PDL that holds by construction: the grid has at most one CTA per SM (checked at create), its predecessor
-// never waits on it, and its successor cannot start before every CTA of it has passed pdl_sync().  With LDM_PDL=0 the LN GEMMs
-// are launched cooperatively instead (the runtime then guarantees co-residency or fails the launch).
+// + launch_dependents) after its prologue and before its first dependent global access, so barrier init / descriptor prefetch /
+// parameter loads overlap the predecessor's tail and the launch latency disappears.
 template <typename... KArgs, typename... Args>
-cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), int grid, int block, int smem, cudaStream_t st, bool coresident, Args&&... args) {
+cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), dim3 grid, int block, int smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.gridDim = grid; cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute at[1];
   cfg.attrs = at; cfg.numAttrs = 0;
   if (h->pdl) { at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1; cfg.numAttrs = 1; }
-  else if (coresident) { at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1; cfg.numAttrs = 1; }
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
@@ -286,13 +255,14 @@ void free_workspace(LdmHandle* h) {
   void** ws[] = {&h->x16, &h->qkv16, &h->att16, &h->z16, &h->hid16, reinterpret_cast<void**>(&h->x32), reinterpret_cast<void**>(&h->y32),
                  reinterpret_cast<void**>(&h->logits), reinterpret_cast<void**>(&h->ids[0]), reinterpret_cast<void**>(&h->ids[1]),
                  reinterpret_cast<void**>(&h->ids_final), reinterpret_cast<void**>(&h->c_seq), reinterpret_cast<void**>(&h->c_seq_orig),
-                 reinterpret_cast<void**>(&h->c_mask), reinterpret_cast<void**>(&h->ln_stats), reinterpret_cast<void**>(&h->rel_lp)};
+                 reinterpret_cast<void**>(&h->c_mask), reinterpret_cast<void**>(&h->rel_lp)};
   for (void** p : ws) { if (*p) cudaFree(*p); *p = nullptr; }
   h->cap = 0;
 }
 
 int ensure_workspace(LdmHandle* h, int n_layouts) {
-  n_layouts = (n_layouts + 1) & ~1;     // GEMM CTA pairs work on 256-row blocks: keep an even number of layout tiles
+  // the GEMM grids put the row blocks in gridDim.y (<= 65535): 2 per layout for the LN GEMMs
+  if (n_layouts > kMaxLayouts) return fail(LDM_ERR_UNSUPPORTED, "batch of %d layouts exceeds the %d a call supports", n_layouts, kMaxLayouts);
   if (n_layouts <= h->cap) return LDM_OK;
   // free the old workspace: nothing may still be running on it, and a failed reallocation must not leave stale pointers behind
   CK(cudaDeviceSynchronize());
@@ -314,10 +284,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   CK(cudaMalloc(reinterpret_cast<void**>(&h->c_seq), nid * 8));
   CK(cudaMalloc(reinterpret_cast<void**>(&h->c_seq_orig), nid * 8));
   CK(cudaMalloc(reinterpret_cast<void**>(&h->c_mask), nid));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->ln_stats), static_cast<size_t>(n_layouts) * 2 * kBM * 2 * sizeof(unsigned long long)));
-  CK(cudaMemset(h->ln_stats, 0, static_cast<size_t>(n_layouts) * 2 * kBM * 2 * sizeof(unsigned long long)));
-  h->ln_epoch = 0;
-  // zero once: the padding layout (odd batch sizes) and the 3 padding rows of every layout tile must stay finite
+  // zero once: the 3 padding rows of every layout tile must stay finite
   CK(cudaMemset(h->x16, 0, M * d * 2)); CK(cudaMemset(h->qkv16, 0, M * kQkvN * 2)); CK(cudaMemset(h->att16, 0, M * kAttN * 2));
   CK(cudaMemset(h->z16, 0, M * d * 2)); CK(cudaMemset(h->hid16, 0, M * ff * 2)); CK(cudaMemset(h->x32, 0, M * d * 4));
   CK(cudaMemset(h->y32, 0, M * d * 4));
@@ -326,34 +293,18 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   h->ws_generation++;
   int rc;
   if ((rc = make_map(&h->m_x16, h->x16, M, d, kBM, h->bf16))) return rc;
-  if ((rc = make_map(&h->m_att16, h->att16, M, kAttN, kBM, h->bf16))) return rc;   // attention's TMA store target and the out-projection's A operand
+  if ((rc = make_map(&h->m_att16, h->att16, M, kAttN, 64, h->bf16))) return rc;   // the out-projection's A operand
   if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles
   if ((rc = make_map(&h->m_z16, h->z16, M, d, kBM, h->bf16))) return rc;
-  if ((rc = make_map(&h->m_hid16, h->hid16, M, ff, kBM, h->bf16))) return rc;
-  if ((rc = make_tail_map(&h->t_x16, h->x16, M, d, h->bf16))) return rc;
-  if ((rc = make_tail_map(&h->t_z16, h->z16, M, d, h->bf16))) return rc;
-  if ((rc = make_block_map(&h->b_qkv16, h->qkv16, M, kQkvN, 2, h->bf16))) return rc;
-  if ((rc = make_block_map(&h->b_hid16, h->hid16, M, ff, 2, h->bf16))) return rc;
-  if ((rc = make_block_map(&h->b_z16, h->z16, M, d, 2, h->bf16))) return rc;
-  if ((rc = make_block_map(&h->b_x16, h->x16, M, d, 2, h->bf16))) return rc;
-  if ((rc = make_block_map(&h->b_x32, h->x32, M, d, 4, false))) return rc;
-  if ((rc = make_block_map(&h->b_y32, h->y32, M, d, 4, false))) return rc;
-  if ((rc = make_block_map(&h->b_logits, h->logits, M, kLogitLd, 4, false))) return rc;
+  if ((rc = make_map(&h->m_hid16, h->hid16, M, ff, 64, h->bf16))) return rc;
   return LDM_OK;
 }
 
 template <bool BF16>
 int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
-  const int np = (n + 1) & ~1;            // layouts incl. the padding layout of an odd batch
-  const int M = np * kBM;
-  const int sms = h->num_sms & ~1;        // CTA pairs
-  // large batches: one CTA pair per 256-row block (it walks all N tiles of the block); small batches: single tiles are
-  // spread over the pairs so that more than np/2 pairs have work (LN epilogues always need whole row blocks)
-  auto tile_sched = [&](int n_tiles) { return (n_tiles > 1 && np / 2 < sms / 2) ? 1 : 0; };
-  auto pair_grid = [&](int n_tiles) { return std::min(tile_sched(n_tiles) ? np * n_tiles : np, sms); };
-  // LN GEMMs: units (row block, column tile) on neighbouring pairs -> an even number of pairs, all of them resident
-  const int ln_grid = std::min(2 * np, h->num_sms) & ~3;
+  const int M = n * kBM;
+  const dim3 ln_grid(1, M / 64);          // LN GEMMs: 64 whole rows per CTA
   int done = 0;
   // alternating sweep direction: every kernel walks the row blocks opposite to its predecessor (GemmParams::rev); the embedding /
   // draw kernels run their blocks in ascending order, so the first GEMM starts from the end.  LDM_SWEEP=0: always ascending
@@ -362,57 +313,52 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   // test tap: stop after `debug_stop_after` launches
 #define LDM_STAGE_DONE() do { if (h->debug_stop_after && ++done >= h->debug_stop_after) { CK(cudaGetLastError()); return LDM_OK; } } while (0)
   if (!skip_embed) {     // skipped inside the loop: the previous step's draw kernel has already written this step's x32 / x16 rows
-    const int warps = np * 128, blocks = (warps * 32 + 255) / 256;
+    const int warps = n * 128, blocks = (warps * 32 + 255) / 256;
     ProfScope ps(h, CAT_EMBED, st);
-    CK(launch_step(h, embed_adaln_kernel<BF16>, blocks, 256, 0, st, false, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
-                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16, n, np, h->S, d));
+    CK(launch_step(h, embed_adaln_kernel<BF16>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
+                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16, n, n, h->S, d));
   }
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
     {  // QKV projection (+bias, q * 1/sqrt(head_dim))
-      GemmParams p{M, kQkvN, d, kQkvN / 256, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
-      p.dbg = h->gemm_dbg; p.tile_sched = tile_sched(p.n_tiles); p.rev = next_rev(); p.store_evict_last = h->l2_hint & 1; p.load_evict_first = ((h->l2_hint & 16) ? 1 : 0) | ((h->l2_hint & 128) ? 4 : 0);
+      GemmParams p{M, kQkvN, d, kQkvN / kPlainBN, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
+      p.rev = next_rev();
       ProfScope ps(h, CAT_QKV, st);
-      CK(launch_step(h, gemm_tc_kernel<256, 256, kAresStages, EPI_QKV, BF16, true>, pair_grid(p.n_tiles), kGemmThreads, GemmSmem<256, kAresStages, EPI_QKV, true>::kBytes, st, false,
-                     h->m_x16, h->m_wqkv[l], h->b_qkv16, h->b_qkv16, h->b_qkv16, h->t_x16, p));
+      CK(launch_step(h, kGemmQkv<BF16>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, h->m_x16, h->m_wqkv[l], p));
     }
     LDM_STAGE_DONE();
     {
       ProfScope ps(h, CAT_ATTN, st);
-      CK(launch_step(h, attention_kernel<BF16>, std::min(np * h->desc.n_heads, 2 * h->num_sms), kAttThreads, kAttSmemBytes, st, false,
-                     h->m_qkv16, h->m_att16, h->S, h->desc.n_heads, np, d / h->desc.n_heads, next_rev(), ((h->l2_hint & 2) ? 1 : 0) | ((h->l2_hint & 64) ? 2 : 0)));
+      CK(launch_step(h, attention_kernel<BF16>, dim3(n * h->desc.n_heads), kAttThreads, kAttSmemBytes, st,
+                     h->m_qkv16, h->att16, h->S, h->desc.n_heads, n, next_rev()));
     }
     LDM_STAGE_DONE();
     {  // out-projection + bias + residual (from the NORMALISED x) -> y32 ; z16 = LayerNorm2(y)   [fused epilogue]
-      GemmParams p{M, d, kAttN, 2, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
-      p.dbg = h->gemm_dbg; p.tile_sched = 1; p.ln_stats = h->ln_stats; p.ln_epoch = ++h->ln_epoch; p.rev = next_rev(); p.store_evict_last = (h->l2_hint & 4) ? 1 : 0; p.load_evict_first = ((h->l2_hint & 16) ? 1 : 0) | ((h->l2_hint & 32) ? 2 : 0) | ((h->l2_hint & 128) ? 4 : 0);
+      GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
+      p.rev = next_rev();
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(launch_step(h, gemm_tc_kernel<224, 240, 3, EPI_LN, BF16>, ln_grid, kGemmThreads, GemmSmem<240, 3, EPI_LN>::kBytes, st, true,
-                     h->m_att16, h->m_wo[l], h->b_z16, h->b_x32, h->b_y32, h->b_y32, p));
+      CK(launch_step(h, kGemmLn<BF16>, ln_grid, kGemmThreads, kLnSmem, st, h->m_att16, h->m_wo[l], p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
-      GemmParams p{M, ff, d, (ff + 255) / 256, h->b1[l], h->hid16, ff, 1.0f, 0};   // 7 tiles of 256 columns + one of 64
-      p.dbg = h->gemm_dbg; p.tile_sched = tile_sched(p.n_tiles); p.rev = next_rev(); p.store_evict_last = h->l2_hint & 1; p.load_evict_first = ((h->l2_hint & 16) ? 1 : 0) | ((h->l2_hint & 128) ? 4 : 0);
+      GemmParams p{M, ff, d, (ff + kPlainBN - 1) / kPlainBN, h->b1[l], h->hid16, ff, 1.0f, 0};   // 7 tiles of 256 columns + one of 64
+      p.rev = next_rev();
       ProfScope ps(h, CAT_FF1, st);
-      CK(launch_step(h, gemm_tc_kernel<256, 256, kAresStages, EPI_RELU, BF16, true>, pair_grid(p.n_tiles), kGemmThreads, GemmSmem<256, kAresStages, EPI_RELU, true>::kBytes, st, false,
-                     h->m_z16, h->m_w1[l], h->b_hid16, h->b_hid16, h->b_hid16, h->t_z16, p));
+      CK(launch_step(h, kGemmFf1<BF16>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, h->m_z16, h->m_w1[l], p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
-      GemmParams p{M, d, ff, 2, h->b2[l], nullptr, d, 1.0f, 0, h->y32, nullptr, nullptr, nullptr, 0, nullptr};
-      const CUtensorMap* mo = &h->b_z16;
+      GemmParams p{M, d, ff, 1, h->b2[l], nullptr, d, 1.0f, 0, h->y32, nullptr, nullptr, nullptr, 0, nullptr};
       if (l + 1 < L) {
         const float* tab = h->adaln + (static_cast<size_t>(l + 1) * T + t_model) * 2 * d;
-        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16; mo = &h->b_x16;
+        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16;
         if (t_layout) { p.ln_scale = h->adaln + static_cast<size_t>(l + 1) * T * 2 * d; p.t_layout = t_layout; p.n_layouts = n; }   // per-layout rows
       } else {
         p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16;
       }
-      p.dbg = h->gemm_dbg; p.tile_sched = 1; p.ln_stats = h->ln_stats; p.ln_epoch = ++h->ln_epoch; p.rev = next_rev(); p.store_evict_last = (h->l2_hint & 8) ? 1 : 0; p.load_evict_first = ((h->l2_hint & 32) ? 2 : 0) | ((h->l2_hint & 128) ? 4 : 0) | ((h->l2_hint & 256) ? 8 : 0);   // hid16 is read by two pairs: never evict_first; 256 = evict_last
+      p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(launch_step(h, gemm_tc_kernel<224, 240, 5, EPI_LN, BF16>, ln_grid, kGemmThreads, GemmSmem<240, 5, EPI_LN>::kBytes, st, true,
-                     h->m_hid16, h->m_w2[l], *mo, h->b_y32, h->b_x32, h->b_x32, p));
+      CK(launch_step(h, kGemmLn<BF16>, ln_grid, kGemmThreads, kLnSmem, st, h->m_hid16, h->m_w2[l], p));
     }
     LDM_STAGE_DONE();
   }
@@ -420,8 +366,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, gemm_tc_kernel<160, 160, 5, EPI_F32, BF16>, pair_grid(1), kGemmThreads, GemmSmem<160, 5, EPI_F32>::kBytes, st, false,
-                   h->m_z16, h->m_whead, h->b_logits, h->b_logits, h->b_logits, h->b_logits, p));
+    CK(launch_step(h, kGemmHead<BF16>, dim3(1, n), kGemmThreads, kHeadSmem, st, h->m_z16, h->m_whead, p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
@@ -496,7 +441,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
     p1.cond_flags &= ~COND_PAD_DISABLE; p1.logprob_out = h->rel_lp; p1.emb_adaln = nullptr;    // its draw is discarded: no embedding
     {
       ProfScope ps(h, CAT_EPILOGUE, st);
-      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, false, p1));
+      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p1));
     }
     RelationParams r{};
     r.n_layouts = B; r.S = h->S; r.C = h->C; r.n_attr = h->desc.n_attr; r.n_elem = h->desc.n_elem; r.n_cat = h->desc.n_cat;
@@ -506,14 +451,14 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
     r.n_update = cond->rel_num_update;
     {
       ProfScope ps(h, CAT_EPILOGUE, st);
-      CK(launch_step(h, relation_update_kernel, B, kRelThreads, 0, st, false, r));
+      CK(launch_step(h, relation_update_kernel, B, kRelThreads, 0, st, r));
     }
     StepParams p2 = p;
     p2.logprob_in = h->rel_lp;
     p2.logprob_out = logprob_out;            // tap: the adjusted log-probs after PAD-disable (what sample() sees, base.py:287)
     {
       ProfScope ps(h, CAT_EPILOGUE, st);
-      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, false, p2));
+      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p2));
     }
     CK(cudaGetLastError());
     return LDM_OK;
@@ -524,8 +469,8 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
                       (p.mode == SAMP_DETERMINISTIC || p.mode == SAMP_RANDOM || p.mode == SAMP_GUMBEL ||
                        (p.mode == SAMP_TOP_P && p.top_p < 0.9999f)) && !h->debug_generic_posterior;
     for (int g = 0; g < p.n_attr; ++g) group_path = group_path && p.grp_n[g] <= 32;
-    if (group_path) CK(launch_step(h, posterior_sample_group_kernel, blocks, 256, 0, st, false, p));
-    else CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, false, p));
+    if (group_path) CK(launch_step(h, posterior_sample_group_kernel, blocks, 256, 0, st, p));
+    else CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p));
   }
   CK(cudaGetLastError());
   return LDM_OK;
@@ -536,7 +481,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
 extern "C" {
 
 const char* ldm_last_error(void) { return g_err; }
-const char* ldm_version(void) { return "ldm_b200 0.1 (sm_100a, tcgen05)"; }
+const char* ldm_version(void) { return "ldm_b200 0.2 (sm_90a, wgmma)"; }
 
 int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (!desc || !w || !out) return fail(LDM_ERR_INVALID, "null argument");
@@ -552,22 +497,18 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   CK(cudaSetDevice(desc->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, desc->device));
-  if (prop.major != 10) return fail(LDM_ERR_UNSUPPORTED, "sm_100a kernels need a Blackwell (CC 10.x) device, found CC %d.%d", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(LDM_ERR_UNSUPPORTED, "sm_90a kernels need a Hopper (CC 9.0) device, found CC %d.%d", prop.major, prop.minor);
   int rc = load_encode();
   if (rc) return rc;
 
   LdmHandle* h = new LdmHandle();
   h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T; h->bf16 = desc->operand_dtype == 1;
   h->G = desc->q_type == 0 ? desc->n_attr : 1;
-  h->num_sms = prop.multiProcessorCount;
-  if (const char* e = getenv("LDM_NUM_SMS")) { const int v = atoi(e); if (v >= 4 && v <= h->num_sms) h->num_sms = v; }   // experiments: persistent grids sized for a share of the GPU
-  if (const char* e = getenv("LDM_GEMM_DEBUG")) h->gemm_dbg = atoi(e);
   if (const char* e = getenv("LDM_GENERIC_POSTERIOR")) h->debug_generic_posterior = atoi(e);
   if (const char* e = getenv("LDM_PDL")) h->pdl = atoi(e);
   if (const char* e = getenv("LDM_GRAPH")) h->use_graph = atoi(e);
   if (const char* e = getenv("LDM_FUSE_EMBED")) h->fuse_embed = atoi(e);
   if (const char* e = getenv("LDM_SWEEP")) h->sweep = atoi(e);
-  if (const char* e = getenv("LDM_L2_HINT")) h->l2_hint = atoi(e);
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
   TRY(dev_upload(h, &h->cat_emb, w->cat_emb, static_cast<size_t>(C) * d));
@@ -620,10 +561,10 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(dev_upload(h, &h->b2[l], w->linear2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2w[l], w->norm2_w + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2b[l], w->norm2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(make_map(&h->m_wqkv[l], h->wqkv[l], kQkvN, d, 128, h->bf16));   // each CTA of a pair loads half of the weight tile
-    TRY(make_map(&h->m_wo[l], h->wo[l], d, kAttN, 120, h->bf16));
-    TRY(make_map(&h->m_w1[l], h->w1[l], ff, d, 128, h->bf16));
-    TRY(make_map(&h->m_w2[l], h->w2[l], d, ff, 120, h->bf16));
+    TRY(make_map(&h->m_wqkv[l], h->wqkv[l], kQkvN, d, kPlainBN, h->bf16));   // one warpgroup's weight rows per box
+    TRY(make_map(&h->m_wo[l], h->wo[l], d, kAttN, kLnBN, h->bf16));
+    TRY(make_map(&h->m_w1[l], h->w1[l], ff, d, kPlainBN, h->bf16));
+    TRY(make_map(&h->m_w2[l], h->w2[l], d, ff, kLnBN, h->bf16));
   }
   {
     float* tmp = nullptr;
@@ -633,7 +574,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     int* hmap_dev = nullptr;
     TRY(dev_upload(h, &hmap_dev, hmap.data(), hmap.size()));
     TRY(pack16(h, &h->whead, tmp, hmap_dev, kLogitLd, d, d));
-    TRY(make_map(&h->m_whead, h->whead, kLogitLd, d, kLogitLd / 2, h->bf16));
+    TRY(make_map(&h->m_whead, h->whead, kLogitLd, d, kHeadBN, h->bf16));
   }
   {
     std::vector<float> sch(static_cast<size_t>(h->G) * 8 * (T + 1));
@@ -651,32 +592,13 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   free_staging(h);
 
   if (h->bf16) {
-    TRY((set_smem(gemm_tc_kernel<256, 256, kAresStages, EPI_QKV, true, true>, GemmSmem<256, kAresStages, EPI_QKV, true>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<256, 256, kAresStages, EPI_RELU, true, true>, GemmSmem<256, kAresStages, EPI_RELU, true>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<160, 160, 5, EPI_F32, true>, GemmSmem<160, 5, EPI_F32>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<224, 240, 5, EPI_LN, true>, GemmSmem<240, 5, EPI_LN>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<224, 240, 3, EPI_LN, true>, GemmSmem<240, 3, EPI_LN>::kBytes)));
-    TRY((set_smem(attention_kernel<true>, kAttSmemBytes)));
+    TRY(set_smem(kGemmQkv<true>, kPlainSmem)); TRY(set_smem(kGemmFf1<true>, kPlainSmem));
+    TRY(set_smem(kGemmHead<true>, kHeadSmem)); TRY(set_smem(kGemmLn<true>, kLnSmem));
+    TRY(set_smem(attention_kernel<true>, kAttSmemBytes));
   } else {
-    TRY((set_smem(gemm_tc_kernel<256, 256, kAresStages, EPI_QKV, false, true>, GemmSmem<256, kAresStages, EPI_QKV, true>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<256, 256, kAresStages, EPI_RELU, false, true>, GemmSmem<256, kAresStages, EPI_RELU, true>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<160, 160, 5, EPI_F32, false>, GemmSmem<160, 5, EPI_F32>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<224, 240, 5, EPI_LN, false>, GemmSmem<240, 5, EPI_LN>::kBytes)));
-    TRY((set_smem(gemm_tc_kernel<224, 240, 3, EPI_LN, false>, GemmSmem<240, 3, EPI_LN>::kBytes)));
-    TRY((set_smem(attention_kernel<false>, kAttSmemBytes)));
-  }
-  if (h->pdl) {
-    // PDL replaces the cooperative launch of the LN GEMMs (see launch_step): their co-residency argument needs one CTA pair per
-    // SM pair to fit at once.  Ask the runtime; otherwise fall back to cooperative launches.
-    auto fits = [&](auto kernel, int smem) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(h->num_sms & ~3); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = smem;
-      int n = 0;
-      return cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) == cudaSuccess && 2 * n >= (h->num_sms & ~3);
-    };
-    const bool ok = h->bf16 ? (fits(gemm_tc_kernel<224, 240, 5, EPI_LN, true>, GemmSmem<240, 5, EPI_LN>::kBytes) && fits(gemm_tc_kernel<224, 240, 3, EPI_LN, true>, GemmSmem<240, 3, EPI_LN>::kBytes))
-                            : (fits(gemm_tc_kernel<224, 240, 5, EPI_LN, false>, GemmSmem<240, 5, EPI_LN>::kBytes) && fits(gemm_tc_kernel<224, 240, 3, EPI_LN, false>, GemmSmem<240, 3, EPI_LN>::kBytes));
-    if (!ok) { cudaGetLastError(); h->pdl = 0; }
+    TRY(set_smem(kGemmQkv<false>, kPlainSmem)); TRY(set_smem(kGemmFf1<false>, kPlainSmem));
+    TRY(set_smem(kGemmHead<false>, kHeadSmem)); TRY(set_smem(kGemmLn<false>, kLnSmem));
+    TRY(set_smem(attention_kernel<false>, kAttSmemBytes));
   }
 #undef TRY
   *out = h;
@@ -967,7 +889,7 @@ int ldm_predict_start(LdmHandle* h, int32_t B, const int64_t* xt_ids, const int3
   StepParams p = base_step_params(h, B);
   p.ids_in = reinterpret_cast<const long long*>(xt_ids); p.t_layout = t_dev; p.lx0_out = log_x0_out;   // ids_out == nullptr: no draw
   const int blocks = (B * h->S * 32 + 255) / 256;
-  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, false, p)); }
+  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p)); }
   CK(cudaGetLastError());
   return LDM_OK;
 }
@@ -979,7 +901,7 @@ int ldm_q_posterior(LdmHandle* h, int32_t B, const float* log_x_start, const int
   StepParams p = base_step_params(h, B);
   p.ids_in = reinterpret_cast<const long long*>(xt_ids); p.t_layout = t_dev; p.lx0_in = log_x_start; p.logprob_out = out;
   const int blocks = (B * h->S * 32 + 255) / 256;
-  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, false, p)); }
+  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p)); }
   CK(cudaGetLastError());
   return LDM_OK;
 }
@@ -1032,10 +954,10 @@ int ldm_vb_terms(LdmHandle* h, int32_t B, const int64_t* x0_ids, const int64_t* 
   v.kl_tok = tok; v.nll_tok = tok + nt; v.aux_tok = kl_aux_out ? tok + 2 * nt : nullptr;
   v.x0_recon = reinterpret_cast<long long*>(x0_recon_out); v.xtm1_recon = reinterpret_cast<long long*>(xtm1_recon_out);
   const int blocks = (B * h->S * 32 + 255) / 256, rblocks = (B * 32 + 255) / 256;
-  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, vb_terms_kernel, blocks, 256, 0, st, false, v)); }
-  { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, false, (const float*)v.kl_tok, kl_out, B, h->S)); }
-  { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, false, (const float*)v.nll_tok, nll_out, B, h->S)); }
-  if (kl_aux_out) { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, false, (const float*)v.aux_tok, kl_aux_out, B, h->S)); }
+  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, vb_terms_kernel, blocks, 256, 0, st, v)); }
+  { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, (const float*)v.kl_tok, kl_out, B, h->S)); }
+  { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, (const float*)v.nll_tok, nll_out, B, h->S)); }
+  if (kl_aux_out) { ProfScope ps(h, CAT_MISC, st); CK(launch_step(h, row_mean_kernel, rblocks, 256, 0, st, (const float*)v.aux_tok, kl_aux_out, B, h->S)); }
   CK(cudaGetLastError());
   return LDM_OK;
 }

@@ -1,4 +1,4 @@
-"""Host mirror of the reference's diffusion-core class API, running on the sm_100a library.
+"""Host mirror of the reference's diffusion-core class API, running on the sm_90a library.
 
   FusedMaskAndReplaceDiffusion   <->  BaseMaskAndReplaceDiffusion (+ Constrained / Vanilla subclasses)
                                       models/categorical_diffusion/base.py:29-371, constrained.py, vanilla.py
@@ -392,7 +392,7 @@ class LayoutDMB200:
 def patch_reference_model(model, operand_dtype: str = "fp16", device=None):
     """Drop-in for a live reference `trainer.models.layoutdm.LayoutDM`: after `load_state_dict`, call
     `patch_reference_model(model)`; `model.sample(...)` (layoutdm.py:77) and `model.model.sample(...)` /
-    `_sample_single_step(...)` then run on the sm_100a library.  Training `forward` is untouched."""
+    `_sample_single_step(...)` then run on the sm_90a library.  Training `forward` is untouched."""
     core = model.model.module if hasattr(model.model, "module") else model.model
     tok = model.tokenizer
     vocab = Vocab.from_tokenizer(tok)

@@ -45,7 +45,7 @@ class Engine:
                  operand_dtype: str = "fp16", device: Optional[int] = None, d_model: int = 464, n_heads: int = 8, d_ff: int = 1856,
                  att_1=0.99999, att_T=0.000009, ctt_1=0.000009, ctt_T=0.99999):
         if not torch.cuda.is_available():
-            raise RuntimeError("layoutdm_b200 needs a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("layoutdm_b200 needs a CUDA (sm_90a, H100) device; there is no CPU fallback")
         self.lib = _lib.load()
         self.vocab = vocab
         self.T = num_timesteps

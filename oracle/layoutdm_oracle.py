@@ -7,11 +7,11 @@ reference's `LayoutDM.sample()` path.  Only `tests/`, `__graft_entry__.smoke()` 
 fails loudly when its CUDA library is missing.
 
 Parity pin: the reference has NO tests / golden vectors of its own (SURVEY.md §4).  This restatement is
-pinned against the *unmodified reference itself*, imported through `oracle/ref_shims` in the build container
+pinned against the *unmodified reference itself*, imported through `oracle/ref_shims` where it is available
 (`tests/golden/make_golden.py`, `tests/test_oracle_vs_reference.py`), and against the fixtures that script
-commits under `tests/golden/` (those travel to the GPU box, /root/reference does not).
+commits under `tests/golden/` (the tests compare against those without the reference).
 
-Every function cites the reference file:line it follows.  `T/` = /root/reference/src/trainer/trainer/.
+Every function cites the reference file:line it follows.  `T/` = src/trainer/trainer/ of the layout-dm checkout.
 Tensor layout here is (B, S, C) ("token-major"); the reference uses (B, C, S).
 """
 from __future__ import annotations

@@ -1,9 +1,8 @@
 """
 TEST / BENCH INFRASTRUCTURE.  Builds the UNMODIFIED reference LayoutDM for oracle validation, golden-vector generation,
-the reference arm of bench.py and the drop-in test of `patch_reference_model`.  The reference package is imported from
-/root/reference when that exists (the build container) and otherwise from the archive oracle/make_ref.py packaged
-(oracle/_ref/trainer_ref.zip, zipimport: it travels to the GPU box, /root/reference does not), in both cases through the
-import stand-ins of oracle/ref_shims.
+the reference arm of bench.py and the drop-in test of `patch_reference_model`.  The reference package is imported from the layout-dm checkout
+(oracle/make_ref.py) when that exists, and otherwise from the archive oracle/make_ref.py packaged
+(oracle/_ref/trainer_ref.zip, zipimport), in both cases through the import stand-ins of oracle/ref_shims.
 
 Recipe = SURVEY.md Appendix B.
 """
@@ -16,14 +15,16 @@ from contextlib import contextmanager
 import numpy as np
 import torch
 
+from oracle import make_ref
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-REF_SRC = "/root/reference/src/trainer"
-REF_ZIP = os.path.join(HERE, "_ref", "trainer_ref.zip")
+REF_SRC = make_ref.REF_PKG_PARENT
+REF_ZIP = make_ref.OUT
 
 
 def reference_source() -> str | None:
-    """where the reference's `trainer` package is imported from: the read-only checkout, else the packaged archive"""
+    """where the reference's `trainer` package is imported from: the checkout, else the packaged archive"""
     if os.path.isdir(os.path.join(REF_SRC, "trainer")):
         return REF_SRC
     return REF_ZIP if os.path.exists(REF_ZIP) else None
@@ -35,7 +36,7 @@ def reference_available() -> bool:
 
 def _setup_path():
     src = reference_source()
-    assert src is not None, "reference not available: run `python oracle/make_ref.py` in the build container"
+    assert src is not None, "reference not available: no reference checkout and no archive packaged by `python oracle/make_ref.py`"
     for p in (src, os.path.join(HERE, "ref_shims")):
         if p not in sys.path:
             sys.path.insert(0, p)

@@ -1,11 +1,11 @@
 """
 Generates the committed golden fixtures under tests/golden/*.npz by running the UNMODIFIED reference
-(/root/reference, imported through oracle/ref_shims) on CPU, and checks the oracle restatement against it while
+(the reference checkout, imported through oracle/ref_shims) on CPU, and checks the oracle restatement against it while
 doing so.  Run in the build container only:
 
     python tests/golden/make_golden.py
 
-What a fixture holds (everything needed on the GPU box, where /root/reference does not exist):
+What a fixture holds (everything the tests need where the reference is absent):
   * the case description (dataset, q_type, T, T_eval, sampling cfg, weight seed/scale, noise seed) and the
     checksum of the synthetic weights (regenerated on the box by oracle.make_weights),
   * the reference's inputs (cond seq/mask/seq_orig, refinement table) and, per loop iteration, the ids the

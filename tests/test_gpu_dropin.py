@@ -1,7 +1,7 @@
 """GPU (-m gpu): the drop-in INTEGRATION.md tells a maintainer to use -- `patch_reference_model(model)` on a LIVE, UNMODIFIED
-reference `LayoutDM` (imported from the packaged archive oracle/_ref/trainer_ref.zip, or /root/reference where that exists).
+reference `LayoutDM` (imported from the packaged archive oracle/_ref/trainer_ref.zip, or the reference checkout).
 After patching, the reference's own `model.sample(...)` / `model.model.sample(get_intermediate_results=True)` /
-`_sample_single_step(...)` run on the sm_100a library and are compared with the golden trajectories the same reference
+`_sample_single_step(...)` run on the sm_90a library and are compared with the golden trajectories the same reference
 produced on the CPU (tests/golden) under the shared noise key."""
 import copy
 

@@ -99,7 +99,7 @@ def test_epilogue_every_step_against_oracle(name):
 
 
 def test_denoiser_logits_at_reference_weight_scale():
-    """the 1e-3 gate proper: tcgen05 denoiser (fp16 operands, fp32 accumulate) vs the fp32 restatement of the reference,
+    """the 1e-3 gate proper: wgmma denoiser (fp16 operands, fp32 accumulate) vs the fp32 restatement of the reference,
     weights at the reference's init scale, several timesteps and token mixes"""
     from layoutdm_b200 import Engine, Vocab
     vo, spec = O.RICO25, O.ModelSpec()

@@ -1,10 +1,9 @@
 """GPU (-m gpu): parity of the LARGE-BATCH schedule -- the code path bench.py times.
 
-At B <= 8 the GEMMs take the tile-granular schedule (one work unit per CTA pair) and attention one item per CTA.  From
-np >= 148 the QKV / FF1 / head GEMMs walk all N tiles of a row block with the A block resident (accumulator ping-pong,
-`aempty` recycling), from np > 74 the LN GEMMs give a pair several (row block, column tile) units (accumulator / phase
-flips, staging reuse), and from np > 37 attention runs several items per CTA (double-buffer recycling).  These tests
-compare that steady state with the oracle on EVERY row: logits <= LOGIT_TOL at the reference's weight scale, and every
+Every kernel runs one tile per CTA (GEMMs: 128-row x 256-column tiles, 64-row whole-row tiles for the LN epilogues;
+attention: one (layout, head) per CTA), so a large batch is many waves of CTAs over the 132 SMs, with the row-block order
+reversed on every other kernel.  The sizes cover one to several waves, an odd batch and the 4096-layout config.  These
+tests compare that steady state with the oracle on EVERY row: logits <= LOGIT_TOL at the reference's weight scale, and every
 intermediate buffer of the launch sequence against the same-rounding oracle so that a failure names the kernel.
 Everything goes through the C ABI."""
 import numpy as np
@@ -61,7 +60,7 @@ def oracle_logits(sd, ids, t, vo, spec, chunk=256, **kw):
 @pytest.mark.parametrize("B", [148, 296, 301, 1024])
 def test_logits_all_rows_large_batch(B):
     """two consecutive denoising steps at the benchmarked schedule; the handle first serves a small batch, so the workspace
-    grows mid-handle; odd B exercises the padding layout.  All B x 125 rows are compared."""
+    grows mid-handle; odd B checks grids sized by the batch itself.  All B x 125 rows are compared."""
     eng, sd, vo, spec = engine()
     small = mixed_ids(5, vo, 1)
     _, lg_s, _ = eng.step(small.cuda(), 11, 11, {"name": "deterministic"}, want_logits=True)
@@ -87,7 +86,7 @@ def test_logits_all_rows_large_batch(B):
 
 
 def test_logits_config4_refinement_T200_B4096():
-    """BASELINE config 4 shape: T=200 model, batch 4096 (28 row blocks per CTA pair)"""
+    """BASELINE config 4 shape: T=200 model, batch 4096 (8192 LN-GEMM CTAs, about 62 waves)"""
     eng, sd, vo, spec = engine(T=200)
     B = 4096
     ids = mixed_ids(B, vo, 4)
@@ -101,7 +100,7 @@ def test_logits_config4_refinement_T200_B4096():
 
 
 def test_stage_taps_large_batch():
-    """every kernel of the launch sequence at B=300 (multi-unit schedule everywhere), against the same-rounding oracle"""
+    """every kernel of the launch sequence at B=300 (several waves of CTAs in every kernel), against the same-rounding oracle"""
     eng, sd, vo, spec = engine()
     B, t, S = 300, 42, vo.S
     ids = mixed_ids(B, vo, 9)

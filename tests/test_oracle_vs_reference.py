@@ -1,4 +1,5 @@
-"""CPU, build container only (skipped when /root/reference is absent): pieces of the oracle against the UNMODIFIED
+"""CPU, only where the reference is available (its checkout or the packaged archive; tests/test_oracle_reference_golden.py
+runs the same comparisons against stored reference outputs everywhere): pieces of the oracle against the UNMODIFIED
 reference beyond what tests/golden/make_golden.py already asserts while generating the fixtures."""
 import numpy as np
 import pytest
@@ -7,7 +8,7 @@ import torch
 import ref_harness as rh
 from oracle import layoutdm_oracle as O
 
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="reference checkout not present (GPU box)")
+pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="reference not available")
 
 
 @pytest.fixture(scope="module")

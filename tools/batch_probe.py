@@ -8,7 +8,7 @@ eng = Engine.from_state_dict(random_state_dict(vocab), vocab)
 cfg = {"name": "random", "temperature": 1.0}
 plan = timestep_plan(100, 100)
 out = {}
-for B in (148, 296, 444, 592, 1024, 1036, 2072):
+for B in (132, 264, 528, 1024, 2048):
     for _ in range(2): eng.sample_loop(B, plan, cfg, seed=1)
     torch.cuda.synchronize(); t0 = time.perf_counter()
     n = 3

@@ -1,5 +1,4 @@
-"""Per-kernel timing of a few denoising steps (CUDA events via ldm_profile_*), optionally with the GEMM bring-up probes:
-    LDM_GEMM_DEBUG=1 (no MMAs) / 2 (no TMA operand loads)  python tools/gemm_probe.py"""
+"""Per-kernel timing of a few denoising steps (CUDA events via ldm_profile_*):  B=1024 STEPS=6 python tools/gemm_probe.py"""
 import os, sys, json
 import torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -13,5 +12,5 @@ plan = timestep_plan(100, 100)[:steps]
 cfg = {"name": "random", "temperature": 1.0}
 eng.sample_loop(B, plan, cfg, seed=1); torch.cuda.synchronize()
 eng.profile_begin(); eng.sample_loop(B, plan, cfg, seed=2); prof = eng.profile_end()
-print(json.dumps({"dbg": os.environ.get("LDM_GEMM_DEBUG", "0"), "B": B,
+print(json.dumps({"B": B,
                   "us_per_launch": {k: round(v[0] * 1e3 / v[1], 1) for k, v in prof.items() if v[1]}}))
