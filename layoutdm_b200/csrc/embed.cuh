@@ -54,19 +54,26 @@ LDM_DEVINL void embed_token_row(const long long id, const int s, const size_t ro
   const float4* e = reinterpret_cast<const float4*>(cat_emb + static_cast<size_t>(id) * d);
   const float4* p = reinterpret_cast<const float4*>(pos + static_cast<size_t>(s) * d);
   float4 v[4];
-  float sum = 0.0f;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const int i = lane + 32 * k;
     if (i < nv) {
       const float4 a = __ldg(e + i), c = __ldg(p + i);
       v[k] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
-      sum += (v[k].x + v[k].y) + (v[k].z + v[k].w);
     } else {
       v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  const float mean = warp_sum(sum) / d;
+  // the row sum is taken of h - h[0]: its terms are of the row's spread, not of its mean, so the mean of a row far from zero
+  // comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the mean, which every
+  // output of the row inherits)
+  const float piv = __shfl_sync(0xffffffffu, v[0].x, 0);
+  float sum = 0.0f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (lane + 32 * k < nv) sum += ((v[k].x - piv) + (v[k].y - piv)) + ((v[k].z - piv) + (v[k].w - piv));
+  }
+  const float mean = piv + warp_sum(sum) / d;
   float var = 0.0f;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {

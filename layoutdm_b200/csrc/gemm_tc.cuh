@@ -59,7 +59,7 @@ struct GemmSmem {
   static constexpr int kStageBytes = kABytes + kWgN * kBBytes;
   static_assert(kBBytes % 1024 == 0, "weight block must keep 1024-B (swizzle atom) alignment");
   static constexpr int kOffBars = STAGES * kStageBytes;
-  static constexpr int kOffStat = kOffBars + 256;                // LN: per-row (sum, sumsq) of each warpgroup's columns
+  static constexpr int kOffStat = kOffBars + 256;                // LN: per-row sum, then sum of squared deviations, of each warpgroup's columns
   static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
   static_assert(2 * STAGES * 8 <= 256, "barrier block overflow");
   static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
@@ -177,13 +177,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
     }
   } else {
     // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
-    //   y = acc + bias + resid (-> y_out), row statistics over the thread's columns, the quad of lanes that shares a row,
-    //   then the other warpgroup (other 232 columns) through shared memory; normalise, 16-bit (+ fp32) outputs.
-    float2* sstat = reinterpret_cast<float2*>(smem + SM::kOffStat);
+    //   y = acc + bias + resid (-> y_out); two-pass row statistics: the row sum over the thread's columns, the quad of lanes
+    //   that shares a row, then the other warpgroup (other 232 columns) through shared memory gives the mean; the sum of
+    //   (y - mean)^2 is reduced the same way.  One pass, E[y^2] - mean^2, loses the variance to cancellation once
+    //   |mean| / std is large.  The sums run over y - pivot, pivot = bias[0] + resid[row][0] (y's column 0 without the GEMM
+    //   term, the same in all 8 threads of a row): their terms are of the row's spread, not of its mean, so the mean of a row
+    //   far from zero comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the
+    //   mean, which every output of the row inherits).  Normalise, 16-bit (+ fp32) outputs.
+    float* ssum = reinterpret_cast<float*>(smem + SM::kOffStat);   // [warpgroup][64 rows] row sums of y - pivot
+    float* ssq = ssum + 2 * 64;                                     // [warpgroup][64 rows] sums of squared deviations
     const int N = p.N;
-    float s0 = 0.0f, q0 = 0.0f, s1 = 0.0f, q1 = 0.0f;
     const float* r0p = p.resid + static_cast<size_t>(row0) * N;
     const float* r1p = p.resid + static_cast<size_t>(row1) * N;
+    const float piv0 = __ldg(p.bias) + r0p[0], piv1 = __ldg(p.bias) + r1p[0];
+    float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
     for (int j = 0; j < BN_WG / 8; ++j) {
       const int c = col0 + 8 * j;
@@ -191,25 +198,39 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
       const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
       acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
       acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
-      s0 += acc[4 * j] + acc[4 * j + 1]; q0 = fmaf(acc[4 * j], acc[4 * j], fmaf(acc[4 * j + 1], acc[4 * j + 1], q0));
-      s1 += acc[4 * j + 2] + acc[4 * j + 3]; q1 = fmaf(acc[4 * j + 2], acc[4 * j + 2], fmaf(acc[4 * j + 3], acc[4 * j + 3], q1));
       if (p.y_out != nullptr) {
         *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
         *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
+      acc[4 * j] -= piv0; acc[4 * j + 1] -= piv0; acc[4 * j + 2] -= piv1; acc[4 * j + 3] -= piv1;   // from here on: y - pivot
+      s0 += acc[4 * j] + acc[4 * j + 1];
+      s1 += acc[4 * j + 2] + acc[4 * j + 3];
     }
 #pragma unroll
     for (int o = 1; o <= 2; o <<= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o); q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
     }
-    if ((lane & 3) == 0) { sstat[wn * 64 + rw] = make_float2(s0, q0); sstat[wn * 64 + rw + 8] = make_float2(s1, q1); }
+    if ((lane & 3) == 0) { ssum[wn * 64 + rw] = s0; ssum[wn * 64 + rw + 8] = s1; }
     named_bar_sync(1, kGemmConsumers);
-    const float2 o0 = sstat[(wn ^ 1) * 64 + rw], o1 = sstat[(wn ^ 1) * 64 + rw + 8];
     const float inv_n = 1.0f / static_cast<float>(N);
-    const float mean0 = (s0 + o0.x) * inv_n, mean1 = (s1 + o1.x) * inv_n;
-    const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + o0.y) * inv_n - mean0 * mean0, 0.0f) + 1e-5f);
-    const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + o1.y) * inv_n - mean1 * mean1, 0.0f) + 1e-5f);
+    const float mean0 = (s0 + ssum[(wn ^ 1) * 64 + rw]) * inv_n, mean1 = (s1 + ssum[(wn ^ 1) * 64 + rw + 8]) * inv_n;   // mean - pivot, like acc
+    float q0 = 0.0f, q1 = 0.0f;
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const float d0 = acc[4 * j] - mean0, d1 = acc[4 * j + 1] - mean0, d2 = acc[4 * j + 2] - mean1, d3 = acc[4 * j + 3] - mean1;
+      q0 = fmaf(d0, d0, fmaf(d1, d1, q0));
+      q1 = fmaf(d2, d2, fmaf(d3, d3, q1));
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+      q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+    }
+    if ((lane & 3) == 0) { ssq[wn * 64 + rw] = q0; ssq[wn * 64 + rw + 8] = q1; }
+    named_bar_sync(1, kGemmConsumers);
+    const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
+    const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
     const float* gam = p.ln_scale;
     const float* bet = p.ln_shift;
     float gadd = p.adaln ? 1.0f : 0.0f;

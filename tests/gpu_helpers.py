@@ -6,8 +6,9 @@ import ctypes as C
 import torch
 
 
-def debug_read(engine, name: str, n_layouts: int) -> torch.Tensor:
-    """copy a workspace buffer of the first n_layouts layouts to the host; returns [n_layouts, 128, cols] float32"""
+def debug_read(engine, name: str, n_layouts: int, raw: bool = False) -> torch.Tensor:
+    """copy a workspace buffer of the first n_layouts layouts to the host; returns [n_layouts, 128, cols] float32
+    (raw: in the buffer's own dtype, for bitwise comparisons)"""
     lib, h = engine.lib, engine._h
     nbytes = lib.ldm_debug_read(h, name.encode(), None, 0, n_layouts)
     assert nbytes > 0, f"unknown buffer {name}"
@@ -16,7 +17,8 @@ def debug_read(engine, name: str, n_layouts: int) -> torch.Tensor:
     out = torch.empty(nbytes // (4 if is32 else 2), dtype=dt)
     rc = lib.ldm_debug_read(h, name.encode(), C.c_void_p(out.data_ptr()), nbytes, n_layouts)
     assert rc == nbytes, f"ldm_debug_read failed rc={rc}"
-    return out.view(n_layouts, 128, -1).float()
+    out = out.view(n_layouts, 128, -1)
+    return out if raw else out.float()
 
 
 def unpack_qkv(qkv: torch.Tensor, S: int = 125, heads: int = 8, dh: int = 58):

@@ -101,9 +101,20 @@ def test_epilogue_every_step_against_oracle(name):
 def test_denoiser_logits_at_reference_weight_scale():
     """the 1e-3 gate proper: wgmma denoiser (fp16 operands, fp32 accumulate) vs the fp32 restatement of the reference,
     weights at the reference's init scale, several timesteps and token mixes"""
+    _logits_vs_fp32_oracle("ref")
+
+
+def test_denoiser_logits_row_offset_weights():
+    """the same 1e-3 gate with + 256 on the out-projection / FF2 biases and the token embedding
+    (kernel_refs.weight_set("offset")): every LayerNorm sees rows whose mean is far from zero"""
+    _logits_vs_fp32_oracle("offset")
+
+
+def _logits_vs_fp32_oracle(weights):
     from layoutdm_b200 import Engine, Vocab
+    import kernel_refs as R
     vo, spec = O.RICO25, O.ModelSpec()
-    sd = O.make_weights(vo, spec, seed=0, scale=1.0)
+    sd = R.weight_set(weights, vo, spec, seed=0)
     _engines.clear()
     eng = Engine.from_state_dict(sd, Vocab.for_dataset("rico25"), num_timesteps=spec.T)
     g = torch.Generator().manual_seed(0)
@@ -116,7 +127,7 @@ def test_denoiser_logits_at_reference_weight_scale():
         with torch.no_grad():
             ref = O.denoiser_forward(sd, ids, t, vo, spec)
         d = (lg.cpu() - ref).abs().max().item()
-        print(f"t={t}: max|logit|={ref.abs().max():.3f} max-abs error {d:.2e}")
+        print(f"{weights} t={t}: max|logit|={ref.abs().max():.3f} max-abs error {d:.2e}")
         worst = max(worst, d)
     assert worst < LOGIT_TOL
 

@@ -17,14 +17,16 @@ pytestmark = pytest.mark.gpu
 
 LOGIT_TOL = 1e-3      # max-abs on fp32 logits vs the fp32 restatement of the reference, weights at the reference's init scale
 STAGE_REL = 4e-3      # per-stage gate vs the same-rounding oracle, relative to the stage's own magnitude: 16-bit buffers carry
-                      # one rounding (2^-11 relative for fp16) plus the accumulated difference of the upstream fp32 stream
+                      # one rounding (2^-11 relative for fp16) plus the accumulated difference of the upstream fp32 stream;
+                      # for bf16 operands the gate scales with the unit roundoff (2^-8 / 2^-11 = 8x)
+U_OP = {"fp16": 2.0 ** -11, "bf16": 2.0 ** -8}
 
 _state = {}
 
 
-def engine(dataset="rico25", T=100, scale=1.0, seed=0):
+def engine(dataset="rico25", T=100, scale=1.0, seed=0, dtype="fp16"):
     from layoutdm_b200 import Engine, Vocab
-    key = (dataset, T, scale, seed)
+    key = (dataset, T, scale, seed, dtype)
     if _state.get("key") != key:
         _state.clear()
         torch.cuda.empty_cache()
@@ -32,7 +34,7 @@ def engine(dataset="rico25", T=100, scale=1.0, seed=0):
         spec = O.ModelSpec(T=T)
         sd = O.make_weights(vo, spec, seed=seed, scale=scale)
         _state.update(key=key, vo=vo, spec=spec, sd=sd,
-                      eng=Engine.from_state_dict(sd, Vocab.for_dataset(dataset), num_timesteps=T))
+                      eng=Engine.from_state_dict(sd, Vocab.for_dataset(dataset), num_timesteps=T, operand_dtype=dtype))
     return _state["eng"], _state["sd"], _state["vo"], _state["spec"]
 
 
@@ -101,14 +103,24 @@ def test_logits_config4_refinement_T200_B4096():
 
 def test_stage_taps_large_batch():
     """every kernel of the launch sequence at B=300 (several waves of CTAs in every kernel), against the same-rounding oracle"""
-    eng, sd, vo, spec = engine()
+    _stage_taps("fp16")
+
+
+def test_stage_taps_large_batch_bf16():
+    """the same with bf16 operands, against the bf16 same-rounding oracle; the gate scales with the unit roundoff"""
+    _stage_taps("bf16")
+
+
+def _stage_taps(dtype):
+    eng, sd, vo, spec = engine(dtype=dtype)
+    gate = STAGE_REL * U_OP[dtype] / U_OP["fp16"]
     B, t, S = 300, 42, vo.S
     ids = mixed_ids(B, vo, 9)
     taps = {}
     with torch.no_grad():
         for i in range(0, B, 100):
             tp = {}
-            O.denoiser_forward(sd, ids[i:i + 100], t, vo, spec, operand_dtype=torch.float16, taps=tp)
+            O.denoiser_forward(sd, ids[i:i + 100], t, vo, spec, operand_dtype=torch.float16 if dtype == "fp16" else torch.bfloat16, taps=tp)
             for k, v in tp.items():
                 taps.setdefault(k, []).append(v)
     taps = {k: torch.cat(v) for k, v in taps.items()}
@@ -122,7 +134,7 @@ def test_stage_taps_large_batch():
         rel = d.max().item() / max(1.0, want.abs().max().item())
         report.append((name, d.max().item(), want.abs().max().item()))
         per_layout = d.reshape(B, -1).amax(dim=1)
-        assert rel < STAGE_REL, f"{name}: max-abs {d.max():.3e} (ref max {want.abs().max():.3f}), worst layouts {per_layout.topk(4).indices.tolist()}"
+        assert rel < gate, f"{name}: max-abs {d.max():.3e} (ref max {want.abs().max():.3f}), worst layouts {per_layout.topk(4).indices.tolist()}"
 
     def run(n):
         G.set_stop_after(eng, n)
@@ -153,7 +165,7 @@ def test_stage_taps_large_batch():
     finally:
         G.set_stop_after(eng, 0)
         for name, d, m in report:
-            print(f"{name:22s} max-abs {d:.3e}  ref max {m:.3f}")
+            print(f"{dtype} {name:22s} max-abs {d:.3e}  ref max {m:.3f}")
 
 
 def test_logprob_in_draw_is_bit_exact():
