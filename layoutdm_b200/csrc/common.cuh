@@ -217,14 +217,41 @@ LDM_DEVINL uint4 philox4x32_10(uint4 c, uint2 k) {
   }
   return c;
 }
+
 // u in (0,1): ((word >> 9) + 0.5) * 2^-23  (exact in fp32)
+LDM_DEVINL float u01_from_bits(uint32_t w) { return (static_cast<float>(w >> 9) + 0.5f) * 1.1920928955078125e-07f; }
+
+// Gumbel noise of a uniform (sampling.py:112-116)
+LDM_DEVINL float gumbel_of(float u) { return -logf(-logf(u + 1e-30f) + 1e-30f); }
+
+// Counter word 1 of the noise contract: the step in bits 0..23, the stream in bits 24+ (0 = draw, 1 = Gumbel of
+// name="gumbel", 2 = q_sample / gumbel_argmax).
+LDM_DEVINL uint32_t noise_ctr(uint32_t step, uint32_t stream) { return (step & 0xFFFFFFu) | (stream << 24); }
+
+// The noise of one token: key = seed, tok = (b_global0 + b) * S + s.  Class c draws word c & 3 of Philox block c >> 2.
+struct TokenNoise {
+  uint2 key; uint32_t tok_lo, tok_hi;
+  LDM_DEVINL TokenNoise(unsigned long long seed, unsigned long long b_global0, int b, int S, int s) {
+    const unsigned long long tok = (b_global0 + b) * static_cast<unsigned long long>(S) + s;
+    key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+    tok_lo = static_cast<uint32_t>(tok); tok_hi = static_cast<uint32_t>(tok >> 32);
+  }
+  LDM_DEVINL uint4 block(int blk, uint32_t ctr) const { return philox4x32_10(make_uint4(static_cast<uint32_t>(blk), ctr, tok_lo, tok_hi), key); }
+  static LDM_DEVINL int block_of(int c) { return c >> 2; }
+  static LDM_DEVINL uint32_t word_of(const uint4& r, int c) { const int k = c & 3; return k == 0 ? r.x : k == 1 ? r.y : k == 2 ? r.z : r.w; }
+  // the words of lane l's classes 4l..4l+3 and 128+l (the class ownership of the one-warp-per-token kernels)
+  LDM_DEVINL void lane_words(int lane, uint32_t ctr, uint32_t (&w)[5]) const {
+    const uint4 a = block(block_of(4 * lane), ctr), b = block(block_of(128 + lane), ctr);
+    w[0] = word_of(a, 4 * lane); w[1] = word_of(a, 4 * lane + 1); w[2] = word_of(a, 4 * lane + 2); w[3] = word_of(a, 4 * lane + 3);
+    w[4] = word_of(b, 128 + lane);
+  }
+};
+
 LDM_DEVINL float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-LDM_DEVINL float u01_from_bits(uint32_t w) { return (static_cast<float>(w >> 9) + 0.5f) * 1.1920928955078125e-07f; }
 
 LDM_DEVINL float warp_max(float v) {
 #pragma unroll

@@ -109,7 +109,6 @@ struct LdmHandle {
   int C = 0, S = 0, L = 0, T = 0, G = 0;
   bool bf16 = false;
   int64_t launches = 0;
-  int debug_generic_posterior = 0;   // env LDM_GENERIC_POSTERIOR=1: always take the all-classes posterior / sampling kernel (tests)
   int pdl = 1;                // env LDM_PDL=0: no programmatic dependent launch
   int debug_stop_after = 0;   // test tap: stop the denoiser after this many launches (0 = run everything)
   bool prof = false;          // per-kernel CUDA-event timing (ldm_profile_begin/end)
@@ -384,6 +383,21 @@ int validate_common(LdmHandle* h, int B, const LdmSampling* s) {
   return LDM_OK;
 }
 
+StepParams base_step_params(const LdmHandle* h, int B) {
+  StepParams p{};
+  p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr;
+  p.pad_id = h->C - 2; p.mask_id = h->C - 1;
+  p.constrained = h->desc.q_type == 0;
+  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) {
+    p.grp_start[g] = g == 0 ? 0 : h->desc.n_cat + (g - 1) * h->desc.n_bins;
+    p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
+  }
+  p.T = h->T; p.sched = h->sched; p.lae = h->lae;
+  p.logits = h->logits; p.ld_logits = kLogitLd;
+  p.mode = SAMP_DETERMINISTIC; p.temperature = 1.0f;
+  return p;
+}
+
 int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_post, const LdmCond* cond, const LdmSampling* samp,
               uint64_t seed, uint32_t step_ctr, int64_t b_global0, long long* ids_out, float* logits_out, float* logprob_out,
               const float* logits_in, const float* logprob_in, cudaStream_t st, const unsigned long long* call = nullptr,
@@ -405,16 +419,8 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
       logits_gather_kernel<<<1024, 256, 0, st>>>(h->logits, logits_out, B, h->S, h->C);
     }
   }
-  StepParams p{};
-  p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr;
-  p.pad_id = h->C - 2; p.mask_id = h->C - 1;
-  p.constrained = h->desc.q_type == 0;
-  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) {
-    p.grp_start[g] = g == 0 ? 0 : h->desc.n_cat + (g - 1) * h->desc.n_bins;
-    p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
-  }
-  p.T = h->T; p.t_post = t_post; p.sched = h->sched; p.lae = h->lae;
-  p.logits = h->logits; p.ld_logits = kLogitLd; p.logprob_in = logprob_in; p.ids_in = ids_in;
+  StepParams p = base_step_params(h, B);
+  p.t_post = t_post; p.logprob_in = logprob_in; p.ids_in = ids_in;
   if (cond && cond->seq) {
     p.cond_seq = reinterpret_cast<const long long*>(cond->seq); p.cond_mask = cond->mask;
     p.cond_seq_orig = reinterpret_cast<const long long*>(cond->seq_orig); p.refine_tbl = cond->refine_table;
@@ -465,11 +471,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
   }
   {
     ProfScope ps(h, CAT_EPILOGUE, st);
-    bool group_path = p.constrained && p.logprob_in == nullptr && p.logprob_out == nullptr &&
-                      (p.mode == SAMP_DETERMINISTIC || p.mode == SAMP_RANDOM || p.mode == SAMP_GUMBEL ||
-                       (p.mode == SAMP_TOP_P && p.top_p < 0.9999f)) && !h->debug_generic_posterior;
-    for (int g = 0; g < p.n_attr; ++g) group_path = group_path && p.grp_n[g] <= 32;
-    if (group_path) CK(launch_step(h, posterior_sample_group_kernel, blocks, 256, 0, st, p));
+    if (group_kernel_applies(p)) CK(launch_step(h, posterior_sample_group_kernel, blocks, 256, 0, st, p));
     else CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p));
   }
   CK(cudaGetLastError());
@@ -504,7 +506,6 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   LdmHandle* h = new LdmHandle();
   h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T; h->bf16 = desc->operand_dtype == 1;
   h->G = desc->q_type == 0 ? desc->n_attr : 1;
-  if (const char* e = getenv("LDM_GENERIC_POSTERIOR")) h->debug_generic_posterior = atoi(e);
   if (const char* e = getenv("LDM_PDL")) h->pdl = atoi(e);
   if (const char* e = getenv("LDM_GRAPH")) h->use_graph = atoi(e);
   if (const char* e = getenv("LDM_FUSE_EMBED")) h->fuse_embed = atoi(e);
@@ -797,20 +798,13 @@ int ldm_sample_host(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
 int ldm_q_sample(LdmHandle* h, int32_t B, const int64_t* x0, const int32_t* t, uint64_t seed, int64_t b_global0, int64_t* xt, void* stream) {
   if (!h || !x0 || !t || !xt || B <= 0) return fail(LDM_ERR_INVALID, "bad ldm_q_sample arguments");
   CK(cudaSetDevice(h->desc.device));
-  QSampleParams p{};
-  p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr; p.pad_id = h->C - 2; p.mask_id = h->C - 1;
-  p.constrained = h->desc.q_type == 0;
-  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) {
-    p.grp_start[g] = g == 0 ? 0 : h->desc.n_cat + (g - 1) * h->desc.n_bins;
-    p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
-  }
-  p.T = h->T; p.sched = h->sched; p.x0 = reinterpret_cast<const long long*>(x0); p.t = t;
-  p.seed = seed; p.b_global0 = b_global0; p.xt = reinterpret_cast<long long*>(xt);
+  StepParams p = base_step_params(h, B);
+  p.seed = seed; p.b_global0 = b_global0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int warps = B * h->S, blocks = (warps * 32 + 255) / 256;
   {
     ProfScope ps(h, CAT_MISC, st);
-    q_sample_kernel<<<blocks, 256, 0, st>>>(p);
+    q_sample_kernel<<<blocks, 256, 0, st>>>(p, reinterpret_cast<const long long*>(x0), t, reinterpret_cast<long long*>(xt));
   }
   CK(cudaGetLastError());
   return LDM_OK;
@@ -855,21 +849,6 @@ int ldm_make_cond(LdmHandle* h, int32_t B, int32_t cond_type, const int64_t* lab
 }
 
 namespace {
-
-StepParams base_step_params(const LdmHandle* h, int B) {
-  StepParams p{};
-  p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr;
-  p.pad_id = h->C - 2; p.mask_id = h->C - 1;
-  p.constrained = h->desc.q_type == 0;
-  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) {
-    p.grp_start[g] = g == 0 ? 0 : h->desc.n_cat + (g - 1) * h->desc.n_bins;
-    p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
-  }
-  p.T = h->T; p.sched = h->sched; p.lae = h->lae;
-  p.logits = h->logits; p.ld_logits = kLogitLd;
-  p.mode = SAMP_DETERMINISTIC; p.temperature = 1.0f;
-  return p;
-}
 
 int run_denoiser_per_layout_t(LdmHandle* h, int B, const long long* ids, const int32_t* t_dev, cudaStream_t st) {
   int rc = ensure_workspace(h, B);

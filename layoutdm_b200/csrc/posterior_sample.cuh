@@ -6,7 +6,8 @@
 //   Converter f_to_p_log/p_to_f_log   T/helpers/layout_tokenizer.py:540-557  (here: compile-free vocab group test)
 //   strong mask / refinement / pad-disable   base.py:243-284, T/helpers/task.py:154-224
 //   sample()                      T/helpers/sampling.py:81-130 ; torch.multinomial(p,1) == argmax(p / Exp(1))
-// Class ownership inside a warp: lane l holds classes 4l..4l+3 (one float4 of logits, one Philox block) and class 128+l.
+// Class ownership inside a warp (lane_classes): lane l holds classes 4l..4l+3 (one float4 of logits, one Philox block) and
+// class 128+l; TokenNoise::lane_words draws the noise words of exactly these classes.
 #pragma once
 #include "common.cuh"
 #include "embed.cuh"
@@ -74,59 +75,99 @@ LDM_DEVINL void embed_next(const StepParams& p, const int b, const int s, const 
   else embed_token_row<false>(best_c, s, row, p.emb_cat, p.emb_pos, p.emb_adaln, p.emb_x32, p.emb_x16, p.emb_d, lane);
 }
 
-// predict_start (base.py:127-146) for one token: float64 log-softmax over the C-1 non-MASK classes, MASK = -70, clamp [-70, 0].
-// Class ownership: lane l holds classes 4l..4l+3 and 128+l.
-LDM_DEVINL void predict_start_token(const StepParams& p, const float* lrow, const int lane, const int (&cls)[5], const bool (&valid)[5], float (&lx0)[5]) {
-  const int C = p.C;
-  float l[5];
-  {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(lrow) + lane);
-    l[0] = v.x; l[1] = v.y; l[2] = v.z; l[3] = v.w;
-    l[4] = valid[4] ? __ldg(lrow + cls[4]) : 0.0f;
+LDM_DEVINL void lane_classes(const int C, const int lane, int (&cls)[5], bool (&valid)[5]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { cls[j] = 4 * lane + j; valid[j] = cls[j] < C; }
+  cls[4] = 128 + lane; valid[4] = cls[4] < C;
+}
+
+// the vocabulary group of token position s: its attribute for the constrained diffusion, the single group 0 for vanilla
+LDM_DEVINL int vocab_group(const StepParams& p, const int s) { return p.constrained ? s % p.n_attr : 0; }
+
+// class c belongs to group g (Converter f_to_p_log): the attribute's own classes plus PAD and MASK; for vanilla every class
+LDM_DEVINL bool in_group(const StepParams& p, const int g, const int c) {
+  return !p.constrained || (c >= p.grp_start[g] && c < p.grp_start[g] + p.grp_n[g]) || c == p.pad_id || c == p.mask_id;
+}
+
+// argmax over the classes the warp holds in N slots per lane, first (smallest) class on ties; slots with on[j] false take no part
+template <int N>
+LDM_DEVINL int warp_argmax_first(const float (&v)[N], const int (&cls)[N], const bool (&on)[N]) {
+  float best = -INFINITY; int best_c = 0x7fffffff;
+#pragma unroll
+  for (int j = 0; j < N; ++j) if (on[j] && (v[j] > best || (v[j] == best && cls[j] < best_c))) { best = v[j]; best_c = cls[j]; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
+    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
   }
+  return best_c;
+}
+
+// the noise of token (b, s) of this call, with the captured graph's {seed, b_global0} override (StepParams::call) resolved
+LDM_DEVINL TokenNoise step_noise(const StepParams& p, const int b, const int s) {
+  const unsigned long long seed = p.call ? __ldg(p.call) : p.seed, bg0 = p.call ? __ldg(p.call + 1) : static_cast<unsigned long long>(p.b_global0);
+  return TokenNoise(seed, bg0, b, p.S, s);
+}
+
+// predict_start (base.py:127-146): the float64 log-sum-exp over the C-1 non-MASK logits of one token's row (lane classes);
+// l receives the lane's logits.  lx0_of maps a logit to log p(x0), clamped to [-70, 0].
+LDM_DEVINL double logit_lse(const StepParams& p, const float* lrow, const int lane, const int (&cls)[5], const bool (&valid)[5], float (&l)[5]) {
+  const float4 v = __ldg(reinterpret_cast<const float4*>(lrow) + lane);
+  l[0] = v.x; l[1] = v.y; l[2] = v.z; l[3] = v.w;
+  l[4] = valid[4] ? __ldg(lrow + cls[4]) : 0.0f;
   float mx = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < 5; ++j) if (valid[j] && cls[j] < C - 1) mx = fmaxf(mx, l[j]);
+  for (int j = 0; j < 5; ++j) if (valid[j] && cls[j] < p.C - 1) mx = fmaxf(mx, l[j]);
   mx = warp_max(mx);
   double dsum = 0.0;
 #pragma unroll
-  for (int j = 0; j < 5; ++j) if (valid[j] && cls[j] < C - 1) dsum += exp(static_cast<double>(l[j]) - static_cast<double>(mx));
+  for (int j = 0; j < 5; ++j) if (valid[j] && cls[j] < p.C - 1) dsum += exp(static_cast<double>(l[j]) - static_cast<double>(mx));
   dsum = warp_sum_d(dsum);
-  const double lse = static_cast<double>(mx) + log(dsum);
-#pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    const float v = (cls[j] < C - 1) ? static_cast<float>(static_cast<double>(l[j]) - lse) : -70.0f;
-    lx0[j] = fminf(fmaxf(v, -70.0f), 0.0f);
-  }
+  return static_cast<double>(mx) + log(dsum);
+}
+LDM_DEVINL float lx0_of(const float logit, const double lse) {
+  return fminf(fmaxf(static_cast<float>(static_cast<double>(logit) - lse), -70.0f), 0.0f);
 }
 
-// q(x_{t-1} | x_t, x0~) in log space for one token, every class (constrained.py:135-206 / vanilla.py:112-151): lx0 = log p(x0)
-// (its MASK entry is not used), x_t the token's current id, t the posterior timestep; classes outside the token's vocabulary
-// group come out as log(1e-30) (Converter.p_to_f_log), invalid lanes as -inf.
-LDM_DEVINL void posterior_token_logprob(const StepParams& p, const int s, const int x_t, const int t, const float (&lx0)[5],
-                                        const int (&cls)[5], const bool (&valid)[5], float (&lp)[5]) {
-  const int g = p.constrained ? (s % p.n_attr) : 0;
-  const int gst = p.grp_start[g], gn = p.grp_n[g];
-  const float* tab = p.sched + static_cast<size_t>(g) * 8 * (p.T + 1);
-  const int tm1 = (t - 1 + (p.T + 1)) % (p.T + 1);
-  const int TT = p.T + 1;
-  const float lat = tab[0 * TT + t], lbt = tab[1 * TT + t], lct = tab[2 * TT + t];
-  const float lcat = tab[3 * TT + t], lcbt = tab[4 * TT + t], lcct = tab[5 * TT + t];
-  const float lcat1 = tab[3 * TT + tm1], lcbt1 = tab[4 * TT + tm1], lcct1 = tab[5 * TT + tm1], l1mcct1 = tab[7 * TT + tm1];
-  const bool is_mask = (x_t == p.mask_id);
+// predict_start for one token, every class (lane classes): MASK = -70
+LDM_DEVINL void predict_start_token(const StepParams& p, const float* lrow, const int lane, const int (&cls)[5], const bool (&valid)[5], float (&lx0)[5]) {
+  float l[5];
+  const double lse = logit_lse(p, lrow, lane, cls, valid, l);
+#pragma unroll
+  for (int j = 0; j < 5; ++j) lx0[j] = (cls[j] < p.C - 1) ? lx0_of(l[j], lse) : -70.0f;
+}
 
-  bool in_grp[5]; float q[5], one[5];
+// The schedule terms of q_posterior at (group g, posterior timestep t): the log_add_exp terms of the lae table, lct / lcct at t,
+// and the entries at t-1 (t = 0 wraps to T).
+struct PostTerms { float4 lae; float lct, lcct, lcat1, lcbt1, lcct1, l1mcct1; };
+LDM_DEVINL PostTerms post_terms(const StepParams& p, const int g, const int t) {
+  const int TT = p.T + 1, tm1 = (t - 1 + TT) % TT;
+  const float* tab = p.sched + static_cast<size_t>(g) * 8 * TT;
+  PostTerms k;
+  k.lae = __ldg(reinterpret_cast<const float4*>(p.lae) + static_cast<size_t>(g) * TT + t);
+  k.lct = tab[2 * TT + t]; k.lcct = tab[5 * TT + t];
+  k.lcat1 = tab[3 * TT + tm1]; k.lcbt1 = tab[4 * TT + tm1]; k.lcct1 = tab[5 * TT + tm1]; k.l1mcct1 = tab[7 * TT + tm1];
+  return k;
+}
+
+// q(x_{t-1} | x_t, x0~) in log space (constrained.py:135-206 / vanilla.py:112-151) for the classes a warp holds in N slots per
+// lane: lx0 = log p(x0) (its MASK entry is not used), x_t the token's current id.  The normalisation runs over the slots with
+// in_grp[j]; only their lp[j] are written.
+template <int N>
+LDM_DEVINL void posterior_logprob(const StepParams& p, const PostTerms& k, const int x_t, const float (&lx0)[N], const int (&cls)[N],
+                                  const bool (&in_grp)[N], float (&lp)[N]) {
+  const bool is_mask = (x_t == p.mask_id);
+  float q[N], one[N];
   float qmax = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    const int c = cls[j];
-    in_grp[j] = valid[j] && (p.constrained ? ((c >= gst && c < gst + gn) || c == p.pad_id || c == p.mask_id) : true);
+  for (int j = 0; j < N; ++j) {
     q[j] = -INFINITY; one[j] = 0.0f;
     if (in_grp[j]) {
-      if (c != p.mask_id) {
-        const float v = (c == x_t) ? 0.0f : kLogEps;
-        const float lq = is_mask ? lcct : log_add_exp(v + lcat, lcbt);
-        one[j] = is_mask ? lct : log_add_exp(v + lat, lbt);
+      if (cls[j] != p.mask_id) {
+        const bool same = (cls[j] == x_t);
+        const float lq = is_mask ? k.lcct : (same ? k.lae.x : k.lae.y);      // = log_add_exp(v + lcat, lcbt), v = 0 / log eps
+        one[j] = is_mask ? k.lct : (same ? k.lae.z : k.lae.w);               // = log_add_exp(v + lat, lbt)
         q[j] = lx0[j] - lq;
       } else {
         q[j] = kLogEps;
@@ -138,28 +179,64 @@ LDM_DEVINL void posterior_token_logprob(const StepParams& p, const int s, const 
   qmax = warp_max(qmax);
   float qs = 0.0f;
 #pragma unroll
-  for (int j = 0; j < 5; ++j) if (in_grp[j]) qs += expf(q[j] - qmax);
+  for (int j = 0; j < N; ++j) if (in_grp[j]) qs += expf(q[j] - qmax);
   const float L = logf(warp_sum(qs)) + qmax;
 #pragma unroll
-  for (int j = 0; j < 5; ++j) {
+  for (int j = 0; j < N; ++j) {
     if (in_grp[j]) {
       const float qn = q[j] - L;
-      const float ev = (cls[j] != p.mask_id) ? log_add_exp(qn + lcat1, lcbt1) : log_add_exp(qn + l1mcct1, lcct1);
+      const float ev = (cls[j] != p.mask_id) ? log_add_exp(qn + k.lcat1, k.lcbt1) : log_add_exp(qn + k.l1mcct1, k.lcct1);
       lp[j] = fminf(fmaxf((ev + one[j]) + L, -70.0f), 0.0f);
-    } else {
-      lp[j] = valid[j] ? kLogEps : -INFINITY;
     }
   }
 }
 
-// One token, every class (lane l: classes 4l..4l+3 and 128+l): any q_type, any sampling mode, log-prob in / out.
+// The posterior for one token, every class (lane classes), t the posterior timestep: classes outside the token's vocabulary
+// group come out as log(1e-30) (Converter.p_to_f_log), invalid lanes as -inf.
+LDM_DEVINL void posterior_token_logprob(const StepParams& p, const int s, const int x_t, const int t, const float (&lx0)[5],
+                                        const int (&cls)[5], const bool (&valid)[5], float (&lp)[5]) {
+  const int g = vocab_group(p, s);
+  bool in_grp[5];
+#pragma unroll
+  for (int j = 0; j < 5; ++j) { in_grp[j] = valid[j] && in_group(p, g, cls[j]); lp[j] = valid[j] ? kLogEps : -INFINITY; }
+  posterior_logprob<5>(p, post_terms(p, g, t), x_t, lx0, cls, in_grp, lp);
+}
+
+// The draw from lg = log-probs / temperature (top-k / top-p already applied), the same for any slot layout: Gumbel noise for
+// name="gumbel" (stream 1), then probs = softmax(lg) and multinomial(probs, 1) = argmax(probs / e), e ~ Exp(1) (stream 0).
+// words(stream, w) returns the noise words of the lane's N slots.
+template <int N, class Words>
+LDM_DEVINL int draw_class(const StepParams& p, float (&lg)[N], const int (&cls)[N], const bool (&on)[N], Words words) {
+  uint32_t w[N];
+  if (p.mode == SAMP_GUMBEL) {
+    words(1u, w);
+#pragma unroll
+    for (int j = 0; j < N; ++j) lg[j] += gumbel_of(u01_from_bits(w[j]));
+  }
+  float m = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < N; ++j) m = fmaxf(m, lg[j]);
+  m = warp_max(m);
+  float ex[N], sm = 0.0f;
+#pragma unroll
+  for (int j = 0; j < N; ++j) { ex[j] = on[j] ? expf(lg[j] - m) : 0.0f; sm += ex[j]; }
+  sm = warp_sum(sm);
+  words(0u, w);
+  float score[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    const float e = -logf(u01_from_bits(w[j]));
+    score[j] = on[j] ? (ex[j] / sm) / e : -INFINITY;
+  }
+  return warp_argmax_first<N>(score, cls, on);
+}
+
+// One token, every class (lane classes): any q_type, any sampling mode, log-prob in / out.
 LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, const int lane) {
   const int b = token / p.S, s = token % p.S;
   const int C = p.C;
   int cls[5]; bool valid[5];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) { cls[j] = 4 * lane + j; valid[j] = cls[j] < C; }
-  cls[4] = 128 + lane; valid[4] = cls[4] < C;
+  lane_classes(C, lane, cls, valid);
 
   const int x_t = static_cast<int>(p.ids_in[token]);
   float lp[5];
@@ -214,20 +291,13 @@ LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, co
   if (p.ids_out == nullptr) return;        // log-probabilities only (q_posterior / predict_start as callable APIs)
 
   // ---- draw ----
-  float score[5];
+  int best_c;
   if (p.mode == SAMP_DETERMINISTIC) {
-#pragma unroll
-    for (int j = 0; j < 5; ++j) score[j] = valid[j] ? lp[j] : -INFINITY;
+    best_c = warp_argmax_first<5>(lp, cls, valid);
   } else {
     float lg[5];
 #pragma unroll
     for (int j = 0; j < 5; ++j) lg[j] = valid[j] ? lp[j] / p.temperature : -INFINITY;
-
-    const unsigned long long seed = p.call ? __ldg(p.call) : p.seed, bg0 = p.call ? __ldg(p.call + 1) : static_cast<unsigned long long>(p.b_global0);
-    const unsigned long long tok = (bg0 + b) * static_cast<unsigned long long>(p.S) + s;
-    const uint2 key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
-    const uint32_t tok_lo = static_cast<uint32_t>(tok), tok_hi = static_cast<uint32_t>(tok >> 32);
-    const uint32_t w1 = p.step_ctr & 0xFFFFFFu;
 
     if (p.mode == SAMP_TOP_K || p.mode == SAMP_TOP_P) {
       float pr[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -276,47 +346,9 @@ LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, co
 #pragma unroll
         for (int j = 0; j < 5; ++j) if (valid[j] && lg[j] < thr) lg[j] = -INFINITY;
       }
-    } else if (p.mode == SAMP_GUMBEL) {
-      const uint4 ga = philox4x32_10(make_uint4(static_cast<uint32_t>(lane), w1 | (1u << 24), tok_lo, tok_hi), key);
-      const uint4 gb = philox4x32_10(make_uint4(32u + (static_cast<uint32_t>(lane) >> 2), w1 | (1u << 24), tok_lo, tok_hi), key);
-      const uint32_t gw[5] = {ga.x, ga.y, ga.z, ga.w, (lane & 3) == 0 ? gb.x : (lane & 3) == 1 ? gb.y : (lane & 3) == 2 ? gb.z : gb.w};
-#pragma unroll
-      for (int j = 0; j < 5; ++j) {
-        const float u = u01_from_bits(gw[j]);
-        lg[j] += -logf(-logf(u + 1e-30f) + 1e-30f);           // sampling.py:112-116
-      }
     }
-
-    // probs = softmax(lg) ; multinomial(probs, 1) = argmax(probs / e), e ~ Exp(1)
-    float m = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) m = fmaxf(m, lg[j]);
-    m = warp_max(m);
-    float ex[5], sm = 0.0f;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) { ex[j] = valid[j] ? expf(lg[j] - m) : 0.0f; sm += ex[j]; }
-    sm = warp_sum(sm);
-    const uint4 ra = philox4x32_10(make_uint4(static_cast<uint32_t>(lane), w1, tok_lo, tok_hi), key);
-    const uint4 rb = philox4x32_10(make_uint4(32u + (static_cast<uint32_t>(lane) >> 2), w1, tok_lo, tok_hi), key);
-    const uint32_t rw[5] = {ra.x, ra.y, ra.z, ra.w, (lane & 3) == 0 ? rb.x : (lane & 3) == 1 ? rb.y : (lane & 3) == 2 ? rb.z : rb.w};
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-      const float e = -logf(u01_from_bits(rw[j]));
-      score[j] = valid[j] ? (ex[j] / sm) / e : -INFINITY;
-    }
-  }
-
-  // argmax with first-index tie break
-  float best = -INFINITY; int best_c = 0x7fffffff;
-#pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    if (valid[j] && (score[j] > best || (score[j] == best && cls[j] < best_c))) { best = score[j]; best_c = cls[j]; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
-    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
+    const TokenNoise nz = step_noise(p, b, s);
+    best_c = draw_class<5>(p, lg, cls, valid, [&](uint32_t stream, uint32_t (&w)[5]) { nz.lane_words(lane, noise_ctr(p.step_ctr, stream), w); });
   }
   if (lane == 0) p.ids_out[token] = best_c;
   embed_next(p, b, s, best_c, lane);
@@ -351,34 +383,15 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
     fixed = (p.cond_flags & COND_HAS_MASK) && p.cond_mask[token];
   }
 
-  // ---- predict_start: float64 log-sum-exp over the C-1 non-MASK logits (lane l: classes 4l..4l+3, 128+l) ----
+  // ---- predict_start: the log-sum-exp over all classes, log p(x0) of the group's ----
   const float* lrow = p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits;
-  double lse;
-  {
-    float l[5];
-    const float4 v = __ldg(reinterpret_cast<const float4*>(lrow) + lane);
-    l[0] = v.x; l[1] = v.y; l[2] = v.z; l[3] = v.w;
-    l[4] = (128 + lane < C) ? __ldg(lrow + 128 + lane) : 0.0f;
-    float mx = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) { const int c = j < 4 ? 4 * lane + j : 128 + lane; if (c < C - 1) mx = fmaxf(mx, l[j]); }
-    mx = warp_max(mx);
-    double dsum = 0.0;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) { const int c = j < 4 ? 4 * lane + j : 128 + lane; if (c < C - 1) dsum += exp(static_cast<double>(l[j]) - static_cast<double>(mx)); }
-    dsum = warp_sum_d(dsum);
-    lse = static_cast<double>(mx) + log(dsum);
-  }
+  int lcls[5]; bool lvalid[5];
+  lane_classes(C, lane, lcls, lvalid);
+  float l[5];
+  const double lse = logit_lse(p, lrow, lane, lcls, lvalid, l);
 
-  const int g = s % p.n_attr;
+  const int g = vocab_group(p, s);
   const int gst = p.grp_start[g], gn = p.grp_n[g];
-  const float* tab = p.sched + static_cast<size_t>(g) * 8 * (p.T + 1);
-  const int t = p.t_post, tm1 = (t - 1 + (p.T + 1)) % (p.T + 1);
-  const int TT = p.T + 1;
-  const float lct = tab[2 * TT + t], lcct = tab[5 * TT + t];
-  const float lcat1 = tab[3 * TT + tm1], lcbt1 = tab[4 * TT + tm1], lcct1 = tab[5 * TT + tm1], l1mcct1 = tab[7 * TT + tm1];
-  const bool is_mask = (x_t == p.mask_id);
-  const float4 lae = __ldg(reinterpret_cast<const float4*>(p.lae) + static_cast<size_t>(g) * TT + t);
   const bool refine = (p.cond_flags & COND_REFINE) && !fixed;
   const float* trow = refine ? p.refine_tbl + static_cast<size_t>(p.cond_seq_orig[token]) * C : nullptr;
 
@@ -386,39 +399,14 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
   int cls[2]; bool on[2];
   cls[0] = gst + lane; on[0] = lane < gn;
   cls[1] = lane == 0 ? p.pad_id : p.mask_id; on[1] = lane < 2;
-  float q[2], one[2], lp[2];
-  float qmax = -INFINITY;
+  float lx0[2], lp[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    q[j] = -INFINITY; one[j] = 0.0f;
-    if (on[j]) {
-      const int c = cls[j];
-      if (c != p.mask_id) {
-        const float lx0 = fminf(fmaxf(static_cast<float>(static_cast<double>(__ldg(lrow + c)) - lse), -70.0f), 0.0f);
-        const bool same = (c == x_t);
-        const float lq = is_mask ? lcct : (same ? lae.x : lae.y);          // = log_add_exp(v + lcat, lcbt), v = 0 / log eps
-        one[j] = is_mask ? lct : (same ? lae.z : lae.w);                   // = log_add_exp(v + lat, lbt)
-        q[j] = lx0 - lq;
-      } else {
-        q[j] = kLogEps;
-        one[j] = is_mask ? 0.0f : kLogEps;
-      }
-      qmax = fmaxf(qmax, q[j]);
-    }
-  }
-  qmax = warp_max(qmax);
-  float qs = 0.0f;
-#pragma unroll
-  for (int j = 0; j < 2; ++j) if (on[j]) qs += expf(q[j] - qmax);
-  const float L = logf(warp_sum(qs)) + qmax;
+  for (int j = 0; j < 2; ++j) lx0[j] = (on[j] && cls[j] != p.mask_id) ? lx0_of(__ldg(lrow + cls[j]), lse) : 0.0f;
+  posterior_logprob<2>(p, post_terms(p, g, p.t_post), x_t, lx0, cls, on, lp);
   float lmax = -INFINITY;
 #pragma unroll
   for (int j = 0; j < 2; ++j) {
-    lp[j] = -INFINITY;
     if (on[j]) {
-      const float qn = q[j] - L;
-      const float ev = (cls[j] != p.mask_id) ? log_add_exp(qn + lcat1, lcbt1) : log_add_exp(qn + l1mcct1, lcct1);
-      lp[j] = fminf(fmaxf((ev + one[j]) + L, -70.0f), 0.0f);
       if (fixed) lp[j] = (cls[j] == cs) ? 0.0f : kLogEps;
       if (refine) lp[j] += __ldg(trow + cls[j]);
       if ((p.cond_flags & COND_PAD_DISABLE) && (s % p.n_attr != 0) && cs != p.pad_id && cls[j] == p.pad_id) lp[j] = kLogEps;
@@ -431,20 +419,16 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
     // above log(1e-30); a caller-supplied table that does sends the token to the all-classes routine
     float tmax = 0.0f;
 #pragma unroll
-    for (int j = 0; j < 5; ++j) {
-      const int c = j < 4 ? 4 * lane + j : 128 + lane;
-      const bool in_grp = (c >= gst && c < gst + gn) || c == p.pad_id || c == p.mask_id;
-      if (c < C && !in_grp) tmax = fmaxf(tmax, __ldg(trow + c));
-    }
+    for (int j = 0; j < 5; ++j) if (lvalid[j] && !in_group(p, g, lcls[j])) tmax = fmaxf(tmax, __ldg(trow + lcls[j]));
     if (warp_max(tmax) > 0.0f) { posterior_token_generic(p, token, lane); return; }
   }
   // every class outside the group sits at log(1e-30): it must be out of reach of the draw (see the header comment)
   const float margin = p.mode == SAMP_DETERMINISTIC ? 0.0f : 40.0f * p.temperature;
   if (!(lmax - kLogEps > margin)) { posterior_token_generic(p, token, lane); return; }
 
-  float score[2];
+  int best_c;
   if (p.mode == SAMP_DETERMINISTIC) {
-    score[0] = lp[0]; score[1] = lp[1];
+    best_c = warp_argmax_first<2>(lp, cls, on);
   } else {
     float lg[2];
 #pragma unroll
@@ -478,61 +462,33 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
 #pragma unroll
       for (int j = 0; j < 2; ++j) if (on[j] && n_before[j] > 0 && static_cast<float>(cum[j]) > p.top_p) lg[j] = -INFINITY;
     }
-    const unsigned long long seed = p.call ? __ldg(p.call) : p.seed, bg0 = p.call ? __ldg(p.call + 1) : static_cast<unsigned long long>(p.b_global0);
-    const unsigned long long tok = (bg0 + b) * static_cast<unsigned long long>(p.S) + s;
-    const uint2 key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
-    const uint32_t tok_lo = static_cast<uint32_t>(tok), tok_hi = static_cast<uint32_t>(tok >> 32);
-    const uint32_t w1 = p.step_ctr & 0xFFFFFFu;
-    // class c draws word c % 4 of Philox block c / 4.  One evaluation per noise stream serves the whole token: lanes 0..8
-    // compute the (at most 9) blocks of the group, lanes 9 / 10 the blocks of PAD / MASK, then every lane fetches its words.
-    const int b0 = gst >> 2;
-    const int my_block = lane < 9 ? b0 + lane : (lane == 9 ? (p.pad_id >> 2) : (p.mask_id >> 2));
-    const int src0 = (cls[0] >> 2) - b0, src1 = lane == 0 ? 9 : 10;
-    auto noise_words = [&](uint32_t stream, uint32_t (&w)[2]) {
-      const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(my_block), w1 | (stream << 24), tok_lo, tok_hi), key);
+    // One Philox evaluation per noise stream serves the whole token: lanes 0..8 compute the (at most 9) blocks of the group,
+    // lanes 9 / 10 the blocks of PAD / MASK, then every lane fetches its words.
+    const TokenNoise nz = step_noise(p, b, s);
+    const int b0 = TokenNoise::block_of(gst);
+    const int my_block = lane < 9 ? b0 + lane : TokenNoise::block_of(lane == 9 ? p.pad_id : p.mask_id);
+    const int src0 = TokenNoise::block_of(cls[0]) - b0, src1 = lane == 0 ? 9 : 10;
+    best_c = draw_class<2>(p, lg, cls, on, [&](uint32_t stream, uint32_t (&w)[2]) {
+      const uint4 r = nz.block(my_block, noise_ctr(p.step_ctr, stream));
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         const int src = j == 0 ? src0 : src1;
-        const uint32_t x = __shfl_sync(0xffffffffu, r.x, src), y = __shfl_sync(0xffffffffu, r.y, src);
-        const uint32_t z = __shfl_sync(0xffffffffu, r.z, src), ww = __shfl_sync(0xffffffffu, r.w, src);
-        const int k = cls[j] & 3;
-        w[j] = k == 0 ? x : k == 1 ? y : k == 2 ? z : ww;
+        const uint4 rs = make_uint4(__shfl_sync(0xffffffffu, r.x, src), __shfl_sync(0xffffffffu, r.y, src),
+                                    __shfl_sync(0xffffffffu, r.z, src), __shfl_sync(0xffffffffu, r.w, src));
+        w[j] = TokenNoise::word_of(rs, cls[j]);
       }
-    };
-    if (p.mode == SAMP_GUMBEL) {
-      uint32_t gw[2];
-      noise_words(1u, gw);
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const float u = u01_from_bits(gw[j]);
-        if (on[j]) lg[j] += -logf(-logf(u + 1e-30f) + 1e-30f);
-      }
-    }
-    float m = warp_max(fmaxf(lg[0], lg[1]));
-    float ex[2], sm = 0.0f;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) { ex[j] = on[j] ? expf(lg[j] - m) : 0.0f; sm += ex[j]; }
-    sm = warp_sum(sm);
-    uint32_t rw[2];
-    noise_words(0u, rw);
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const float e = -logf(u01_from_bits(rw[j]));
-      score[j] = on[j] ? (ex[j] / sm) / e : -INFINITY;
-    }
-  }
-  float best = -INFINITY; int best_c = 0x7fffffff;
-#pragma unroll
-  for (int j = 0; j < 2; ++j)
-    if (on[j] && (score[j] > best || (score[j] == best && cls[j] < best_c))) { best = score[j]; best_c = cls[j]; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
-    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
+    });
   }
   if (lane == 0) p.ids_out[token] = best_c;
   embed_next(p, b, s, best_c, lane);
+}
+
+// the preconditions of posterior_sample_group_kernel (its header comment)
+inline bool group_kernel_applies(const StepParams& p) {
+  bool ok = p.constrained && p.logprob_in == nullptr && p.logprob_out == nullptr &&
+            (p.mode == SAMP_DETERMINISTIC || p.mode == SAMP_RANDOM || p.mode == SAMP_GUMBEL || (p.mode == SAMP_TOP_P && p.top_p < 0.9999f));
+  for (int g = 0; g < p.n_attr; ++g) ok = ok && p.grp_n[g] <= 32;
+  return ok;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -552,19 +508,6 @@ struct VbParams {
   long long* x0_recon; long long* xtm1_recon;      // [n_layouts][S] or nullptr
 };
 
-LDM_DEVINL int warp_argmax_first(float v[5], const int (&cls)[5], const bool (&valid)[5]) {
-  float best = -INFINITY; int best_c = 0x7fffffff;
-#pragma unroll
-  for (int j = 0; j < 5; ++j) if (valid[j] && (v[j] > best || (v[j] == best && cls[j] < best_c))) { best = v[j]; best_c = cls[j]; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
-    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
-  }
-  return best_c;
-}
-
 __global__ void __launch_bounds__(256) vb_terms_kernel(const VbParams v) {
   const StepParams& p = v.sp;
   const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -573,18 +516,16 @@ __global__ void __launch_bounds__(256) vb_terms_kernel(const VbParams v) {
   const int b = token / p.S, s = token % p.S;
   const int C = p.C;
   int cls[5]; bool valid[5];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) { cls[j] = 4 * lane + j; valid[j] = cls[j] < C; }
-  cls[4] = 128 + lane; valid[4] = cls[4] < C;
+  lane_classes(C, lane, cls, valid);
   const int x_t = static_cast<int>(p.ids_in[token]);
   const int x0 = static_cast<int>(v.x0[token]);
   const int t = __ldg(p.t_layout + b);
   float lx0[5], lmp[5], lxs[5], ltp[5];
-  predict_start_token(p, p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits, lane, cls, valid, lx0);
-  posterior_token_logprob(p, s, x_t, t, lx0, cls, valid, lmp);
 #pragma unroll
   for (int j = 0; j < 5; ++j) lxs[j] = (cls[j] == x0) ? 0.0f : kLogEps;            // index_to_log_onehot (util.py:34-40)
   posterior_token_logprob(p, s, x_t, t, lxs, cls, valid, ltp);
+  predict_start_token(p, p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits, lane, cls, valid, lx0);
+  posterior_token_logprob(p, s, x_t, t, lx0, cls, valid, lmp);
   float kl = 0.0f, nll = 0.0f, aux = 0.0f;
 #pragma unroll
   for (int j = 0; j < 5; ++j) {
@@ -600,8 +541,8 @@ __global__ void __launch_bounds__(256) vb_terms_kernel(const VbParams v) {
 #pragma unroll
     for (int j = 0; j < 5; ++j) if (valid[j]) p.logprob_out[static_cast<size_t>(token) * C + cls[j]] = lmp[j];
   }
-  const int a0 = v.x0_recon ? warp_argmax_first(lx0, cls, valid) : 0;
-  const int a1 = v.xtm1_recon ? warp_argmax_first(lmp, cls, valid) : 0;
+  const int a0 = v.x0_recon ? warp_argmax_first<5>(lx0, cls, valid) : 0;
+  const int a1 = v.xtm1_recon ? warp_argmax_first<5>(lmp, cls, valid) : 0;
   if (lane == 0) {
     v.kl_tok[token] = kl * w; v.nll_tok[token] = nll;
     if (v.aux_tok) v.aux_tok[token] = aux * w;
@@ -629,11 +570,9 @@ __global__ void q_pred_kernel(const StepParams p, const float* __restrict__ lx, 
   const size_t n = static_cast<size_t>(p.n_layouts) * p.S * p.C;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % p.C); const size_t tok = i / p.C; const int s = static_cast<int>(tok % p.S); const int b = static_cast<int>(tok / p.S);
-    const int g = p.constrained ? (s % p.n_attr) : 0;
-    const int gst = p.grp_start[g], gn = p.grp_n[g];
-    const bool in_grp = p.constrained ? ((c >= gst && c < gst + gn) || c == p.pad_id || c == p.mask_id) : true;
+    const int g = vocab_group(p, s);
     float r = kLogEps;
-    if (in_grp) {
+    if (in_group(p, g, c)) {
       const int TT = p.T + 1;
       const int t = (__ldg(p.t_layout + b) + TT) % TT;
       const float* tab = p.sched + static_cast<size_t>(g) * 8 * TT;
@@ -652,29 +591,18 @@ __global__ void __launch_bounds__(256) gumbel_argmax_kernel(const float* __restr
   const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (token >= n_layouts * S) return;
   const int b = token / S, s = token % S;
-  const unsigned long long tok = (static_cast<unsigned long long>(b_global0) + b) * static_cast<unsigned long long>(S) + s;
-  const uint2 key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
-  const uint32_t tok_lo = static_cast<uint32_t>(tok), tok_hi = static_cast<uint32_t>(tok >> 32);
-  const uint4 ga = philox4x32_10(make_uint4(static_cast<uint32_t>(lane), 2u << 24, tok_lo, tok_hi), key);
-  const uint4 gb = philox4x32_10(make_uint4(32u + (static_cast<uint32_t>(lane) >> 2), 2u << 24, tok_lo, tok_hi), key);
-  const uint32_t gw[5] = {ga.x, ga.y, ga.z, ga.w, (lane & 3) == 0 ? gb.x : (lane & 3) == 1 ? gb.y : (lane & 3) == 2 ? gb.z : gb.w};
-  float best = -INFINITY; int best_c = 0x7fffffff;
+  int cls[5]; bool on[5];
+  lane_classes(C, lane, cls, on);
+  uint32_t w[5];
+  TokenNoise(seed, b_global0, b, S, s).lane_words(lane, noise_ctr(0, 2), w);
+  float score[5];
 #pragma unroll
   for (int j = 0; j < 5; ++j) {
-    const int c = j < 4 ? 4 * lane + j : 128 + lane;
-    if (c >= C) continue;
-    const float l = logits[static_cast<size_t>(token) * C + c];
-    if (!(l > -INFINITY)) continue;
-    const float u = u01_from_bits(gw[j]);
-    const float score = l + (-logf(-logf(u + 1e-30f) + 1e-30f));
-    if (score > best || (score == best && c < best_c)) { best = score; best_c = c; }
+    const float l = on[j] ? logits[static_cast<size_t>(token) * C + cls[j]] : -INFINITY;
+    on[j] = l > -INFINITY;
+    score[j] = on[j] ? l + gumbel_of(u01_from_bits(w[j])) : -INFINITY;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
-    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
-  }
+  const int best_c = warp_argmax_first<5>(score, cls, on);
   if (lane == 0) ids_out[token] = best_c;
 }
 
@@ -683,54 +611,32 @@ __global__ void __launch_bounds__(256) gumbel_argmax_kernel(const float* __restr
 // q_pred  T/models/categorical_diffusion/constrained.py:112-133 (vanilla.py:90-110), log_sample_categorical :208-221,
 // q_sample :223-230; the training forward applies it per attribute on the partial vocabularies (:232-260) -- here per token
 // on the full ids (classes outside the token's group are impossible).  One warp per token, same class ownership as above.
-struct QSampleParams {
-  int n_layouts, S, C, n_attr, pad_id, mask_id, constrained;
-  int grp_start[kMaxAttr], grp_n[kMaxAttr];
-  int T;
-  const float* sched;                    // [G][8][T+1]
-  const long long* x0;                   // [n_layouts][S]
-  const int* t;                          // [n_layouts]
-  unsigned long long seed; long long b_global0;
-  long long* xt;                         // [n_layouts][S]
-};
-
-__global__ void __launch_bounds__(256) q_sample_kernel(const QSampleParams p) {
+__global__ void __launch_bounds__(256) q_sample_kernel(const StepParams p, const long long* __restrict__ x0, const int* __restrict__ t,
+                                                       long long* __restrict__ xt) {
   const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (token >= p.n_layouts * p.S) return;
   const int b = token / p.S, s = token % p.S;
-  const int C = p.C;
-  const int x0 = static_cast<int>(p.x0[token]);
-  const int t = p.t[b];
-  const int g = p.constrained ? (s % p.n_attr) : 0;
-  const int gst = p.grp_start[g], gn = p.grp_n[g];
+  const int x0_id = static_cast<int>(x0[token]);
+  const int tb = t[b];
+  const int g = vocab_group(p, s);
   const int TT = p.T + 1;
   const float* tab = p.sched + static_cast<size_t>(g) * 8 * TT;
-  const float lcat = tab[3 * TT + t], lcbt = tab[4 * TT + t], lcct = tab[5 * TT + t], l1m = tab[7 * TT + t];
-  const unsigned long long tok = (static_cast<unsigned long long>(p.b_global0) + b) * static_cast<unsigned long long>(p.S) + s;
-  const uint2 key = make_uint2(static_cast<uint32_t>(p.seed), static_cast<uint32_t>(p.seed >> 32));
-  const uint32_t tok_lo = static_cast<uint32_t>(tok), tok_hi = static_cast<uint32_t>(tok >> 32);
-  const uint4 ga = philox4x32_10(make_uint4(static_cast<uint32_t>(lane), 2u << 24, tok_lo, tok_hi), key);
-  const uint4 gb = philox4x32_10(make_uint4(32u + (static_cast<uint32_t>(lane) >> 2), 2u << 24, tok_lo, tok_hi), key);
-  const uint32_t gw[5] = {ga.x, ga.y, ga.z, ga.w, (lane & 3) == 0 ? gb.x : (lane & 3) == 1 ? gb.y : (lane & 3) == 2 ? gb.z : gb.w};
-  float best = -INFINITY; int best_c = 0x7fffffff;
+  const float lcat = tab[3 * TT + tb], lcbt = tab[4 * TT + tb], lcct = tab[5 * TT + tb], l1m = tab[7 * TT + tb];
+  int cls[5]; bool on[5];
+  lane_classes(p.C, lane, cls, on);
+  uint32_t w[5];
+  TokenNoise(p.seed, p.b_global0, b, p.S, s).lane_words(lane, noise_ctr(0, 2), w);
+  float score[5];
 #pragma unroll
   for (int j = 0; j < 5; ++j) {
-    const int c = j < 4 ? 4 * lane + j : 128 + lane;
-    const bool in_grp = c < C && (p.constrained ? ((c >= gst && c < gst + gn) || c == p.pad_id || c == p.mask_id) : true);
-    if (!in_grp) continue;
-    const float v = (c == x0) ? 0.0f : kLogEps;                          // log(clamp(onehot, 1e-30))
+    const int c = cls[j];
+    on[j] = on[j] && in_group(p, g, c);
+    const float v = (c == x0_id) ? 0.0f : kLogEps;                       // log(clamp(onehot, 1e-30))
     const float logit = (c != p.mask_id) ? log_add_exp(v + lcat, lcbt) : log_add_exp(v + l1m, lcct);
-    const float u = u01_from_bits(gw[j]);
-    const float score = logit + (-logf(-logf(u + 1e-30f) + 1e-30f));
-    if (score > best || (score == best && c < best_c)) { best = score; best_c = c; }
+    score[j] = on[j] ? logit + gumbel_of(u01_from_bits(w[j])) : -INFINITY;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oc = __shfl_xor_sync(0xffffffffu, best_c, o);
-    if (ob > best || (ob == best && oc < best_c)) { best = ob; best_c = oc; }
-  }
-  if (lane == 0) p.xt[token] = best_c;
+  const int best_c = warp_argmax_first<5>(score, cls, on);
+  if (lane == 0) xt[token] = best_c;
 }
 
 // ---------------------------------------------------------------------------------------------------------
