@@ -46,7 +46,10 @@ typedef struct {
   int32_t n_layers;       /* 4 */
   int32_t num_timesteps;  /* T (== AdaLN embedding rows) */
   int32_t q_type;         /* 0 = constrained (per-attribute transition matrices), 1 = vanilla */
-  int32_t operand_dtype;  /* tensor-core operand type: 0 = fp16, 1 = bf16; accumulation is fp32 */
+  int32_t operand_dtype;  /* tensor-core operand type, accumulation is fp32: 0 = fp16, 1 = bf16, 2 = bf16x3 (every operand
+                             a bf16 pair hi = bf16(x), lo = bf16(x - hi); products a_hi w_hi + a_hi w_lo + a_lo w_hi: fp32-class
+                             accuracy for 3x the MMAs, 2x the operand bytes and ~1.24 MB more workspace per layout);
+                             other values: LDM_ERR_INVALID */
   int32_t device;         /* CUDA device ordinal */
   double att_1, att_T, ctt_1, ctt_T;  /* alpha_schedule() endpoints, util.py:47-49 */
 } LdmModelDesc;
@@ -211,7 +214,8 @@ int ldm_profile_begin(LdmHandle* h);
 int ldm_profile_end(LdmHandle* h, float* ms_per_category, int64_t* launches_per_category, int32_t n_categories);
 
 /* test taps (tests/ and tools/ only): stop the denoiser after n launches (0 = off); read a workspace buffer
- * ("x32","y32","x16","z16","att16","qkv16","hid16","logits") of the first n_layouts layouts to host; returns bytes. */
+ * ("x32","y32","x16","z16","att16","qkv16","hid16","logits"; operand_dtype 2 also the lo planes "x16_lo","z16_lo","att16_lo",
+ * "qkv16_lo","hid16_lo") of the first n_layouts layouts to host; returns bytes (< 0: unknown name). */
 int ldm_debug_set_stop_after(LdmHandle* h, int32_t n_launches);
 int64_t ldm_debug_read(const LdmHandle* h, const char* name, void* dst_host, int64_t capacity_bytes, int32_t n_layouts);
 

@@ -11,6 +11,9 @@ LIB_PATH = os.path.join(_HERE, "libldm_b200.so")
 LDM_OK, LDM_ERR_INVALID, LDM_ERR_CUDA, LDM_ERR_UNSUPPORTED = 0, -1, -2, -3
 PROFILE_CATEGORIES = ("embed_adaln", "qkv_gemm", "attention", "outproj_gemm", "ff1_gemm", "ff2_gemm", "head_gemm", "posterior_sample", "misc")
 SAMPLING_MODES = {"deterministic": 0, "random": 1, "top_k": 2, "top_p": 3, "gumbel": 4}
+# LdmModelDesc.operand_dtype: tensor-core operands fp16, bf16, or bf16 (hi, lo) pairs ("bf16x3": three MMAs per product,
+# fp32-class operand precision)
+OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "bf16x3": 2}
 
 
 class LdmModelDesc(C.Structure):

@@ -106,6 +106,16 @@ LDM_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
+// The same for a 64-byte-swizzled K-major tile (TMA SWIZZLE_64B; tile base 512-B aligned): rows of 32 x 16-bit (64 B), 8-row
+// groups 512 B apart (SBO); a k-step of 16 advances the start address by 32 B.  Swizzle mode 2 = 64B.
+LDM_DEVINL uint64_t make_smem_desc_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(512 >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
+  return d;
+}
 
 // both operands from shared memory, both K-major
 // operand lists of the wrappers below: LDM_ACCn = "{%0, ..., %(n-1)}", LDM_OUTn = the matching "+f" constraints
@@ -189,19 +199,42 @@ LDM_DEVINL void wgmma_rs_n64_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t
 #undef LDM_F
 
 // ------------------------------------------------------------------------------------------------------------
-// operand dtype helpers (fp16 or bf16 tensor-core operands; accumulation is always fp32)
+// operand modes (LdmModelDesc::operand_dtype; accumulation is always fp32):
+//   OP_F16, OP_BF16 : one 16-bit operand per value
+//   OP_BF16X3       : every 16-bit operand is a pair of bf16 planes, hi = bf16(x), lo = bf16(x - hi), and a product is
+//                     a_hi w_hi + a_hi w_lo + a_lo w_hi (three wgmmas into one accumulator).  The dropped a_lo w_lo is at most
+//                     2^-16 |a w|, and hi + lo is within 2^-16 |x| of x: fp32-class operands on bf16 tensor cores.
 // ------------------------------------------------------------------------------------------------------------
-template <bool BF16> struct OpT;
-template <> struct OpT<false> {
+enum : int { OP_F16 = 0, OP_BF16 = 1, OP_BF16X3 = 2 };
+template <int MODE> struct OpT;
+template <> struct OpT<OP_F16> {
   using T = __half; using T2 = __half2;
   static LDM_DEVINL uint32_t pack(float a, float b) { __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<uint32_t*>(&h); }
   static LDM_DEVINL T from(float a) { return __float2half_rn(a); }
 };
-template <> struct OpT<true> {
+template <> struct OpT<OP_BF16> {
   using T = __nv_bfloat16; using T2 = __nv_bfloat162;
   static LDM_DEVINL uint32_t pack(float a, float b) { __nv_bfloat162 h = __floats2bfloat162_rn(a, b); return *reinterpret_cast<uint32_t*>(&h); }
   static LDM_DEVINL T from(float a) { return __float2bfloat16_rn(a); }
 };
+template <> struct OpT<OP_BF16X3> : OpT<OP_BF16> {
+  // the pair of (a, b): hi = (bf16(a), bf16(b)), lo = (bf16(a - hi_a), bf16(b - hi_b)); x - hi is exact in fp32
+  static LDM_DEVINL void pack_pair(float a, float b, uint32_t& hi, uint32_t& lo) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    const float2 hf = __bfloat1622float2(h);
+    const __nv_bfloat162 l = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h); lo = *reinterpret_cast<const uint32_t*>(&l);
+  }
+  static LDM_DEVINL void from_pair(float a, T& hi, T& lo) { hi = __float2bfloat16_rn(a); lo = __float2bfloat16_rn(a - __bfloat162float(hi)); }
+};
+// the wgmma input type of a mode
+template <int MODE> constexpr bool kOpBf16 = MODE != OP_F16;
+template <int MODE> constexpr bool kOpSplit = MODE == OP_BF16X3;
+
+// TMA descriptors of one operand: the 16-bit plane, plus the lo plane in the split mode (kernel parameters; a one-plane struct
+// has the layout of a bare CUtensorMap)
+template <int MODE> struct OpMaps { CUtensorMap hi; };
+template <> struct OpMaps<OP_BF16X3> { CUtensorMap hi, lo; };
 
 // ------------------------------------------------------------------------------------------------------------
 // Philox4x32-10 (the noise contract shared with oracle/layoutdm_oracle.py::uniforms)

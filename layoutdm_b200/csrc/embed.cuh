@@ -26,11 +26,12 @@ __global__ void adaln_table_kernel(const float* __restrict__ emb /*[L][T][d]*/, 
 }
 
 // fp32 -> 16-bit operand conversion with optional row/col repacking: dst[r][c] = src[src_row(r)][c] for c < src_cols,
-// zero elsewhere.  row_map / col_map == nullptr: identity (maps give the source row / column, -1 = zero).
-template <bool BF16>
+// zero elsewhere.  row_map / col_map == nullptr: identity (maps give the source row / column, -1 = zero).  Split mode: dst is the
+// hi plane and dst_lo the lo plane of the pair.
+template <int MODE>
 __global__ void pack_weight_kernel(const float* __restrict__ src, void* __restrict__ dst_, const int* __restrict__ row_map,
-                                   const int* __restrict__ col_map, int dst_rows, int dst_cols, int src_cols) {
-  using O = OpT<BF16>;
+                                   const int* __restrict__ col_map, int dst_rows, int dst_cols, int src_cols, void* __restrict__ dst_lo) {
+  using O = OpT<MODE>;
   typename O::T* dst = static_cast<typename O::T*>(dst_);
   const size_t n = static_cast<size_t>(dst_rows) * dst_cols;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -38,15 +39,18 @@ __global__ void pack_weight_kernel(const float* __restrict__ src, void* __restri
     const int sr = row_map ? row_map[r] : r;
     const int sc = col_map ? col_map[c] : (c < src_cols ? c : -1);
     const float v = (sr >= 0 && sc >= 0) ? src[static_cast<size_t>(sr) * src_cols + sc] : 0.0f;
-    dst[i] = O::from(v);
+    if constexpr (kOpSplit<MODE>) O::from_pair(v, dst[i], static_cast<typename O::T*>(dst_lo)[i]);
+    else dst[i] = O::from(v);
   }
 }
 
-// one token row: h = cat_emb[id] + pos[s]; x = LN(h) * (1 + scale_t) + shift_t -> fp32 residual row + 16-bit operand row (whole warp)
-template <bool BF16>
+// one token row: h = cat_emb[id] + pos[s]; x = LN(h) * (1 + scale_t) + shift_t -> fp32 residual row + 16-bit operand row (whole warp;
+// split mode: + the lo plane row in x16_lo)
+template <int MODE>
 LDM_DEVINL void embed_token_row(const long long id, const int s, const size_t row, const float* __restrict__ cat_emb, const float* __restrict__ pos,
-                                const float* __restrict__ adaln /*[2d] of (layer 0, t)*/, float* __restrict__ x32, void* __restrict__ x16_, const int d, const int lane) {
-  using O = OpT<BF16>;
+                                const float* __restrict__ adaln /*[2d] of (layer 0, t)*/, float* __restrict__ x32, void* __restrict__ x16_, const int d, const int lane,
+                                void* __restrict__ x16_lo = nullptr) {
+  using O = OpT<MODE>;
   typename O::T* x16 = static_cast<typename O::T*>(x16_);
   const int nv = d / 4;                      // float4 per row (464 / 4 = 116)
   float4* o32 = reinterpret_cast<float4*>(x32 + row * d);
@@ -96,18 +100,27 @@ LDM_DEVINL void embed_token_row(const long long id, const int s, const size_t ro
       r.z = (v[k].z - mean) * rstd * (1.0f + g.z) + h.z;
       r.w = (v[k].w - mean) * rstd * (1.0f + g.w) + h.w;
       o32[i] = r;
-      o16[i] = make_uint2(O::pack(r.x, r.y), O::pack(r.z, r.w));
+      if constexpr (kOpSplit<MODE>) {
+        uint2 hi, lo;
+        O::pack_pair(r.x, r.y, hi.x, lo.x);
+        O::pack_pair(r.z, r.w, hi.y, lo.y);
+        o16[i] = hi;
+        reinterpret_cast<uint2*>(static_cast<typename O::T*>(x16_lo) + row * d)[i] = lo;
+      } else {
+        o16[i] = make_uint2(O::pack(r.x, r.y), O::pack(r.z, r.w));
+      }
     }
   }
 }
 
-template <bool BF16>
+template <int MODE>
 __global__ void __launch_bounds__(256)
 embed_adaln_kernel(const long long* __restrict__ ids /*[B][S]*/, const float* __restrict__ cat_emb /*[C][d]*/,
                    const float* __restrict__ pos /*[S][d]*/, const float* __restrict__ adaln_tab /*[T][2d] of layer 0*/, int t_model,
                    const int* __restrict__ t_layout /*[n_layouts] per-layout timesteps (training-side calls) or nullptr*/,
-                   float* __restrict__ x32 /*[B*128][d]*/, void* __restrict__ x16_, int n_layouts, int n_layouts_padded, int S, int d) {
-  using O = OpT<BF16>;
+                   float* __restrict__ x32 /*[B*128][d]*/, void* __restrict__ x16_, int n_layouts, int n_layouts_padded, int S, int d,
+                   void* __restrict__ x16_lo /*split mode: lo plane of x16*/) {
+  using O = OpT<MODE>;
   typename O::T* x16 = static_cast<typename O::T*>(x16_);
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp_global >= n_layouts_padded * 128) return;
@@ -119,11 +132,15 @@ embed_adaln_kernel(const long long* __restrict__ ids /*[B][S]*/, const float* __
     float4* o32 = reinterpret_cast<float4*>(x32 + row * d);
     uint2* o16 = reinterpret_cast<uint2*>(x16 + row * d);
     for (int i = lane; i < nv; i += 32) { o32[i] = make_float4(0.f, 0.f, 0.f, 0.f); o16[i] = make_uint2(0u, 0u); }
+    if constexpr (kOpSplit<MODE>) {
+      uint2* l16 = reinterpret_cast<uint2*>(static_cast<typename O::T*>(x16_lo) + row * d);
+      for (int i = lane; i < nv; i += 32) l16[i] = make_uint2(0u, 0u);
+    }
     return;
   }
   const long long id = ids[static_cast<size_t>(b) * S + s];
   const float* adaln = adaln_tab + static_cast<size_t>(t_layout != nullptr ? __ldg(t_layout + b) : t_model) * 2 * d;
-  embed_token_row<BF16>(id, s, row, cat_emb, pos, adaln, x32, x16_, d, lane);
+  embed_token_row<MODE>(id, s, row, cat_emb, pos, adaln, x32, x16_, d, lane, x16_lo);
 }
 
 }  // namespace ldm

@@ -2,6 +2,7 @@
 //
 //   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 * n_layouts (one 128-row block = one layout)
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
+//   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; see below
 //
 // One kernel template, one output tile per CTA, 288 threads:
 //   warps 0..7 : two consumer warpgroups.  Each issues m64 x BN_WG x k16 wgmmas from the shared-memory ring (fp32
@@ -15,6 +16,10 @@
 // Epilogues:  QKV (bias, q-scale, 16-bit) | RELU (FF1: bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
 //             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused).
 //
+// Split mode: a ring stage holds four boxes, A_hi | A_lo | W_hi | W_lo, of a 32-element k-block with the 64-byte swizzle, so a
+// stage keeps the bytes (and the GEMMs their stage counts) of the 64-element one-plane k-block.  Each k16 step issues three
+// wgmmas into the accumulator: a_lo w_hi, a_hi w_lo, a_hi w_hi.  16-bit outputs are written as (hi, lo) pairs (out, out_lo).
+//
 // Reference ops replaced: nn.Linear / nn.MultiheadAttention projections / nn.LayerNorm / AdaLayerNorm in
 // T/models/transformer_utils.py:79-83,165-210 and T/models/common/nn_lib.py:187-189,235.
 #pragma once
@@ -24,6 +29,7 @@ namespace ldm {
 
 constexpr int kBM = 128;       // rows of one layout tile (125 tokens + 3 pad rows)
 constexpr int kBK = 64;        // K elements per smem stage (= 128 B = one swizzle row)
+constexpr int kBKSplit = 32;   // split mode: K elements per stage and plane (= 64 B = one 64-byte swizzle row)
 constexpr int kWgK = 16;       // K per wgmma (16-bit operands)
 constexpr int kGemmThreads = 288;
 constexpr int kGemmConsumers = 256;
@@ -49,15 +55,20 @@ struct GemmParams {
   int n_layouts;          //   AdaLN table and every layout reloads its (scale, shift) row; nullptr: one timestep for all
   int rev;                // 1: walk the row blocks from the last to the first.  Consecutive kernels alternate the direction, so a consumer starts
                           // with the rows its producer wrote last -- the part of the intermediate that is still in L2
+  void* out_lo;           // split mode: lo plane of the 16-bit output (same layout as out)
 };
 
-template <int BN_WG, int WG_M, int STAGES>
+template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false>
 struct GemmSmem {
   static constexpr int kWgN = 3 - WG_M;                          // warpgroups along N
-  static constexpr int kABytes = 64 * WG_M * kBK * 2;
-  static constexpr int kBBytes = BN_WG * kBK * 2;                // one warpgroup's weight rows
-  static constexpr int kStageBytes = kABytes + kWgN * kBBytes;
-  static_assert(kBBytes % 1024 == 0, "weight block must keep 1024-B (swizzle atom) alignment");
+  static constexpr int kPlanes = SPLIT ? 2 : 1;
+  static constexpr int kKB = SPLIT ? kBKSplit : kBK;             // K elements per stage
+  static constexpr int kRowBytes = kKB * 2;                      // one smem row = one swizzle row (128 B, split: 64 B)
+  static constexpr int kAPlane = 64 * WG_M * kRowBytes;
+  static constexpr int kABytes = kPlanes * kAPlane;              // A_hi (| A_lo)
+  static constexpr int kBBytes = BN_WG * kRowBytes;              // one warpgroup's weight rows of one plane
+  static constexpr int kStageBytes = kABytes + kPlanes * kWgN * kBBytes;   // ... | W_hi blocks (| W_lo blocks)
+  static_assert(kBBytes % (SPLIT ? 512 : 1024) == 0, "weight block must keep the swizzle atom's alignment");
   static constexpr int kOffBars = STAGES * kStageBytes;
   static constexpr int kOffStat = kOffBars + 256;                // LN: per-row sum, then sum of squared deviations, of each warpgroup's columns
   static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
@@ -74,12 +85,14 @@ LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t a
 }
 
 // grid: (n_tiles, M / (64 WG_M))
-template <int BN_WG, int WG_M, int STAGES, int EPI, bool BF16>
+template <int BN_WG, int WG_M, int STAGES, int EPI, int MODE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows*/, const __grid_constant__ CUtensorMap map_b /*box 64 x BN_WG rows*/,
-               const GemmParams p) {
-  using SM = GemmSmem<BN_WG, WG_M, STAGES>;
-  using O = OpT<BF16>;
+gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x 64 WG_M rows*/,
+               const __grid_constant__ OpMaps<MODE> map_b /*box 64 (split: 32) x BN_WG rows*/, const GemmParams p) {
+  constexpr bool BF16 = kOpBf16<MODE>, SPLIT = kOpSplit<MODE>;
+  using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT>;
+  using O = OpT<MODE>;
+  constexpr int kKB = SM::kKB;
   constexpr int kBMt = 64 * WG_M, kAcc = BN_WG / 2;
   static_assert(EPI != EPI_LN || (WG_M == 1 && BN_WG == 232), "LN epilogue is laid out for 464 = 2 x 232 columns");
   static_assert(EPI == EPI_LN || WG_M == 2, "plain epilogues use 128-row tiles");
@@ -90,14 +103,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
   uint64_t* empty = full + STAGES;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int num_kb = (p.K + kBK - 1) / kBK;
+  const int num_kb = (p.K + kKB - 1) / kKB;
   const int n_mblk = p.M / kBMt;
   const int m_blk = p.rev ? n_mblk - 1 - static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.y);
   const int m0 = m_blk * kBMt, n0 = static_cast<int>(blockIdx.x) * BN_WG * SM::kWgN;
 
   if (threadIdx.x == kGemmConsumers) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
+    tma_prefetch_desc(&map_a.hi);
+    tma_prefetch_desc(&map_b.hi);
+    if constexpr (SPLIT) { tma_prefetch_desc(&map_a.lo); tma_prefetch_desc(&map_b.lo); }
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
     fence_mbar_init();
   }
@@ -112,9 +126,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
         mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
         uint8_t* st = smem + s * SM::kStageBytes;
         mbar_arrive_expect_tx(&full[s], SM::kStageBytes);    // out-of-bounds box parts are zero-filled and still counted
-        tma_load_2d(st, &map_a, &full[s], kb * kBK, m0);
+        tma_load_2d(st, &map_a.hi, &full[s], kb * kKB, m0);
 #pragma unroll
-        for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b, &full[s], kb * kBK, n0 + wn * BN_WG);
+        for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b.hi, &full[s], kb * kKB, n0 + wn * BN_WG);
+        if constexpr (SPLIT) {
+          tma_load_2d(st + SM::kAPlane, &map_a.lo, &full[s], kb * kKB, m0);
+#pragma unroll
+          for (int wn = 0; wn < SM::kWgN; ++wn)
+            tma_load_2d(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes, &map_b.lo, &full[s], kb * kKB, n0 + wn * BN_WG);
+        }
       }
     }
     return;
@@ -130,14 +150,31 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
     const int s = kb % STAGES;
     mbar_wait(&full[s], (kb / STAGES) & 1);
     const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
-    const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
-    const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
-    wgmma_fence();
-    if (kb * kBK + kBK <= p.K) {
+    if constexpr (!SPLIT) {
+      const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
+      const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
+      wgmma_fence();
+      if (kb * kBK + kBK <= p.K) {
 #pragma unroll
-      for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
-    } else {                                                // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
-      wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
+        for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
+      } else {                                              // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
+        wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
+      }
+    } else {
+      const uint64_t da = make_smem_desc_sw64(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc_sw64(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
+      const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
+      const uint64_t db_lo = make_smem_desc_sw64(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
+      wgmma_fence();
+      // K % 32 is 0 or 16 (d = 464: 16): the tail k-block is a single k-step
+      const int nk = kb * kKB + kKB <= p.K ? kKB / kWgK : 1;
+#pragma unroll
+      for (int k = 0; k < kKB / kWgK; ++k) {
+        if (k < nk) {                                       // +32 B per k-step (>>4 = 2); the small terms first
+          wgmma_ss<true, BN_WG>(acc, da_lo + 2 * k, db + 2 * k, (kb | k) != 0);
+          wgmma_ss<true, BN_WG>(acc, da + 2 * k, db_lo + 2 * k, 1);
+          wgmma_ss<true, BN_WG>(acc, da + 2 * k, db + 2 * k, 1);
+        }
+      }
     }
     wgmma_commit();
     // keep this k-block's MMAs in flight; once the previous k-block's have retired its stage goes back to the producer
@@ -171,8 +208,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
       } else {
         uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
         uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
-        *o0 = O::pack(v[0], v[1]);
-        *o1 = O::pack(v[2], v[3]);
+        if constexpr (SPLIT) {
+          uint32_t* l0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row0) * p.ldo + c);
+          uint32_t* l1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row1) * p.ldo + c);
+          O::pack_pair(v[0], v[1], *o0, *l0);
+          O::pack_pair(v[2], v[3], *o1, *l1);
+        } else {
+          *o0 = O::pack(v[0], v[1]);
+          *o1 = O::pack(v[2], v[3]);
+        }
       }
     }
   } else {
@@ -246,8 +290,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a /*box 64 x 64 WG_M rows
       const float2 g = __ldg(reinterpret_cast<const float2*>(gam + c)), h = __ldg(reinterpret_cast<const float2*>(bet + c));
       const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + gadd) + h.y;
       const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + gadd) + h.y;
-      *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
-      *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
+      if constexpr (SPLIT) {
+        typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
+        O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
+        O::pack_pair(v2, v3, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row1) * N + c));
+      } else {
+        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
+        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
+      }
       if (p.out32 != nullptr) {
         *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
         *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);

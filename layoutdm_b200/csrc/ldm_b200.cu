@@ -42,17 +42,20 @@ constexpr int kAttN = 8 * kHeadPad;        // 512: attention output, heads padde
 constexpr int kMaxLayouts = 32767;  // layouts per call
 constexpr int kLogitLd = 160;       // padded logits row (C <= 160)
 constexpr int kDModel = 464;        // the kernels are laid out for the paper's backbone: d = 464 (LN tiles 224 + 240), ff = 4 d
-// GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, bf16>
+// GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, operand mode>
 constexpr int kPlainBN = 256, kPlainStages = 4;   // QKV / FF1: 128 x 256 tiles
 constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
 constexpr int kLnBN = 232, kLnStages = 3;         // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue)
-template <bool BF16> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_QKV, BF16>;
-template <bool BF16> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_RELU, BF16>;
-template <bool BF16> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, BF16>;
-template <bool BF16> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, BF16>;
+template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_QKV, MODE>;
+template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_RELU, MODE>;
+template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
+template <int MODE> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, MODE>;
 constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages>::kBytes;
 constexpr int kHeadSmem = GemmSmem<kHeadBN, 2, kHeadStages>::kBytes;
 constexpr int kLnSmem = GemmSmem<kLnBN, 1, kLnStages>::kBytes;
+// the split mode's stage (two planes of a 32-element k-block) has the bytes of the one-plane 64-element stage: same stage counts
+static_assert(GemmSmem<kPlainBN, 2, kPlainStages, true>::kBytes == kPlainSmem && GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem &&
+              GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem, "split-mode ring stages must keep the one-plane sizes");
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -70,13 +73,14 @@ int load_encode() {
 }
 
 // 2-D row-major [rows][cols] 16-bit tensor, box = box_rows x 64 columns, 128-byte swizzle, zero OOB fill (TMA operand loads).
-int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16) {
+// sw64: box_rows x 32 columns with the 64-byte swizzle (the split-mode GEMM operands).
+int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16, bool sw64 = false) {
   const cuuint64_t dims[2] = {cols, rows};
   const cuuint64_t strides[1] = {cols * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kBK), box_rows};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(sw64 ? kBKSplit : kBK), box_rows};
   const cuuint32_t estr[2] = {1, 1};
   CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims,
-                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu box_rows=%u", (int)r,
                                      (unsigned long long)rows, (unsigned long long)cols, box_rows);
@@ -107,7 +111,9 @@ __global__ void fill_ids_kernel(long long* dst, long long v, size_t n) {
 struct LdmHandle {
   LdmModelDesc desc;
   int C = 0, S = 0, L = 0, T = 0, G = 0;
-  bool bf16 = false;
+  int mode = OP_F16;          // operand mode (LdmModelDesc::operand_dtype)
+  bool bf16 = false;          // bf16 operand data (OP_BF16, OP_BF16X3)
+  bool split = false;         // OP_BF16X3: every 16-bit weight and activation buffer has a lo plane (the *_lo members)
   int64_t launches = 0;
   int pdl = 1;                // env LDM_PDL=0: no programmatic dependent launch
   int debug_stop_after = 0;   // test tap: stop the denoiser after this many launches (0 = run everything)
@@ -120,6 +126,8 @@ struct LdmHandle {
   float *bqkv[kMaxLayers] = {}, *bo[kMaxLayers] = {}, *b1[kMaxLayers] = {}, *b2[kMaxLayers] = {}, *ln2w[kMaxLayers] = {}, *ln2b[kMaxLayers] = {};
   float *hlnw = nullptr, *hlnb = nullptr;
   CUtensorMap m_wqkv[kMaxLayers], m_wo[kMaxLayers], m_w1[kMaxLayers], m_w2[kMaxLayers], m_whead;
+  void *wqkv_lo[kMaxLayers] = {}, *wo_lo[kMaxLayers] = {}, *w1_lo[kMaxLayers] = {}, *w2_lo[kMaxLayers] = {}, *whead_lo = nullptr;
+  CUtensorMap m_wqkv_lo[kMaxLayers], m_wo_lo[kMaxLayers], m_w1_lo[kMaxLayers], m_w2_lo[kMaxLayers], m_whead_lo;
   // workspace (device), sized for cap layouts
   int cap = 0;
   void *x16 = nullptr, *qkv16 = nullptr, *att16 = nullptr, *z16 = nullptr, *hid16 = nullptr;
@@ -130,12 +138,15 @@ struct LdmHandle {
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
   CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
+  void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
+  CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
   // CUDA graph of the whole T-step loop (ldm_sample_loop): captured once per (batch, plan, sampling, conditioning kind) and
   // replayed; everything that changes from call to call lives in device memory (noise key block, staged cond / start ids)
   int use_graph = 1;           // env LDM_GRAPH=0: plain stream launches
   int sweep = 1;               // env LDM_SWEEP=0: every kernel walks its row blocks in ascending order (no alternating directions)
-  int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw
+  int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
+                               // The split mode always launches it: the draw kernels write one 16-bit plane only
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   uint64_t graph_key = 0;
@@ -174,15 +185,36 @@ void free_staging(LdmHandle* h) {
   h->staging.clear();
 }
 
-int pack16(LdmHandle* h, void** dst, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
+// 16-bit weight (split mode: the hi plane in dst, the lo plane in dst_lo)
+int pack16(LdmHandle* h, void** dst, void** dst_lo, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
            const int* col_map_dev = nullptr) {
-  CK(cudaMalloc(dst, static_cast<size_t>(dst_rows) * dst_cols * 2));
+  const size_t bytes = static_cast<size_t>(dst_rows) * dst_cols * 2;
+  CK(cudaMalloc(dst, bytes));
   h->owned.push_back(*dst);
+  if (h->split) { CK(cudaMalloc(dst_lo, bytes)); h->owned.push_back(*dst_lo); }
   const int blocks = 512;
-  if (h->bf16) pack_weight_kernel<true><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols);
-  else pack_weight_kernel<false><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols);
+  if (h->mode == OP_BF16X3) pack_weight_kernel<OP_BF16X3><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, *dst_lo);
+  else if (h->mode == OP_BF16) pack_weight_kernel<OP_BF16><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
+  else pack_weight_kernel<OP_F16><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
   CK(cudaGetLastError());
   return LDM_OK;
+}
+
+// TMA descriptor(s) of one GEMM operand plane pair: 128-byte swizzle, split mode: both planes with the 64-byte swizzle
+int make_op_maps(const LdmHandle* h, CUtensorMap* m, CUtensorMap* m_lo, const void* base, const void* base_lo, uint64_t rows, uint64_t cols,
+                 uint32_t box_rows) {
+  int rc = make_map(m, base, rows, cols, box_rows, h->bf16, h->split);
+  if (rc || !h->split) return rc;
+  return make_map(m_lo, base_lo, rows, cols, box_rows, h->bf16, true);
+}
+
+template <int MODE>
+OpMaps<MODE> op_maps(const CUtensorMap& hi, const CUtensorMap& lo) {
+  OpMaps<MODE> m;
+  m.hi = hi;
+  if constexpr (kOpSplit<MODE>) m.lo = lo;
+  else (void)lo;
+  return m;
 }
 
 // util.py:47-70 + constrained.py:64-90: float64 schedule, fp32 log tables, 8 rows of length T+1 per group
@@ -251,7 +283,8 @@ int set_smem(K kernel, int bytes) {
 }
 
 void free_workspace(LdmHandle* h) {
-  void** ws[] = {&h->x16, &h->qkv16, &h->att16, &h->z16, &h->hid16, reinterpret_cast<void**>(&h->x32), reinterpret_cast<void**>(&h->y32),
+  void** ws[] = {&h->x16, &h->qkv16, &h->att16, &h->z16, &h->hid16, &h->x16_lo, &h->qkv16_lo, &h->att16_lo, &h->z16_lo, &h->hid16_lo,
+                 reinterpret_cast<void**>(&h->x32), reinterpret_cast<void**>(&h->y32),
                  reinterpret_cast<void**>(&h->logits), reinterpret_cast<void**>(&h->ids[0]), reinterpret_cast<void**>(&h->ids[1]),
                  reinterpret_cast<void**>(&h->ids_final), reinterpret_cast<void**>(&h->c_seq), reinterpret_cast<void**>(&h->c_seq_orig),
                  reinterpret_cast<void**>(&h->c_mask), reinterpret_cast<void**>(&h->rel_lp)};
@@ -268,6 +301,21 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   free_workspace(h);
   const size_t M = static_cast<size_t>(n_layouts) * kBM;
   const int d = h->desc.d_model, ff = h->desc.d_ff;
+  if (h->split) {
+    // the lo planes: ~1.24 MB per layout.  An allocation that does not fit is reported (not left as the runtime's last error)
+    // and releases what this call allocated
+    void** lo[] = {&h->x16_lo, &h->qkv16_lo, &h->att16_lo, &h->z16_lo, &h->hid16_lo};
+    const size_t cols[] = {static_cast<size_t>(d), static_cast<size_t>(kQkvN), static_cast<size_t>(kAttN), static_cast<size_t>(d), static_cast<size_t>(ff)};
+    for (int i = 0; i < 5; ++i) {
+      const cudaError_t e = cudaMalloc(lo[i], M * cols[i] * 2);
+      if (e != cudaSuccess) {
+        cudaGetLastError();
+        free_workspace(h);
+        return fail(LDM_ERR_CUDA, "split-operand workspace for %d layouts does not fit: %s", n_layouts, cudaGetErrorString(e));
+      }
+      CK(cudaMemset(*lo[i], 0, M * cols[i] * 2));
+    }
+  }
   CK(cudaMalloc(&h->x16, M * d * 2));
   CK(cudaMalloc(&h->qkv16, M * kQkvN * 2));
   CK(cudaMalloc(&h->att16, M * kAttN * 2));
@@ -291,16 +339,18 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   h->cap = n_layouts;
   h->ws_generation++;
   int rc;
-  if ((rc = make_map(&h->m_x16, h->x16, M, d, kBM, h->bf16))) return rc;
-  if ((rc = make_map(&h->m_att16, h->att16, M, kAttN, 64, h->bf16))) return rc;   // the out-projection's A operand
-  if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles
-  if ((rc = make_map(&h->m_z16, h->z16, M, d, kBM, h->bf16))) return rc;
-  if ((rc = make_map(&h->m_hid16, h->hid16, M, ff, 64, h->bf16))) return rc;
+  if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM))) return rc;
+  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64))) return rc;   // the out-projection's A operand
+  if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles (128-byte swizzle in every mode)
+  if (h->split && (rc = make_map(&h->m_qkv16_lo, h->qkv16_lo, M, kQkvN, kBM, h->bf16))) return rc;
+  if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM))) return rc;
+  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64))) return rc;
   return LDM_OK;
 }
 
-template <bool BF16>
+template <int MODE>
 int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
+  const auto maps = [](const CUtensorMap& hi, const CUtensorMap& lo) { return op_maps<MODE>(hi, lo); };
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
   const int M = n * kBM;
   const dim3 ln_grid(1, M / 64);          // LN GEMMs: 64 whole rows per CTA
@@ -314,50 +364,50 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   if (!skip_embed) {     // skipped inside the loop: the previous step's draw kernel has already written this step's x32 / x16 rows
     const int warps = n * 128, blocks = (warps * 32 + 255) / 256;
     ProfScope ps(h, CAT_EMBED, st);
-    CK(launch_step(h, embed_adaln_kernel<BF16>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
-                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16, n, n, h->S, d));
+    CK(launch_step(h, embed_adaln_kernel<MODE>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
+                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16, n, n, h->S, d, h->x16_lo));
   }
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
     {  // QKV projection (+bias, q * 1/sqrt(head_dim))
       GemmParams p{M, kQkvN, d, kQkvN / kPlainBN, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
-      p.rev = next_rev();
+      p.rev = next_rev(); p.out_lo = h->qkv16_lo;
       ProfScope ps(h, CAT_QKV, st);
-      CK(launch_step(h, kGemmQkv<BF16>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, h->m_x16, h->m_wqkv[l], p));
+      CK(launch_step(h, kGemmQkv<MODE>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]), p));
     }
     LDM_STAGE_DONE();
     {
       ProfScope ps(h, CAT_ATTN, st);
-      CK(launch_step(h, attention_kernel<BF16>, dim3(n * h->desc.n_heads), kAttThreads, kAttSmemBytes, st,
-                     h->m_qkv16, h->att16, h->S, h->desc.n_heads, n, next_rev()));
+      CK(launch_step(h, attention_kernel<MODE>, dim3(n * h->desc.n_heads), kAttThreads, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes, st,
+                     maps(h->m_qkv16, h->m_qkv16_lo), h->att16, h->S, h->desc.n_heads, n, next_rev(), h->att16_lo));
     }
     LDM_STAGE_DONE();
     {  // out-projection + bias + residual (from the NORMALISED x) -> y32 ; z16 = LayerNorm2(y)   [fused epilogue]
       GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
-      p.rev = next_rev();
+      p.rev = next_rev(); p.out_lo = h->z16_lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(launch_step(h, kGemmLn<BF16>, ln_grid, kGemmThreads, kLnSmem, st, h->m_att16, h->m_wo[l], p));
+      CK(launch_step(h, kGemmLn<MODE>, ln_grid, kGemmThreads, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
       GemmParams p{M, ff, d, (ff + kPlainBN - 1) / kPlainBN, h->b1[l], h->hid16, ff, 1.0f, 0};   // 7 tiles of 256 columns + one of 64
-      p.rev = next_rev();
+      p.rev = next_rev(); p.out_lo = h->hid16_lo;
       ProfScope ps(h, CAT_FF1, st);
-      CK(launch_step(h, kGemmFf1<BF16>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, h->m_z16, h->m_w1[l], p));
+      CK(launch_step(h, kGemmFf1<MODE>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]), p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
       GemmParams p{M, d, ff, 1, h->b2[l], nullptr, d, 1.0f, 0, h->y32, nullptr, nullptr, nullptr, 0, nullptr};
       if (l + 1 < L) {
         const float* tab = h->adaln + (static_cast<size_t>(l + 1) * T + t_model) * 2 * d;
-        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16;
+        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16; p.out_lo = h->x16_lo;
         if (t_layout) { p.ln_scale = h->adaln + static_cast<size_t>(l + 1) * T * 2 * d; p.t_layout = t_layout; p.n_layouts = n; }   // per-layout rows
       } else {
-        p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16;
+        p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16; p.out_lo = h->z16_lo;
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(launch_step(h, kGemmLn<BF16>, ln_grid, kGemmThreads, kLnSmem, st, h->m_hid16, h->m_w2[l], p));
+      CK(launch_step(h, kGemmLn<MODE>, ln_grid, kGemmThreads, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), p));
     }
     LDM_STAGE_DONE();
   }
@@ -365,11 +415,20 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, kGemmHead<BF16>, dim3(1, n), kGemmThreads, kHeadSmem, st, h->m_z16, h->m_whead, p));
+    CK(launch_step(h, kGemmHead<MODE>, dim3(1, n), kGemmThreads, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
   return LDM_OK;
+}
+
+// the denoiser in the handle's operand mode
+int run_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
+  switch (h->mode) {
+    case OP_BF16X3: return launch_denoiser<OP_BF16X3>(h, n, ids_in, t_model, st, t_layout, skip_embed);
+    case OP_BF16: return launch_denoiser<OP_BF16>(h, n, ids_in, t_model, st, t_layout, skip_embed);
+    default: return launch_denoiser<OP_F16>(h, n, ids_in, t_model, st, t_layout, skip_embed);
+  }
 }
 
 int validate_common(LdmHandle* h, int B, const LdmSampling* s) {
@@ -411,7 +470,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
       ProfScope ps(h, CAT_MISC, st);
       logits_scatter_kernel<<<1024, 256, 0, st>>>(logits_in, h->logits, B, h->S, h->C);
     } else {
-      rc = h->bf16 ? launch_denoiser<true>(h, B, ids_in, t_model, st, nullptr, skip_embed) : launch_denoiser<false>(h, B, ids_in, t_model, st, nullptr, skip_embed);
+      rc = run_denoiser(h, B, ids_in, t_model, st, nullptr, skip_embed);
       if (rc) return rc;
     }
     if (logits_out != nullptr) {
@@ -496,6 +555,8 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     return fail(LDM_ERR_UNSUPPORTED, "vocabulary C=%d must be in [129,160] and S=%d <= 125", C, S);
   if (desc->q_type != 0 && desc->q_type != 1) return fail(LDM_ERR_INVALID, "q_type must be 0 (constrained) or 1 (vanilla)");
   if (desc->q_type == 0 && desc->n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "constrained q_type needs the c-x-y-w-h layout (5 attributes)");
+  if (desc->operand_dtype < OP_F16 || desc->operand_dtype > OP_BF16X3)
+    return fail(LDM_ERR_INVALID, "operand_dtype must be 0 (fp16), 1 (bf16) or 2 (bf16x3), got %d", desc->operand_dtype);
   CK(cudaSetDevice(desc->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, desc->device));
@@ -504,11 +565,13 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (rc) return rc;
 
   LdmHandle* h = new LdmHandle();
-  h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T; h->bf16 = desc->operand_dtype == 1;
+  h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T;
+  h->mode = desc->operand_dtype; h->bf16 = h->mode != OP_F16; h->split = h->mode == OP_BF16X3;
   h->G = desc->q_type == 0 ? desc->n_attr : 1;
   if (const char* e = getenv("LDM_PDL")) h->pdl = atoi(e);
   if (const char* e = getenv("LDM_GRAPH")) h->use_graph = atoi(e);
   if (const char* e = getenv("LDM_FUSE_EMBED")) h->fuse_embed = atoi(e);
+  if (h->split) h->fuse_embed = 0;
   if (const char* e = getenv("LDM_SWEEP")) h->sweep = atoi(e);
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
@@ -545,27 +608,27 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   for (int l = 0; l < L; ++l) {
     float* tmp = nullptr;
     TRY(dev_upload_tmp(h, &tmp, w->in_proj_w + static_cast<size_t>(l) * 3 * d * d, static_cast<size_t>(3) * d * d));
-    TRY(pack16(h, &h->wqkv[l], tmp, qmap_dev, kQkvN, d, d));
+    TRY(pack16(h, &h->wqkv[l], &h->wqkv_lo[l], tmp, qmap_dev, kQkvN, d, d));
     std::vector<float> bq(kQkvN, 0.0f);
     for (int r = 0; r < kQkvN; ++r) if (qmap[r] >= 0) bq[r] = w->in_proj_b[static_cast<size_t>(l) * 3 * d + qmap[r]];
     // column dh of every V head = 1 (zero weight row + unit bias): the attention kernel reads the softmax denominator from it
     for (int hh = 0; hh < desc->n_heads; ++hh) bq[2 * 8 * kHeadPad + hh * kHeadPad + dh] = 1.0f;
     TRY(dev_upload(h, &h->bqkv[l], bq.data(), bq.size()));
     TRY(dev_upload_tmp(h, &tmp, w->out_proj_w + static_cast<size_t>(l) * d * d, static_cast<size_t>(d) * d));
-    TRY(pack16(h, &h->wo[l], tmp, nullptr, d, kAttN, d, amap_dev));      // K = 512: head h occupies columns h*64 .. h*64+57
+    TRY(pack16(h, &h->wo[l], &h->wo_lo[l], tmp, nullptr, d, kAttN, d, amap_dev));      // K = 512: head h occupies columns h*64 .. h*64+57
     TRY(dev_upload(h, &h->bo[l], w->out_proj_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload_tmp(h, &tmp, w->linear1_w + static_cast<size_t>(l) * ff * d, static_cast<size_t>(ff) * d));
-    TRY(pack16(h, &h->w1[l], tmp, nullptr, ff, d, d));
+    TRY(pack16(h, &h->w1[l], &h->w1_lo[l], tmp, nullptr, ff, d, d));
     TRY(dev_upload(h, &h->b1[l], w->linear1_b + static_cast<size_t>(l) * ff, static_cast<size_t>(ff)));
     TRY(dev_upload_tmp(h, &tmp, w->linear2_w + static_cast<size_t>(l) * d * ff, static_cast<size_t>(d) * ff));
-    TRY(pack16(h, &h->w2[l], tmp, nullptr, d, ff, ff));
+    TRY(pack16(h, &h->w2[l], &h->w2_lo[l], tmp, nullptr, d, ff, ff));
     TRY(dev_upload(h, &h->b2[l], w->linear2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2w[l], w->norm2_w + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2b[l], w->norm2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(make_map(&h->m_wqkv[l], h->wqkv[l], kQkvN, d, kPlainBN, h->bf16));   // one warpgroup's weight rows per box
-    TRY(make_map(&h->m_wo[l], h->wo[l], d, kAttN, kLnBN, h->bf16));
-    TRY(make_map(&h->m_w1[l], h->w1[l], ff, d, kPlainBN, h->bf16));
-    TRY(make_map(&h->m_w2[l], h->w2[l], d, ff, kLnBN, h->bf16));
+    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN));   // one warpgroup's weight rows per box
+    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN));
+    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN));
+    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN));
   }
   {
     float* tmp = nullptr;
@@ -574,8 +637,8 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     for (int r = 0; r < kLogitLd; ++r) hmap[r] = r < C ? r : -1;
     int* hmap_dev = nullptr;
     TRY(dev_upload(h, &hmap_dev, hmap.data(), hmap.size()));
-    TRY(pack16(h, &h->whead, tmp, hmap_dev, kLogitLd, d, d));
-    TRY(make_map(&h->m_whead, h->whead, kLogitLd, d, kHeadBN, h->bf16));
+    TRY(pack16(h, &h->whead, &h->whead_lo, tmp, hmap_dev, kLogitLd, d, d));
+    TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN));
   }
   {
     std::vector<float> sch(static_cast<size_t>(h->G) * 8 * (T + 1));
@@ -592,14 +655,18 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (cudaDeviceSynchronize() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(cudaGetLastError())); }
   free_staging(h);
 
-  if (h->bf16) {
-    TRY(set_smem(kGemmQkv<true>, kPlainSmem)); TRY(set_smem(kGemmFf1<true>, kPlainSmem));
-    TRY(set_smem(kGemmHead<true>, kHeadSmem)); TRY(set_smem(kGemmLn<true>, kLnSmem));
-    TRY(set_smem(attention_kernel<true>, kAttSmemBytes));
+  if (h->mode == OP_BF16X3) {
+    TRY(set_smem(kGemmQkv<OP_BF16X3>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_BF16X3>, kPlainSmem));
+    TRY(set_smem(kGemmHead<OP_BF16X3>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16X3>, kLnSmem));
+    TRY(set_smem(attention_kernel<OP_BF16X3>, kAttSmemBytesSplit));
+  } else if (h->mode == OP_BF16) {
+    TRY(set_smem(kGemmQkv<OP_BF16>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_BF16>, kPlainSmem));
+    TRY(set_smem(kGemmHead<OP_BF16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16>, kLnSmem));
+    TRY(set_smem(attention_kernel<OP_BF16>, kAttSmemBytes));
   } else {
-    TRY(set_smem(kGemmQkv<false>, kPlainSmem)); TRY(set_smem(kGemmFf1<false>, kPlainSmem));
-    TRY(set_smem(kGemmHead<false>, kHeadSmem)); TRY(set_smem(kGemmLn<false>, kLnSmem));
-    TRY(set_smem(attention_kernel<false>, kAttSmemBytes));
+    TRY(set_smem(kGemmQkv<OP_F16>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_F16>, kPlainSmem));
+    TRY(set_smem(kGemmHead<OP_F16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_F16>, kLnSmem));
+    TRY(set_smem(attention_kernel<OP_F16>, kAttSmemBytes));
   }
 #undef TRY
   *out = h;
@@ -853,7 +920,7 @@ namespace {
 int run_denoiser_per_layout_t(LdmHandle* h, int B, const long long* ids, const int32_t* t_dev, cudaStream_t st) {
   int rc = ensure_workspace(h, B);
   if (rc) return rc;
-  return h->bf16 ? launch_denoiser<true>(h, B, ids, 0, st, t_dev) : launch_denoiser<false>(h, B, ids, 0, st, t_dev);
+  return run_denoiser(h, B, ids, 0, st, t_dev);
 }
 
 }  // namespace
@@ -983,7 +1050,13 @@ int64_t ldm_debug_read(const LdmHandle* h, const char* name, void* dst, int64_t 
   else if (!strcmp(name, "qkv16")) { src = h->qkv16; bytes = M * kQkvN * 2; }
   else if (!strcmp(name, "hid16")) { src = h->hid16; bytes = M * ff * 2; }
   else if (!strcmp(name, "logits")) { src = h->logits; bytes = M * kLogitLd * 4; }
+  else if (!strcmp(name, "x16_lo")) { src = h->x16_lo; bytes = M * d * 2; }
+  else if (!strcmp(name, "z16_lo")) { src = h->z16_lo; bytes = M * d * 2; }
+  else if (!strcmp(name, "att16_lo")) { src = h->att16_lo; bytes = M * kAttN * 2; }
+  else if (!strcmp(name, "qkv16_lo")) { src = h->qkv16_lo; bytes = M * kQkvN * 2; }
+  else if (!strcmp(name, "hid16_lo")) { src = h->hid16_lo; bytes = M * ff * 2; }
   else return -1;
+  if (!h->split && strstr(name, "_lo") != nullptr) return -1;   // lo planes exist in the split mode only
   if (dst && capacity_bytes >= static_cast<int64_t>(bytes)) {
     if (cudaDeviceSynchronize() != cudaSuccess) return -2;
     if (cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -2;

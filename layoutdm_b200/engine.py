@@ -44,6 +44,8 @@ class Engine:
     def __init__(self, vocab: Vocab, weights: Dict[str, torch.Tensor], num_timesteps: int = 100, q_type: str = "constrained",
                  operand_dtype: str = "fp16", device: Optional[int] = None, d_model: int = 464, n_heads: int = 8, d_ff: int = 1856,
                  att_1=0.99999, att_T=0.000009, ctt_1=0.000009, ctt_T=0.99999):
+        if operand_dtype not in _lib.OPERAND_DTYPES:
+            raise ValueError(f"operand_dtype must be one of {', '.join(_lib.OPERAND_DTYPES)}, got {operand_dtype!r}")
         if not torch.cuda.is_available():
             raise RuntimeError("layoutdm_b200 needs a CUDA (sm_90a, H100) device; there is no CPU fallback")
         self.lib = _lib.load()
@@ -55,7 +57,7 @@ class Engine:
         self.device = torch.device("cuda", self.device_index)
         L = weights["in_proj_w"].shape[0]
         desc = _lib.LdmModelDesc(vocab.n_cat, vocab.n_bins, vocab.n_elem, vocab.n_attr, d_model, n_heads, d_ff, L, num_timesteps,
-                                 {"constrained": 0, "vanilla": 1}[q_type], {"fp16": 0, "bf16": 1}[operand_dtype], self.device_index,
+                                 {"constrained": 0, "vanilla": 1}[q_type], _lib.OPERAND_DTYPES[operand_dtype], self.device_index,
                                  att_1, att_T, ctt_1, ctt_T)
         w = _lib.LdmWeights()
         keep = []
