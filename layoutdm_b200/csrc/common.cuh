@@ -17,6 +17,7 @@ constexpr float kLogEps = -69.07755278982137f;  // log(1e-30), T/models/categori
 // shared-memory addressing
 // ------------------------------------------------------------------------------------------------------------
 LDM_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+LDM_DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------
 // programmatic dependent launch (every kernel of the step is launched with programmatic stream serialization): the
@@ -73,6 +74,27 @@ LDM_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* ba
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// TMA 2-D tile store from shared memory, completion tracked per thread in bulk groups
+LDM_DEVINL void tma_store_2d(const CUtensorMap* map, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+LDM_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still reading their shared-memory source
+template <int N>
+LDM_DEVINL void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every bulk group of this thread complete (its global writes done)
+LDM_DEVINL void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory writes before later async-proxy (TMA) reads of them
+LDM_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// warp-specialised register split: every warp of a warpgroup executes it; the new per-thread count is a multiple of 8
+template <int R>
+LDM_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+LDM_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
 LDM_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 

@@ -4,11 +4,18 @@
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
 //   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; see below
 //
-// One kernel template, one output tile per CTA, 288 threads:
-//   warps 0..7 : two consumer warpgroups.  Each issues m64 x BN_WG x k16 wgmmas from the shared-memory ring (fp32
-//                accumulators in registers) and runs the epilogue on its own accumulator fragment.
-//   warp 8     : TMA producer (one lane): cp.async.bulk.tensor 2-D tiles with the 128-byte swizzle into a STAGES-deep
-//                ring, completion on mbarriers (full: TMA bytes landed, empty: both warpgroups' MMAs have read the stage).
+// One kernel template, 384 threads; CTA b runs tiles b, b + gridDim.x, ... (the column tile varies fastest, so consecutive
+// tiles share their A row block in L2).  The GEMMs with TMA-staged stores are launched persistent (min(tiles, SMs) CTAs),
+// the others with one CTA per tile:
+//   warps 0..7  : two consumer warpgroups (setmaxnreg: 232 registers).  Each issues m64 x BN_WG x k16 wgmmas from the
+//                 shared-memory ring (fp32 accumulators in registers) and runs the epilogue on its own accumulator fragment.
+//   warps 8..11 : producer warpgroup (setmaxnreg: 40 registers), one lane issues the TMA loads: cp.async.bulk.tensor 2-D
+//                 tiles with the 128-byte swizzle into a STAGES-deep ring, completion on mbarriers (full: TMA bytes landed,
+//                 empty: both warpgroups' MMAs have read the stage).  Ring slot and phase run on across tiles, so the
+//                 producer fills the ring with the next tile while the consumers run this tile's epilogue.
+// Stores: the 16-bit QKV / FF1 epilogues (one-plane modes) write the fragment into a shared-memory staging tile and one
+// thread per warpgroup stores it with TMA; the consumers go on to the next tile while the store drains.  The other epilogues
+// store straight from the fragment.
 // Tile shapes:
 //   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (QKV, FF1: 256 columns; vocabulary head: 160)
 //   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the LN epilogue: 2 x 232 = 464 =
@@ -31,8 +38,8 @@ constexpr int kBM = 128;       // rows of one layout tile (125 tokens + 3 pad ro
 constexpr int kBK = 64;        // K elements per smem stage (= 128 B = one swizzle row)
 constexpr int kBKSplit = 32;   // split mode: K elements per stage and plane (= 64 B = one 64-byte swizzle row)
 constexpr int kWgK = 16;       // K per wgmma (16-bit operands)
-constexpr int kGemmThreads = 288;
 constexpr int kGemmConsumers = 256;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // persistent block: 128 x 40 + 256 x 232 <= the SM's 64 K registers
 
 enum : int { EPI_QKV = 0, EPI_RELU = 1, EPI_F32 = 2, EPI_LN = 3 };
 
@@ -58,7 +65,16 @@ struct GemmParams {
   void* out_lo;           // split mode: lo plane of the 16-bit output (same layout as out)
 };
 
-template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false>
+// TMA-staged stores: the 16-bit plain epilogues of the one-plane modes (the split mode's (hi, lo) pair outputs would need two
+// staging tiles, which leave too few ring stages).  These GEMMs are the persistent ones: 384 threads (producer warpgroup),
+// min(tiles, SMs) CTAs.  The others store from the fragment, have nothing to overlap their epilogue with, and run one tile per
+// CTA with 288 threads (one producer warp)
+template <int EPI, bool SPLIT>
+constexpr bool kStagedStore = (EPI == EPI_QKV || EPI == EPI_RELU) && !SPLIT;
+template <int EPI, int MODE>
+constexpr int kGemmThreads = kStagedStore<EPI, kOpSplit<MODE>> ? 384 : 288;
+
+template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false, bool STAGED = false>
 struct GemmSmem {
   static constexpr int kWgN = 3 - WG_M;                          // warpgroups along N
   static constexpr int kPlanes = SPLIT ? 2 : 1;
@@ -69,7 +85,13 @@ struct GemmSmem {
   static constexpr int kBBytes = BN_WG * kRowBytes;              // one warpgroup's weight rows of one plane
   static constexpr int kStageBytes = kABytes + kPlanes * kWgN * kBBytes;   // ... | W_hi blocks (| W_lo blocks)
   static_assert(kBBytes % (SPLIT ? 512 : 1024) == 0, "weight block must keep the swizzle atom's alignment");
-  static constexpr int kOffBars = STAGES * kStageBytes;
+  // staging tile of a 16-bit output tile: [column block of 64][row][128 B] with the 128-byte swizzle, so warpgroup wm's rows of
+  // column block cb are one TMA store box (64 columns x 64 rows) at cb * kStoreCb + wm * 8 KB
+  static constexpr int kStoreCb = 64 * WG_M * 128;
+  static constexpr int kStoreBytes = STAGED ? (kWgN * BN_WG / 64) * kStoreCb : 0;
+  static_assert(!STAGED || BN_WG % 64 == 0, "staged stores go out in 64-column boxes");
+  static constexpr int kOffStore = STAGES * kStageBytes;
+  static constexpr int kOffBars = kOffStore + kStoreBytes;
   static constexpr int kOffStat = kOffBars + 256;                // LN: per-row sum, then sum of squared deviations, of each warpgroup's columns
   static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
   static_assert(2 * STAGES * 8 <= 256, "barrier block overflow");
@@ -84,13 +106,15 @@ LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t a
   else { static_assert(N == 128, "unsupported wgmma width"); wgmma_ss_n128<BF16>(d, da, db, accumulate); }
 }
 
-// grid: (n_tiles, M / (64 WG_M))
+// grid: staged (persistent): up to tiles = n_tiles * M / (64 WG_M) CTAs, otherwise exactly one CTA per tile; map_out: the TMA
+// store map of a staged epilogue (box 64 x 64 rows)
 template <int BN_WG, int WG_M, int STAGES, int EPI, int MODE>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(kGemmThreads<EPI, MODE>, 1)
 gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x 64 WG_M rows*/,
-               const __grid_constant__ OpMaps<MODE> map_b /*box 64 (split: 32) x BN_WG rows*/, const GemmParams p) {
-  constexpr bool BF16 = kOpBf16<MODE>, SPLIT = kOpSplit<MODE>;
-  using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT>;
+               const __grid_constant__ OpMaps<MODE> map_b /*box 64 (split: 32) x BN_WG rows*/,
+               const __grid_constant__ CUtensorMap map_out, const GemmParams p) {
+  constexpr bool BF16 = kOpBf16<MODE>, SPLIT = kOpSplit<MODE>, STAGED = kStagedStore<EPI, SPLIT>;
+  using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT, STAGED>;
   using O = OpT<MODE>;
   constexpr int kKB = SM::kKB;
   constexpr int kBMt = 64 * WG_M, kAcc = BN_WG / 2;
@@ -104,205 +128,260 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int num_kb = (p.K + kKB - 1) / kKB;
-  const int n_mblk = p.M / kBMt;
-  const int m_blk = p.rev ? n_mblk - 1 - static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.y);
-  const int m0 = m_blk * kBMt, n0 = static_cast<int>(blockIdx.x) * BN_WG * SM::kWgN;
+  const int n_mblk = p.M / kBMt, n_work = n_mblk * p.n_tiles;
+  // tile t: row block t / n_tiles (walked from the last one down when rev), column tile t % n_tiles
+  const auto tile_m0 = [&](int t) { const int mb = t / p.n_tiles; return (p.rev ? n_mblk - 1 - mb : mb) * kBMt; };
+  const auto tile_n0 = [&](int t) { return (t % p.n_tiles) * BN_WG * SM::kWgN; };
 
   if (threadIdx.x == kGemmConsumers) {
     tma_prefetch_desc(&map_a.hi);
     tma_prefetch_desc(&map_b.hi);
     if constexpr (SPLIT) { tma_prefetch_desc(&map_a.lo); tma_prefetch_desc(&map_b.lo); }
+    if constexpr (STAGED) tma_prefetch_desc(&map_out);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
     fence_mbar_init();
   }
   __syncthreads();
   pdl_sync();                                                // everything above overlapped the previous kernel's tail
 
-  if (warp == kGemmConsumers / 32) {
+  if (warp >= kGemmConsumers / 32) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
-        uint8_t* st = smem + s * SM::kStageBytes;
-        mbar_arrive_expect_tx(&full[s], SM::kStageBytes);    // out-of-bounds box parts are zero-filled and still counted
-        tma_load_2d(st, &map_a.hi, &full[s], kb * kKB, m0);
+    if constexpr (STAGED) setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == kGemmConsumers) {
+      int s = 0;
+      uint32_t phase = 0;                                    // ring slot and pass, carried from tile to tile
+      for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+        const int m0 = tile_m0(t), n0 = tile_n0(t);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[s], phase ^ 1);
+          uint8_t* st = smem + s * SM::kStageBytes;
+          mbar_arrive_expect_tx(&full[s], SM::kStageBytes);    // out-of-bounds box parts are zero-filled and still counted
+          tma_load_2d(st, &map_a.hi, &full[s], kb * kKB, m0);
 #pragma unroll
-        for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b.hi, &full[s], kb * kKB, n0 + wn * BN_WG);
-        if constexpr (SPLIT) {
-          tma_load_2d(st + SM::kAPlane, &map_a.lo, &full[s], kb * kKB, m0);
+          for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b.hi, &full[s], kb * kKB, n0 + wn * BN_WG);
+          if constexpr (SPLIT) {
+            tma_load_2d(st + SM::kAPlane, &map_a.lo, &full[s], kb * kKB, m0);
 #pragma unroll
-          for (int wn = 0; wn < SM::kWgN; ++wn)
-            tma_load_2d(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes, &map_b.lo, &full[s], kb * kKB, n0 + wn * BN_WG);
+            for (int wn = 0; wn < SM::kWgN; ++wn)
+              tma_load_2d(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes, &map_b.lo, &full[s], kb * kKB, n0 + wn * BN_WG);
+          }
+          if (++s == STAGES) { s = 0; phase ^= 1; }
         }
+        if constexpr (!STAGED) break;                        // one tile per CTA
       }
     }
     return;
   }
 
   // ===================== consumer warpgroups =====================
+  if constexpr (STAGED) setmaxnreg_inc<kConsumerRegs>();
   const int wg = warp >> 2;
   const int wm = WG_M == 2 ? wg : 0, wn = WG_M == 2 ? 0 : wg;
   float acc[kAcc];
 #pragma unroll
   for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(&full[s], (kb / STAGES) & 1);
-    const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
-    if constexpr (!SPLIT) {
-      const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
-      const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
-      wgmma_fence();
-      if (kb * kBK + kBK <= p.K) {
+  int s = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+    const int m0 = tile_m0(t), n0 = tile_n0(t);
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[s], phase);
+      const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
+      if constexpr (!SPLIT) {
+        const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
+        const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
+        wgmma_fence();
+        if (kb * kBK + kBK <= p.K) {
 #pragma unroll
-        for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
-      } else {                                              // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
-        wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
+          for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
+        } else {                                              // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
+          wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
+        }
+      } else {
+        const uint64_t da = make_smem_desc_sw64(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc_sw64(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
+        const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
+        const uint64_t db_lo = make_smem_desc_sw64(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
+        wgmma_fence();
+        // K % 32 is 0 or 16 (d = 464: 16): the tail k-block is a single k-step
+        const int nk = kb * kKB + kKB <= p.K ? kKB / kWgK : 1;
+#pragma unroll
+        for (int k = 0; k < kKB / kWgK; ++k) {
+          if (k < nk) {                                       // +32 B per k-step (>>4 = 2); the small terms first
+            wgmma_ss<true, BN_WG>(acc, da_lo + 2 * k, db + 2 * k, (kb | k) != 0);
+            wgmma_ss<true, BN_WG>(acc, da + 2 * k, db_lo + 2 * k, 1);
+            wgmma_ss<true, BN_WG>(acc, da + 2 * k, db + 2 * k, 1);
+          }
+        }
+      }
+      wgmma_commit();
+      // keep this k-block's MMAs in flight; once the previous k-block's have retired its stage goes back to the producer
+      if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]); }
+      if (++s == STAGES) { s = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]);         // the tile's last stage: refilled with the next tile during the epilogue
+
+    const int rw = (warp & 3) * 16 + (lane >> 2);           // fragment rows rw and rw + 8 of the warpgroup's 64
+    const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
+    const int col0 = n0 + wn * BN_WG + 2 * (lane & 3);        // + 8 j: columns col, col + 1 of n8 block j
+
+    if constexpr (STAGED) {
+      // bias (q-scale | ReLU), 16-bit, into the staging tile; then one thread of the warpgroup stores its 64 rows with TMA
+      float scale = 1.0f;
+      if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
+      const bool leader = (threadIdx.x & 127) == 0;
+      uint8_t* stage = smem + SM::kOffStore + wm * 64 * 128;
+      const uint32_t stage_u32 = smem_u32(stage);            // 32-bit shared addresses: 64-bit generic ones cost registers per column block
+      // one named barrier per warpgroup, with a compile-time id
+      const auto wg_bar = [&]() { if (wg == 0) named_bar_sync(2, 128); else named_bar_sync(3, 128); };
+      if (leader) bulk_wait_group_read<0>();                   // the previous tile's store has read the staging tile
+      wg_bar();
+      const int sw = (rw & 7) << 4;                            // 128-byte swizzle: 16-byte chunk ^= row % 8 (rw + 8: the same)
+#pragma unroll
+      for (int j = 0; j < BN_WG / 8; ++j) {
+        const int c = col0 + 8 * j;
+        if (c >= p.N) continue;                               // columns past N: the TMA store clips them
+        const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
+        float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          if constexpr (EPI == EPI_QKV) v[e] *= scale;
+          if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
+        }
+        const uint32_t blk = stage_u32 + (j >> 3) * SM::kStoreCb + ((((j & 7) << 4) ^ sw) | (4 * (lane & 3)));
+        st_shared_u32(blk + rw * 128, O::pack(v[0], v[1]));
+        st_shared_u32(blk + (rw + 8) * 128, O::pack(v[2], v[3]));
+      }
+      fence_proxy_async_smem();
+      wg_bar();
+      if (leader) {
+#pragma unroll
+        for (int cb = 0; cb < BN_WG / 64; ++cb)
+          if (n0 + cb * 64 < p.N) tma_store_2d(&map_out, stage + cb * SM::kStoreCb, n0 + cb * 64, m0 + wm * 64);
+        bulk_commit_group();
+      }
+    } else if constexpr (EPI != EPI_LN) {
+      float scale = 1.0f;
+      if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
+#pragma unroll
+      for (int j = 0; j < BN_WG / 8; ++j) {
+        const int c = col0 + 8 * j;
+        if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
+        const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
+        float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          if constexpr (EPI == EPI_QKV) v[e] *= scale;
+          if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
+        }
+        if constexpr (EPI == EPI_F32) {
+          float* o = static_cast<float*>(p.out);
+          *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
+          *reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * p.ldo + c) = make_float2(v[2], v[3]);
+        } else {
+          uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
+          uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
+          if constexpr (SPLIT) {
+            uint32_t* l0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row0) * p.ldo + c);
+            uint32_t* l1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row1) * p.ldo + c);
+            O::pack_pair(v[0], v[1], *o0, *l0);
+            O::pack_pair(v[2], v[3], *o1, *l1);
+          } else {
+            *o0 = O::pack(v[0], v[1]);
+            *o1 = O::pack(v[2], v[3]);
+          }
+        }
       }
     } else {
-      const uint64_t da = make_smem_desc_sw64(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc_sw64(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
-      const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
-      const uint64_t db_lo = make_smem_desc_sw64(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
-      wgmma_fence();
-      // K % 32 is 0 or 16 (d = 464: 16): the tail k-block is a single k-step
-      const int nk = kb * kKB + kKB <= p.K ? kKB / kWgK : 1;
+      // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
+      //   y = acc + bias + resid (-> y_out); two-pass row statistics: the row sum over the thread's columns, the quad of lanes
+      //   that shares a row, then the other warpgroup (other 232 columns) through shared memory gives the mean; the sum of
+      //   (y - mean)^2 is reduced the same way.  One pass, E[y^2] - mean^2, loses the variance to cancellation once
+      //   |mean| / std is large.  The sums run over y - pivot, pivot = bias[0] + resid[row][0] (y's column 0 without the GEMM
+      //   term, the same in all 8 threads of a row): their terms are of the row's spread, not of its mean, so the mean of a row
+      //   far from zero comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the
+      //   mean, which every output of the row inherits).  Normalise, 16-bit (+ fp32) outputs.
+      float* ssum = reinterpret_cast<float*>(smem + SM::kOffStat);   // [warpgroup][64 rows] row sums of y - pivot
+      float* ssq = ssum + 2 * 64;                                     // [warpgroup][64 rows] sums of squared deviations
+      const int N = p.N;
+      const float* r0p = p.resid + static_cast<size_t>(row0) * N;
+      const float* r1p = p.resid + static_cast<size_t>(row1) * N;
+      const float piv0 = __ldg(p.bias) + r0p[0], piv1 = __ldg(p.bias) + r1p[0];
+      float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
-      for (int k = 0; k < kKB / kWgK; ++k) {
-        if (k < nk) {                                       // +32 B per k-step (>>4 = 2); the small terms first
-          wgmma_ss<true, BN_WG>(acc, da_lo + 2 * k, db + 2 * k, (kb | k) != 0);
-          wgmma_ss<true, BN_WG>(acc, da + 2 * k, db_lo + 2 * k, 1);
-          wgmma_ss<true, BN_WG>(acc, da + 2 * k, db + 2 * k, 1);
+      for (int j = 0; j < BN_WG / 8; ++j) {
+        const int c = col0 + 8 * j;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+        const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
+        acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
+        acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
+        if (p.y_out != nullptr) {
+          *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
+        acc[4 * j] -= piv0; acc[4 * j + 1] -= piv0; acc[4 * j + 2] -= piv1; acc[4 * j + 3] -= piv1;   // from here on: y - pivot
+        s0 += acc[4 * j] + acc[4 * j + 1];
+        s1 += acc[4 * j + 2] + acc[4 * j + 3];
       }
-    }
-    wgmma_commit();
-    // keep this k-block's MMAs in flight; once the previous k-block's have retired its stage goes back to the producer
-    if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[(kb - 1) % STAGES]); }
-  }
-  wgmma_wait<0>();
-  fence_acc(acc);
-
-  const int rw = (warp & 3) * 16 + (lane >> 2);             // fragment rows rw and rw + 8 of the warpgroup's 64
-  const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
-  const int col0 = n0 + wn * BN_WG + 2 * (lane & 3);        // + 8 j: columns col, col + 1 of n8 block j
-
-  if constexpr (EPI != EPI_LN) {
-    float scale = 1.0f;
-    if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
 #pragma unroll
-    for (int j = 0; j < BN_WG / 8; ++j) {
-      const int c = col0 + 8 * j;
-      if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
-      const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
-      float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        if constexpr (EPI == EPI_QKV) v[e] *= scale;
-        if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
+      for (int o = 1; o <= 2; o <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
       }
-      if constexpr (EPI == EPI_F32) {
-        float* o = static_cast<float*>(p.out);
-        *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
-        *reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * p.ldo + c) = make_float2(v[2], v[3]);
-      } else {
-        uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
-        uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
+      if ((lane & 3) == 0) { ssum[wn * 64 + rw] = s0; ssum[wn * 64 + rw + 8] = s1; }
+      named_bar_sync(1, kGemmConsumers);
+      const float inv_n = 1.0f / static_cast<float>(N);
+      const float mean0 = (s0 + ssum[(wn ^ 1) * 64 + rw]) * inv_n, mean1 = (s1 + ssum[(wn ^ 1) * 64 + rw + 8]) * inv_n;   // mean - pivot, like acc
+      float q0 = 0.0f, q1 = 0.0f;
+#pragma unroll
+      for (int j = 0; j < BN_WG / 8; ++j) {
+        const float d0 = acc[4 * j] - mean0, d1 = acc[4 * j + 1] - mean0, d2 = acc[4 * j + 2] - mean1, d3 = acc[4 * j + 3] - mean1;
+        q0 = fmaf(d0, d0, fmaf(d1, d1, q0));
+        q1 = fmaf(d2, d2, fmaf(d3, d3, q1));
+      }
+#pragma unroll
+      for (int o = 1; o <= 2; o <<= 1) {
+        q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+        q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+      }
+      if ((lane & 3) == 0) { ssq[wn * 64 + rw] = q0; ssq[wn * 64 + rw + 8] = q1; }
+      named_bar_sync(1, kGemmConsumers);
+      const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
+      const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
+      const float* gam = p.ln_scale;
+      const float* bet = p.ln_shift;
+      float gadd = p.adaln ? 1.0f : 0.0f;
+      if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
+        const int layout = m0 / kBM;
+        const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
+        gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
+      }
+      typename O::T* out16 = static_cast<typename O::T*>(p.out);
+#pragma unroll
+      for (int j = 0; j < BN_WG / 8; ++j) {
+        const int c = col0 + 8 * j;
+        const float2 g = __ldg(reinterpret_cast<const float2*>(gam + c)), h = __ldg(reinterpret_cast<const float2*>(bet + c));
+        const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + gadd) + h.y;
+        const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + gadd) + h.y;
         if constexpr (SPLIT) {
-          uint32_t* l0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row0) * p.ldo + c);
-          uint32_t* l1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row1) * p.ldo + c);
-          O::pack_pair(v[0], v[1], *o0, *l0);
-          O::pack_pair(v[2], v[3], *o1, *l1);
+          typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
+          O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
+          O::pack_pair(v2, v3, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row1) * N + c));
         } else {
-          *o0 = O::pack(v[0], v[1]);
-          *o1 = O::pack(v[2], v[3]);
+          *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
+          *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
+        }
+        if (p.out32 != nullptr) {
+          *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
+          *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);
         }
       }
     }
-  } else {
-    // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
-    //   y = acc + bias + resid (-> y_out); two-pass row statistics: the row sum over the thread's columns, the quad of lanes
-    //   that shares a row, then the other warpgroup (other 232 columns) through shared memory gives the mean; the sum of
-    //   (y - mean)^2 is reduced the same way.  One pass, E[y^2] - mean^2, loses the variance to cancellation once
-    //   |mean| / std is large.  The sums run over y - pivot, pivot = bias[0] + resid[row][0] (y's column 0 without the GEMM
-    //   term, the same in all 8 threads of a row): their terms are of the row's spread, not of its mean, so the mean of a row
-    //   far from zero comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the
-    //   mean, which every output of the row inherits).  Normalise, 16-bit (+ fp32) outputs.
-    float* ssum = reinterpret_cast<float*>(smem + SM::kOffStat);   // [warpgroup][64 rows] row sums of y - pivot
-    float* ssq = ssum + 2 * 64;                                     // [warpgroup][64 rows] sums of squared deviations
-    const int N = p.N;
-    const float* r0p = p.resid + static_cast<size_t>(row0) * N;
-    const float* r1p = p.resid + static_cast<size_t>(row1) * N;
-    const float piv0 = __ldg(p.bias) + r0p[0], piv1 = __ldg(p.bias) + r1p[0];
-    float s0 = 0.0f, s1 = 0.0f;
-#pragma unroll
-    for (int j = 0; j < BN_WG / 8; ++j) {
-      const int c = col0 + 8 * j;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-      const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
-      acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
-      acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
-      if (p.y_out != nullptr) {
-        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-      acc[4 * j] -= piv0; acc[4 * j + 1] -= piv0; acc[4 * j + 2] -= piv1; acc[4 * j + 3] -= piv1;   // from here on: y - pivot
-      s0 += acc[4 * j] + acc[4 * j + 1];
-      s1 += acc[4 * j + 2] + acc[4 * j + 3];
-    }
-#pragma unroll
-    for (int o = 1; o <= 2; o <<= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    }
-    if ((lane & 3) == 0) { ssum[wn * 64 + rw] = s0; ssum[wn * 64 + rw + 8] = s1; }
-    named_bar_sync(1, kGemmConsumers);
-    const float inv_n = 1.0f / static_cast<float>(N);
-    const float mean0 = (s0 + ssum[(wn ^ 1) * 64 + rw]) * inv_n, mean1 = (s1 + ssum[(wn ^ 1) * 64 + rw + 8]) * inv_n;   // mean - pivot, like acc
-    float q0 = 0.0f, q1 = 0.0f;
-#pragma unroll
-    for (int j = 0; j < BN_WG / 8; ++j) {
-      const float d0 = acc[4 * j] - mean0, d1 = acc[4 * j + 1] - mean0, d2 = acc[4 * j + 2] - mean1, d3 = acc[4 * j + 3] - mean1;
-      q0 = fmaf(d0, d0, fmaf(d1, d1, q0));
-      q1 = fmaf(d2, d2, fmaf(d3, d3, q1));
-    }
-#pragma unroll
-    for (int o = 1; o <= 2; o <<= 1) {
-      q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-      q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-    }
-    if ((lane & 3) == 0) { ssq[wn * 64 + rw] = q0; ssq[wn * 64 + rw + 8] = q1; }
-    named_bar_sync(1, kGemmConsumers);
-    const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
-    const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
-    const float* gam = p.ln_scale;
-    const float* bet = p.ln_shift;
-    float gadd = p.adaln ? 1.0f : 0.0f;
-    if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
-      const int layout = m0 / kBM;
-      const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
-      gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
-    }
-    typename O::T* out16 = static_cast<typename O::T*>(p.out);
-#pragma unroll
-    for (int j = 0; j < BN_WG / 8; ++j) {
-      const int c = col0 + 8 * j;
-      const float2 g = __ldg(reinterpret_cast<const float2*>(gam + c)), h = __ldg(reinterpret_cast<const float2*>(bet + c));
-      const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + gadd) + h.y;
-      const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + gadd) + h.y;
-      if constexpr (SPLIT) {
-        typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
-        O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
-        O::pack_pair(v2, v3, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row1) * N + c));
-      } else {
-        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
-        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
-      }
-      if (p.out32 != nullptr) {
-        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
-        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);
-      }
-    }
+    if constexpr (!STAGED) break;                            // one tile per CTA
+  }
+  if constexpr (STAGED) {
+    if ((threadIdx.x & 127) == 0) bulk_wait_group_all();   // the last staged stores are complete before the CTA exits
   }
 }
 

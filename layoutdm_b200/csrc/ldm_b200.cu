@@ -4,6 +4,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -43,19 +44,27 @@ constexpr int kMaxLayouts = 32767;  // layouts per call
 constexpr int kLogitLd = 160;       // padded logits row (C <= 160)
 constexpr int kDModel = 464;        // the kernels are laid out for the paper's backbone: d = 464 (LN tiles 224 + 240), ff = 4 d
 // GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, operand mode>
-constexpr int kPlainBN = 256, kPlainStages = 4;   // QKV / FF1: 128 x 256 tiles
+// QKV / FF1: 128 x 256 tiles; 3 ring stages next to the 64 KB store staging tile (one-plane modes), 4 in the split mode,
+// which stores straight from the fragment
+constexpr int kPlainBN = 256;
+template <int MODE> constexpr int kPlainStages = kOpSplit<MODE> ? 4 : 3;
 constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
 constexpr int kLnBN = 232, kLnStages = 3;         // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue)
-template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_QKV, MODE>;
-template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI_RELU, MODE>;
+template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_QKV, MODE>;
+template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_RELU, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
 template <int MODE> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, MODE>;
-constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages>::kBytes;
+template <int MODE>
+constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages<MODE>, kOpSplit<MODE>, kStagedStore<EPI_QKV, kOpSplit<MODE>>>::kBytes;
 constexpr int kHeadSmem = GemmSmem<kHeadBN, 2, kHeadStages>::kBytes;
 constexpr int kLnSmem = GemmSmem<kLnBN, 1, kLnStages>::kBytes;
-// the split mode's stage (two planes of a 32-element k-block) has the bytes of the one-plane 64-element stage: same stage counts
-static_assert(GemmSmem<kPlainBN, 2, kPlainStages, true>::kBytes == kPlainSmem && GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem &&
-              GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem, "split-mode ring stages must keep the one-plane sizes");
+// the split mode's stage (two planes of a 32-element k-block) has the bytes of the one-plane 64-element stage, so the head and
+// LN GEMMs keep their stage counts in every mode (the plain GEMMs trade the staging tile for a fourth stage)
+static_assert(GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem && GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem &&
+              GemmSmem<kPlainBN, 2, 4, true>::kStageBytes == GemmSmem<kPlainBN, 2, 4>::kStageBytes,
+              "split-mode ring stages must keep the one-plane sizes");
+static_assert(kStagedStore<EPI_QKV, false> == kStagedStore<EPI_RELU, false> && kStagedStore<EPI_QKV, true> == kStagedStore<EPI_RELU, true>,
+              "QKV and FF1 share one shared-memory size");
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -137,7 +146,8 @@ struct LdmHandle {
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
-  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
+  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs (m_hid16: also FF1's store map)
+  CUtensorMap m_qkv16_st;                                                    // 64-row boxes: the QKV GEMM's TMA stores (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
@@ -145,6 +155,8 @@ struct LdmHandle {
   // replayed; everything that changes from call to call lives in device memory (noise key block, staged cond / start ids)
   int use_graph = 1;           // env LDM_GRAPH=0: plain stream launches
   int sweep = 1;               // env LDM_SWEEP=0: every kernel walks its row blocks in ascending order (no alternating directions)
+  int num_sms = 0;             // the persistent GEMMs run at most one CTA per SM
+  int gemm_ctas = 0;           // env LDM_GEMM_CTAS=n (n >= 1): at most n CTAs in a persistent GEMM launch; 0: no cap
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
                                // The split mode always launches it: the draw kernels write one 16-bit plane only
   cudaStream_t cap_stream = nullptr;
@@ -293,7 +305,6 @@ void free_workspace(LdmHandle* h) {
 }
 
 int ensure_workspace(LdmHandle* h, int n_layouts) {
-  // the GEMM grids put the row blocks in gridDim.y (<= 65535): 2 per layout for the LN GEMMs
   if (n_layouts > kMaxLayouts) return fail(LDM_ERR_UNSUPPORTED, "batch of %d layouts exceeds the %d a call supports", n_layouts, kMaxLayouts);
   if (n_layouts <= h->cap) return LDM_OK;
   // free the old workspace: nothing may still be running on it, and a failed reallocation must not leave stale pointers behind
@@ -343,6 +354,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64))) return rc;   // the out-projection's A operand
   if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles (128-byte swizzle in every mode)
   if (h->split && (rc = make_map(&h->m_qkv16_lo, h->qkv16_lo, M, kQkvN, kBM, h->bf16))) return rc;
+  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, 64, h->bf16))) return rc;
   if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM))) return rc;
   if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64))) return rc;
   return LDM_OK;
@@ -353,7 +365,17 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   const auto maps = [](const CUtensorMap& hi, const CUtensorMap& lo) { return op_maps<MODE>(hi, lo); };
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
   const int M = n * kBM;
-  const dim3 ln_grid(1, M / 64);          // LN GEMMs: 64 whole rows per CTA
+  // Grids: the GEMMs with TMA-staged stores are persistent (one CTA per SM), their epilogue stores drain under the next tile's
+  // MMAs.  The others store from the fragment, so a CTA has nothing to overlap its epilogue with; one tile per CTA lets the
+  // hardware hand each SM its next tile the moment it is free, which measured faster for them than a static persistent split
+  // (the kernels of the latter run exactly one tile per CTA: LDM_GEMM_CTAS caps the persistent grids only)
+  const auto grid = [&](int tiles, bool persistent) {
+    if (!persistent) return dim3(tiles);
+    return dim3(std::min({tiles, h->num_sms, h->gemm_ctas > 0 ? h->gemm_ctas : tiles}));
+  };
+  const int ln_tiles = M / 64;            // LN GEMMs: 64 whole rows per tile
+  const CUtensorMap no_store{};            // map_out of the epilogues that store from the fragment
+  constexpr bool kStaged = kStagedStore<EPI_QKV, kOpSplit<MODE>>;
   int done = 0;
   // alternating sweep direction: every kernel walks the row blocks opposite to its predecessor (GemmParams::rev); the embedding /
   // draw kernels run their blocks in ascending order, so the first GEMM starts from the end.  LDM_SWEEP=0: always ascending
@@ -373,7 +395,8 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       GemmParams p{M, kQkvN, d, kQkvN / kPlainBN, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
       p.rev = next_rev(); p.out_lo = h->qkv16_lo;
       ProfScope ps(h, CAT_QKV, st);
-      CK(launch_step(h, kGemmQkv<MODE>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]), p));
+      CK(launch_step(h, kGemmQkv<MODE>, grid(p.n_tiles * n, kStaged), kGemmThreads<EPI_QKV, MODE>, kPlainSmem<MODE>, st, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]),
+                     kStaged ? h->m_qkv16_st : no_store, p));
     }
     LDM_STAGE_DONE();
     {
@@ -386,14 +409,15 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
       p.rev = next_rev(); p.out_lo = h->z16_lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(launch_step(h, kGemmLn<MODE>, ln_grid, kGemmThreads, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), p));
+      CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), no_store, p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
       GemmParams p{M, ff, d, (ff + kPlainBN - 1) / kPlainBN, h->b1[l], h->hid16, ff, 1.0f, 0};   // 7 tiles of 256 columns + one of 64
       p.rev = next_rev(); p.out_lo = h->hid16_lo;
       ProfScope ps(h, CAT_FF1, st);
-      CK(launch_step(h, kGemmFf1<MODE>, dim3(p.n_tiles, n), kGemmThreads, kPlainSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]), p));
+      CK(launch_step(h, kGemmFf1<MODE>, grid(p.n_tiles * n, kStaged), kGemmThreads<EPI_RELU, MODE>, kPlainSmem<MODE>, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]),
+                     kStaged ? h->m_hid16 : no_store, p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
@@ -407,7 +431,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(launch_step(h, kGemmLn<MODE>, ln_grid, kGemmThreads, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), p));
+      CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), no_store, p));
     }
     LDM_STAGE_DONE();
   }
@@ -415,7 +439,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, kGemmHead<MODE>, dim3(1, n), kGemmThreads, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), p));
+    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads<EPI_F32, MODE>, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), no_store, p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
@@ -573,6 +597,8 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (const char* e = getenv("LDM_FUSE_EMBED")) h->fuse_embed = atoi(e);
   if (h->split) h->fuse_embed = 0;
   if (const char* e = getenv("LDM_SWEEP")) h->sweep = atoi(e);
+  h->num_sms = prop.multiProcessorCount;
+  if (const char* e = getenv("LDM_GEMM_CTAS")) h->gemm_ctas = std::max(1, atoi(e));
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
   TRY(dev_upload(h, &h->cat_emb, w->cat_emb, static_cast<size_t>(C) * d));
@@ -656,15 +682,15 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   free_staging(h);
 
   if (h->mode == OP_BF16X3) {
-    TRY(set_smem(kGemmQkv<OP_BF16X3>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_BF16X3>, kPlainSmem));
+    TRY(set_smem(kGemmQkv<OP_BF16X3>, kPlainSmem<OP_BF16X3>)); TRY(set_smem(kGemmFf1<OP_BF16X3>, kPlainSmem<OP_BF16X3>));
     TRY(set_smem(kGemmHead<OP_BF16X3>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16X3>, kLnSmem));
     TRY(set_smem(attention_kernel<OP_BF16X3>, kAttSmemBytesSplit));
   } else if (h->mode == OP_BF16) {
-    TRY(set_smem(kGemmQkv<OP_BF16>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_BF16>, kPlainSmem));
+    TRY(set_smem(kGemmQkv<OP_BF16>, kPlainSmem<OP_BF16>)); TRY(set_smem(kGemmFf1<OP_BF16>, kPlainSmem<OP_BF16>));
     TRY(set_smem(kGemmHead<OP_BF16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16>, kLnSmem));
     TRY(set_smem(attention_kernel<OP_BF16>, kAttSmemBytes));
   } else {
-    TRY(set_smem(kGemmQkv<OP_F16>, kPlainSmem)); TRY(set_smem(kGemmFf1<OP_F16>, kPlainSmem));
+    TRY(set_smem(kGemmQkv<OP_F16>, kPlainSmem<OP_F16>)); TRY(set_smem(kGemmFf1<OP_F16>, kPlainSmem<OP_F16>));
     TRY(set_smem(kGemmHead<OP_F16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_F16>, kLnSmem));
     TRY(set_smem(attention_kernel<OP_F16>, kAttSmemBytes));
   }
