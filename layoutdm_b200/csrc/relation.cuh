@@ -28,7 +28,9 @@ struct RelationParams {
 
 LDM_DEVINL float rel_center(const RelationParams& p, int a, int bin) {
   if (p.centers != nullptr) return __ldg(p.centers + a * p.n_bins + bin);
-  return static_cast<float>(a < 2 ? bin : bin + 1) * (1.0f / p.n_bins);        // bbox_tokenizer.py:150-156 (linear decode)
+  // linear decode (bbox_tokenizer.py:150-156): the centres are float32(linspace), i.e. bin / n correctly rounded.  bin * (1 / n)
+  // rounds twice and is an ulp off for some bins when n is not a power of two
+  return __fdiv_rn(static_cast<float>(a < 2 ? bin : bin + 1), static_cast<float>(p.n_bins));
 }
 
 __global__ void __launch_bounds__(kRelThreads) relation_update_kernel(const RelationParams p) {
