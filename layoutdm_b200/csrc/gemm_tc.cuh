@@ -385,4 +385,240 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
   }
 }
 
+// ============ persistent LN GEMM: out-projection / FF2 in the one-plane modes ============
+// 64 x 464 tiles (whole rows), min(tiles, SMs) CTAs of 384 threads; CTA b runs tiles b, b + gridDim.x, ...  The LayerNorm runs
+// in warps of its own and the fp32 traffic goes through bulk copies, so a tile's epilogue overlaps the next tile's MMAs:
+//   warps 0..7  : two MMA warpgroups, 64 rows x 232 columns each, m64n232k16 from the ring.  After a tile's last k-block they
+//                 wait for the tile's residual rows in the tile buffer, replace them by y = acc + (bias + resid) and go
+//                 straight on to the next tile.
+//   warps 8..10 : epilogue: the row statistics, the LayerNorm / AdaLN and the 16-bit stores from the tile buffer.  Warp 8
+//                 also issues the bulk copies of whole rows between the buffer and global memory: y out (the next residual),
+//                 the normalised fp32 rows (written back into the buffer) out, and the next tile's residual rows in.
+//   warp 11     : producer, one lane issues the TMA loads.
+// 168 registers for every warp, no setmaxnreg: ptxas compiles the whole kernel under the launch bound's register count, and a
+// 512-thread block (a whole producer warpgroup) would leave the m64n232 wgmma 128, fewer than it needs.  Three epilogue warps
+// cannot keep enough loads and stores in flight to move a tile's ~300 KB of fp32 rows at HBM rate themselves (~40 us per
+// tile); the bulk copies need no registers.  Ring: 3 stages of 32-element k-blocks with the 64-byte swizzle (the split mode's
+// geometry, one plane): a 64-element k-block leaves room for only 2 stages beside the 118 KB tile buffer.  The split mode keeps
+// the fragment-epilogue kernel above: its two-plane stages do not fit beside the buffer.
+// The results are bit for bit those of the fragment epilogue: the same k16 MMA sequence, y = acc + (bias + resid), and the row
+// statistics keep its summation order (per row 8 chains (h, q), h = column half, q = quad lane, each summing
+// (y_c - piv) + (y_c+1 - piv) over c = 232 h + 8 j + 2 q, j ascending; (q0 + q1) + (q2 + q3), then half + half) and its FMA
+// contractions (y - mean is one fma(-sum, 1/N, y - piv), the output fma(d * rstd, gamma + gadd, beta)).
+constexpr int kLnThreads = 384, kLnEpiThreads = 96;
+struct LnSmem {
+  static constexpr int kRows = 64, kWgCols = 232, kCols = 2 * kWgCols, kStages = 3;
+  static constexpr int kKB = kBKSplit;                           // 32-element k-blocks, 64-byte swizzle rows
+  static constexpr int kABytes = kRows * kKB * 2;
+  static constexpr int kBBytes = kWgCols * kKB * 2;              // one MMA warpgroup's weight rows
+  static constexpr int kStageBytes = kABytes + 2 * kBBytes;
+  static_assert(kABytes % 512 == 0 && kBBytes % 512 == 0, "boxes must keep the 64-byte swizzle atom's alignment");
+  // tile buffer [64][kLd] fp32: the 8-float pad puts the 8 rows of a fragment access in distinct 32-byte bank groups and
+  // keeps every row 16-byte aligned for the bulk copies
+  static constexpr int kLd = kCols + 8;
+  static constexpr int kOffBuf = kStages * kStageBytes;
+  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // full[3], empty[3], res_full, buf_full
+  static constexpr int kOffStat = kOffBars + 64;                 // per row: pivot, row sum of y - pivot, rstd
+  static constexpr int kBytes = kOffStat + 3 * kRows * 4 + 1024 /*align slack*/;
+  static_assert(kLd * 4 % 16 == 0, "bulk copies need 16-byte aligned rows");
+  static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
+};
+
+template <int MODE>
+__global__ void __launch_bounds__(kLnThreads, 1)
+gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-byte swizzle*/,
+               const __grid_constant__ CUtensorMap map_b /*box 32 x 232 rows, 64-byte swizzle*/, const GemmParams p) {
+  static_assert(!kOpSplit<MODE>, "the split mode runs the fragment-epilogue LN GEMM");
+  constexpr bool BF16 = kOpBf16<MODE>;
+  using SM = LnSmem;
+  using O = OpT<MODE>;
+  constexpr int kRows = SM::kRows, kWgCols = SM::kWgCols, kLd = SM::kLd, kAcc = kWgCols / 2;
+  constexpr int kEpi = kGemmConsumers, kProducer = kEpi + kLnEpiThreads;   // first thread of the epilogue warps / producer warp
+
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
+  uint64_t* empty = full + SM::kStages;
+  uint64_t* res_full = empty + SM::kStages;                      // the tile's residual rows have landed in the buffer
+  uint64_t* buf_full = res_full + 1;                             // the MMA warpgroups wrote y into the buffer
+  float* buf = reinterpret_cast<float*>(smem + SM::kOffBuf);
+  float* s_piv = reinterpret_cast<float*>(smem + SM::kOffStat);
+  float* s_sum = s_piv + kRows;
+  float* s_rstd = s_sum + kRows;
+
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  const int N = p.N;
+  const int num_kb = p.K / SM::kKB;                             // K % 32 == 0 (checked at create)
+  const int n_work = p.M / kRows;
+  const auto tile_m0 = [&](int t) { return (p.rev ? n_work - 1 - t : t) * kRows; };
+
+  if (threadIdx.x == kProducer) {
+    tma_prefetch_desc(&map_a);
+    tma_prefetch_desc(&map_b);
+    for (int i = 0; i < SM::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
+    mbar_init(res_full, 1);
+    mbar_init(buf_full, kGemmConsumers);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();                                                // everything above overlapped the previous kernel's tail
+
+  if (threadIdx.x >= kProducer) {
+    // ===================== TMA producer =====================
+    if (threadIdx.x == kProducer) {
+      int s = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+        const int m0 = tile_m0(t);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[s], phase ^ 1);
+          uint8_t* st = smem + s * SM::kStageBytes;
+          mbar_arrive_expect_tx(&full[s], SM::kStageBytes);
+          tma_load_2d(st, &map_a, &full[s], kb * SM::kKB, m0);
+          tma_load_2d(st + SM::kABytes, &map_b, &full[s], kb * SM::kKB, 0);
+          tma_load_2d(st + SM::kABytes + SM::kBBytes, &map_b, &full[s], kb * SM::kKB, kWgCols);
+          if (++s == SM::kStages) { s = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  if (threadIdx.x >= kEpi) {
+    // ===================== epilogue warps =====================
+    const int et = threadIdx.x - kEpi;
+    const bool copier = et < 32;                             // warp 8: the bulk copies, one row per lane at a time
+    const uint32_t row_bytes = static_cast<uint32_t>(N) * sizeof(float);
+    const float inv_n = 1.0f / static_cast<float>(N);
+    constexpr int kVec = kWgCols / 2;                        // float4 columns of a row (116)
+    constexpr int kTotal = kRows * kVec;                     // float4 of a tile; element i = k * 96 + et
+    constexpr int kPerThread = (kTotal + kLnEpiThreads - 1) / kLnEpiThreads;
+    // the residual rows of tile t into the buffer (the buffer is free: every read of it and every bulk store from it is done)
+    const auto load_resid = [&](int t) {
+      if (lane == 0) mbar_arrive_expect_tx(res_full, kRows * row_bytes);
+      __syncwarp();
+      const float* src = p.resid + static_cast<size_t>(tile_m0(t)) * N;
+      for (int r = lane; r < kRows; r += 32) bulk_copy_g2s(buf + r * kLd, src + static_cast<size_t>(r) * N, row_bytes, res_full);
+    };
+    const auto store_rows = [&](float* dst) {                // the buffer's rows to dst, one bulk group per lane
+      for (int r = lane; r < kRows; r += 32) bulk_copy_s2g(dst + static_cast<size_t>(r) * N, buf + r * kLd, row_bytes);
+      bulk_commit_group();
+    };
+    if (copier) load_resid(blockIdx.x);
+    uint32_t bphase = 0;
+    for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+      const int m0 = tile_m0(t);
+      mbar_wait(buf_full, bphase);
+      if (copier && p.y_out != nullptr) store_rows(p.y_out + static_cast<size_t>(m0) * N);
+      // row statistics, a group of 4 rows per warp at a time; lane = 8 row + 4 h + q owns chain (h, q) of its row
+      {
+        const int h = (lane >> 2) & 1, q = lane & 3;
+#pragma unroll 1
+        for (int g = et >> 5; g < kRows / 4; g += kLnEpiThreads / 32) {
+          const int r = 4 * g + (lane >> 3);
+          const float piv = s_piv[r];
+          const float* yr = buf + r * kLd + h * kWgCols + 2 * q;
+          float s = 0.0f;
+#pragma unroll
+          for (int j = 0; j < kWgCols / 8; ++j) {
+            const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
+            s += (y.x - piv) + (y.y - piv);
+          }
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          s += __shfl_xor_sync(0xffffffffu, s, 4);           // the row sum of y - pivot; mean - pivot = s / N
+          float v = 0.0f;
+#pragma unroll
+          for (int j = 0; j < kWgCols / 8; ++j) {
+            const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
+            const float d0 = fmaf(-s, inv_n, y.x - piv), d1 = fmaf(-s, inv_n, y.y - piv);
+            v = fmaf(d0, d0, fmaf(d1, d1, v));
+          }
+          v += __shfl_xor_sync(0xffffffffu, v, 1);
+          v += __shfl_xor_sync(0xffffffffu, v, 2);
+          v += __shfl_xor_sync(0xffffffffu, v, 4);
+          if ((lane & 7) == 0) { s_sum[r] = s; s_rstd[r] = 1.0f / sqrtf(fmaxf(v * inv_n, 0.0f) + 1e-5f); }
+        }
+      }
+      if (copier) bulk_wait_group_read<0>();                 // the y rows are out of the buffer before it is overwritten
+      named_bar_sync(1, kLnEpiThreads);
+      // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a bulk store
+      const float* gam = p.ln_scale;
+      const float* bet = p.ln_shift;
+      float gadd = p.adaln ? 1.0f : 0.0f;
+      if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
+        const int layout = m0 / kBM;
+        const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
+        gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
+      }
+      typename O::T* out16 = static_cast<typename O::T*>(p.out);
+      const bool keep32 = p.out32 != nullptr;
+#pragma unroll 6
+      for (int k = 0; k < kPerThread; ++k) {
+        const int i = k * kLnEpiThreads + et, r = i / kVec, c = (i - r * kVec) * 4;
+        if (i >= kTotal) continue;
+        float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
+        const float4 y = *bp;
+        const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), b = __ldg(reinterpret_cast<const float4*>(bet + c));
+        const float piv = s_piv[r], s = s_sum[r], rstd = s_rstd[r];
+        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + gadd, b.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + gadd, b.y),
+                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + gadd, b.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + gadd, b.w));
+        *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
+        if (keep32) *bp = v;
+      }
+      if (keep32) fence_proxy_async_smem();                  // the fp32 rows are visible to the bulk store
+      named_bar_sync(1, kLnEpiThreads);
+      if (copier) {
+        if (keep32) store_rows(p.out32 + static_cast<size_t>(m0) * N);
+        bulk_wait_group_read<0>();
+        if (t + static_cast<int>(gridDim.x) < n_work) load_resid(t + gridDim.x);
+      }
+      bphase ^= 1;
+    }
+    if (copier) bulk_wait_group_all();                       // the last bulk stores are complete before the CTA exits
+    return;
+  }
+
+  // ===================== MMA warpgroups =====================
+  const int wn = warp >> 2;                                  // column half
+  float acc[kAcc];
+  int s = 0;
+  uint32_t phase = 0, bphase = 0;
+  const int rw = (warp & 3) * 16 + (lane >> 2);              // fragment rows rw and rw + 8 of the tile
+  const int cw = wn * kWgCols + 2 * (lane & 3);              // + 8 j: columns c, c + 1 of n8 block j
+  float* bw = buf + rw * kLd + cw;
+  for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[s], phase);
+      const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
+      const uint64_t da = make_smem_desc_sw64(st);
+      const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < SM::kKB / kWgK; ++k) wgmma_ss<BF16, kWgCols>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step
+      wgmma_commit();
+      if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[s == 0 ? SM::kStages - 1 : s - 1]); }
+      if (++s == SM::kStages) { s = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    mbar_arrive(&empty[s == 0 ? SM::kStages - 1 : s - 1]);
+    // y = acc + (bias + resid) over the residual rows in the buffer; the pivot bias[0] + resid[row][0] of rows rw, rw + 8
+    mbar_wait(res_full, bphase);
+    if (cw == 0) { const float b0 = __ldg(p.bias); s_piv[rw] = b0 + bw[0]; s_piv[rw + 8] = b0 + bw[8 * kLd]; }
+#pragma unroll
+    for (int j = 0; j < kAcc / 4; ++j) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + cw + 8 * j));
+      float2* y0 = reinterpret_cast<float2*>(bw + 8 * j);
+      float2* y1 = reinterpret_cast<float2*>(bw + 8 * kLd + 8 * j);
+      const float2 r0 = *y0, r1 = *y1;
+      *y0 = make_float2(acc[4 * j] + (b.x + r0.x), acc[4 * j + 1] + (b.y + r0.y));
+      *y1 = make_float2(acc[4 * j + 2] + (b.x + r1.x), acc[4 * j + 3] + (b.y + r1.y));
+    }
+    fence_proxy_async_smem();                                // y is visible to the bulk store of y_out
+    mbar_arrive(buf_full);
+    bphase ^= 1;
+  }
+}
+
 }  // namespace ldm

@@ -49,7 +49,10 @@ constexpr int kDModel = 464;        // the kernels are laid out for the paper's 
 constexpr int kPlainBN = 256;
 template <int MODE> constexpr int kPlainStages = kOpSplit<MODE> ? 4 : 3;
 constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
-constexpr int kLnBN = 232, kLnStages = 3;         // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue)
+// out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue).  fp16 / bf16: gemm_ln_kernel (persistent, epilogue
+// warps, 32-element k-blocks: K = 512 and 1856 have no tail); the split mode: the fragment-epilogue kernel below
+constexpr int kLnBN = 232, kLnStages = 3;
+static_assert(LnSmem::kWgCols == kLnBN && kAttN % LnSmem::kKB == 0 && 4 * kDModel % LnSmem::kKB == 0, "persistent LN GEMM shapes");
 template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_QKV, MODE>;
 template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_RELU, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
@@ -146,7 +149,9 @@ struct LdmHandle {
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
-  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs (m_hid16: also FF1's store map)
+  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs (m_att16: 64-byte swizzle;
+                                                                             // m_hid16: FF1's store map, FF2's A operand in the split mode)
+  CUtensorMap m_hid16_k32;                                                   // fp16 / bf16: FF2's A operand (64 rows x 32 columns, 64-byte swizzle)
   CUtensorMap m_qkv16_st;                                                    // 64-row boxes: the QKV GEMM's TMA stores (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
@@ -212,10 +217,11 @@ int pack16(LdmHandle* h, void** dst, void** dst_lo, const float* src_dev, const 
   return LDM_OK;
 }
 
-// TMA descriptor(s) of one GEMM operand plane pair: 128-byte swizzle, split mode: both planes with the 64-byte swizzle
+// TMA descriptor(s) of one GEMM operand plane pair: 128-byte swizzle, split mode: both planes with the 64-byte swizzle.
+// sw64: the 64-byte swizzle in every mode (the LN GEMMs' operands: the persistent LN GEMM's ring holds 32-element k-blocks)
 int make_op_maps(const LdmHandle* h, CUtensorMap* m, CUtensorMap* m_lo, const void* base, const void* base_lo, uint64_t rows, uint64_t cols,
-                 uint32_t box_rows) {
-  int rc = make_map(m, base, rows, cols, box_rows, h->bf16, h->split);
+                 uint32_t box_rows, bool sw64 = false) {
+  int rc = make_map(m, base, rows, cols, box_rows, h->bf16, h->split || sw64);
   if (rc || !h->split) return rc;
   return make_map(m_lo, base_lo, rows, cols, box_rows, h->bf16, true);
 }
@@ -351,12 +357,13 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   h->ws_generation++;
   int rc;
   if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM))) return rc;
-  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64))) return rc;   // the out-projection's A operand
+  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64, true))) return rc;   // the out-projection's A operand
   if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles (128-byte swizzle in every mode)
   if (h->split && (rc = make_map(&h->m_qkv16_lo, h->qkv16_lo, M, kQkvN, kBM, h->bf16))) return rc;
   if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, 64, h->bf16))) return rc;
   if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM))) return rc;
   if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64))) return rc;
+  if (!h->split && (rc = make_map(&h->m_hid16_k32, h->hid16, M, ff, 64, h->bf16, true))) return rc;
   return LDM_OK;
 }
 
@@ -365,10 +372,11 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   const auto maps = [](const CUtensorMap& hi, const CUtensorMap& lo) { return op_maps<MODE>(hi, lo); };
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
   const int M = n * kBM;
-  // Grids: the GEMMs with TMA-staged stores are persistent (one CTA per SM), their epilogue stores drain under the next tile's
-  // MMAs.  The others store from the fragment, so a CTA has nothing to overlap its epilogue with; one tile per CTA lets the
-  // hardware hand each SM its next tile the moment it is free, which measured faster for them than a static persistent split
-  // (the kernels of the latter run exactly one tile per CTA: LDM_GEMM_CTAS caps the persistent grids only)
+  // Grids: the GEMMs with TMA-staged stores and the fp16 / bf16 LN GEMMs (epilogue warps) are persistent (one CTA per SM):
+  // their epilogues run under the next tile's MMAs.  The others store from the fragment, so a CTA has nothing to overlap its
+  // epilogue with; one tile per CTA lets the hardware hand each SM its next tile the moment it is free, which measured faster
+  // for them than a static persistent split (the kernels of the latter run exactly one tile per CTA: LDM_GEMM_CTAS caps the
+  // persistent grids only)
   const auto grid = [&](int tiles, bool persistent) {
     if (!persistent) return dim3(tiles);
     return dim3(std::min({tiles, h->num_sms, h->gemm_ctas > 0 ? h->gemm_ctas : tiles}));
@@ -409,7 +417,10 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
       p.rev = next_rev(); p.out_lo = h->z16_lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), no_store, p));
+      if constexpr (kOpSplit<MODE>)
+        CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), no_store, p));
+      else
+        CK(launch_step(h, gemm_ln_kernel<MODE>, grid(ln_tiles, true), kLnThreads, LnSmem::kBytes, st, h->m_att16, h->m_wo[l], p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
@@ -431,7 +442,10 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), no_store, p));
+      if constexpr (kOpSplit<MODE>)
+        CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), no_store, p));
+      else
+        CK(launch_step(h, gemm_ln_kernel<MODE>, grid(ln_tiles, true), kLnThreads, LnSmem::kBytes, st, h->m_hid16_k32, h->m_w2[l], p));
     }
     LDM_STAGE_DONE();
   }
@@ -652,9 +666,9 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(dev_upload(h, &h->ln2w[l], w->norm2_w + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2b[l], w->norm2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN));   // one warpgroup's weight rows per box
-    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN));
+    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, true));
     TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN));
-    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN));
+    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, true));
   }
   {
     float* tmp = nullptr;
@@ -687,11 +701,11 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(set_smem(attention_kernel<OP_BF16X3>, kAttSmemBytesSplit));
   } else if (h->mode == OP_BF16) {
     TRY(set_smem(kGemmQkv<OP_BF16>, kPlainSmem<OP_BF16>)); TRY(set_smem(kGemmFf1<OP_BF16>, kPlainSmem<OP_BF16>));
-    TRY(set_smem(kGemmHead<OP_BF16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16>, kLnSmem));
+    TRY(set_smem(kGemmHead<OP_BF16>, kHeadSmem)); TRY(set_smem(gemm_ln_kernel<OP_BF16>, LnSmem::kBytes));
     TRY(set_smem(attention_kernel<OP_BF16>, kAttSmemBytes));
   } else {
     TRY(set_smem(kGemmQkv<OP_F16>, kPlainSmem<OP_F16>)); TRY(set_smem(kGemmFf1<OP_F16>, kPlainSmem<OP_F16>));
-    TRY(set_smem(kGemmHead<OP_F16>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_F16>, kLnSmem));
+    TRY(set_smem(kGemmHead<OP_F16>, kHeadSmem)); TRY(set_smem(gemm_ln_kernel<OP_F16>, LnSmem::kBytes));
     TRY(set_smem(attention_kernel<OP_F16>, kAttSmemBytes));
   }
 #undef TRY
