@@ -77,10 +77,10 @@ attention_kernel(const __grid_constant__ OpMaps<MODE> map_qkv /*[M][1536], box 6
 #pragma unroll
   for (int i = 0; i < 64; ++i) s[i] = 0.0f;
   {
-    const uint64_t da = make_smem_desc_sw128(sbase + kAttOffQ + wg * 64 * 128), db = make_smem_desc_sw128(sbase + kAttOffK);
+    const uint64_t da = make_smem_desc<128>(sbase + kAttOffQ + wg * 64 * 128), db = make_smem_desc<128>(sbase + kAttOffK);
     wgmma_fence();
     if constexpr (SPLIT) {
-      const uint64_t da_lo = make_smem_desc_sw128(sbase + kAttOffLo + kAttOffQ + wg * 64 * 128), db_lo = make_smem_desc_sw128(sbase + kAttOffLo + kAttOffK);
+      const uint64_t da_lo = make_smem_desc<128>(sbase + kAttOffLo + kAttOffQ + wg * 64 * 128), db_lo = make_smem_desc<128>(sbase + kAttOffLo + kAttOffK);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         wgmma_ss_n128<true>(s, da_lo + 2 * k, db + 2 * k, k != 0);
@@ -141,7 +141,7 @@ attention_kernel(const __grid_constant__ OpMaps<MODE> map_qkv /*[M][1536], box 6
   if constexpr (SPLIT) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const uint64_t dv = make_smem_desc_sw128(sbase + kAttOffV + k * 2048), dv_lo = make_smem_desc_sw128(sbase + kAttOffLo + kAttOffV + k * 2048);
+      const uint64_t dv = make_smem_desc<128>(sbase + kAttOffV + k * 2048), dv_lo = make_smem_desc<128>(sbase + kAttOffLo + kAttOffV + k * 2048);
       wgmma_rs_n64_tb<true>(o, pl[k], dv, k != 0);
       wgmma_rs_n64_tb<true>(o, pa[k], dv_lo, 1);
       wgmma_rs_n64_tb<true>(o, pa[k], dv, 1);
@@ -149,7 +149,7 @@ attention_kernel(const __grid_constant__ OpMaps<MODE> map_qkv /*[M][1536], box 6
   } else {
 #pragma unroll
     for (int k = 0; k < 8; ++k)                                  // 16 keys per MMA: V advances 16 rows = 2 KB
-      wgmma_rs_n64_tb<BF16>(o, pa[k], make_smem_desc_sw128(sbase + kAttOffV + k * 2048), k != 0);
+      wgmma_rs_n64_tb<BF16>(o, pa[k], make_smem_desc<128>(sbase + kAttOffV + k * 2048), k != 0);
   }
   wgmma_commit();
   wgmma_wait<0>();

@@ -127,27 +127,20 @@ LDM_DEVINL void fence_acc(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Shared-memory matrix descriptor of a 128-byte-swizzled operand tile (what TMA SWIZZLE_128B writes; tile base 1024-B
-// aligned).  K-major: rows of 64 x 16-bit (128 B), 8-row groups 1024 B apart (SBO); a k-step of 16 advances the start
-// address by 32 B.  MN-major (64 contiguous N elements per 128-B row, one row per K index): 8-K-row groups 1024 B apart.
+// Shared-memory matrix descriptor of an operand tile with the SW-byte swizzle (what TMA SWIZZLE_<SW>B writes; tile base
+// aligned to the 8-row swizzle atom, 8 SW bytes).  K-major: rows of SW / 2 16-bit elements (SW bytes), 8-row groups 8 SW bytes
+// apart (SBO); a k-step of 16 advances the start address by 32 B.  MN-major (SW = 128: 64 contiguous N elements per 128-B
+// row, one row per K index): 8-K-row groups 1024 B apart.
 // Bit layout (PTX ISA "matrix descriptor" for wgmma): [0,14) addr>>4, [16,30) LBO>>4 (unused here), [32,46) SBO>>4,
-// [62,64) swizzle mode (1 = 128B).
-LDM_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
+// [62,64) swizzle mode (1 = 128B, 2 = 64B).
+template <int SW>
+LDM_DEVINL uint64_t make_smem_desc(uint32_t smem_addr) {
+  static_assert(SW == 128 || SW == 64, "the kernels use the 128- and 64-byte swizzles");
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 62;
-  return d;
-}
-// The same for a 64-byte-swizzled K-major tile (TMA SWIZZLE_64B; tile base 512-B aligned): rows of 32 x 16-bit (64 B), 8-row
-// groups 512 B apart (SBO); a k-step of 16 advances the start address by 32 B.  Swizzle mode 2 = 64B.
-LDM_DEVINL uint64_t make_smem_desc_sw64(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(2) << 62;
+  d |= static_cast<uint64_t>(8 * SW >> 4) << 32;
+  d |= static_cast<uint64_t>(SW == 128 ? 1 : 2) << 62;
   return d;
 }
 

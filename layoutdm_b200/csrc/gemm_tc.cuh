@@ -188,8 +188,8 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
       mbar_wait(&full[s], phase);
       const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
       if constexpr (!SPLIT) {
-        const uint64_t da = make_smem_desc_sw128(st + wm * 64 * 128);
-        const uint64_t db = make_smem_desc_sw128(st + SM::kABytes + wn * SM::kBBytes);
+        const uint64_t da = make_smem_desc<128>(st + wm * 64 * 128);
+        const uint64_t db = make_smem_desc<128>(st + SM::kABytes + wn * SM::kBBytes);
         wgmma_fence();
         if (kb * kBK + kBK <= p.K) {
 #pragma unroll
@@ -198,9 +198,9 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
           wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
         }
       } else {
-        const uint64_t da = make_smem_desc_sw64(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc_sw64(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
-        const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
-        const uint64_t db_lo = make_smem_desc_sw64(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
+        const uint64_t da = make_smem_desc<64>(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc<64>(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
+        const uint64_t db = make_smem_desc<64>(st + SM::kABytes + wn * SM::kBBytes);
+        const uint64_t db_lo = make_smem_desc<64>(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
         wgmma_fence();
         // K % 32 is 0 or 16 (d = 464: 16): the tail k-block is a single k-step
         const int nk = kb * kKB + kKB <= p.K ? kKB / kWgK : 1;
@@ -591,8 +591,8 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full[s], phase);
       const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
-      const uint64_t da = make_smem_desc_sw64(st);
-      const uint64_t db = make_smem_desc_sw64(st + SM::kABytes + wn * SM::kBBytes);
+      const uint64_t da = make_smem_desc<64>(st);
+      const uint64_t db = make_smem_desc<64>(st + SM::kABytes + wn * SM::kBBytes);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < SM::kKB / kWgK; ++k) wgmma_ss<BF16, kWgCols>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step

@@ -294,9 +294,16 @@ cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), dim3 grid,
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-template <typename K>
-int set_smem(K kernel, int bytes) {
-  CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+// the dynamic shared memory of the kernels of MODE that use more than the default 48 KB
+template <int MODE>
+int set_smem() {
+  constexpr auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  CK(cudaFuncSetAttribute(kGemmQkv<MODE>, attr, kPlainSmem<MODE>));
+  CK(cudaFuncSetAttribute(kGemmFf1<MODE>, attr, kPlainSmem<MODE>));
+  CK(cudaFuncSetAttribute(kGemmHead<MODE>, attr, kHeadSmem));
+  if constexpr (kOpSplit<MODE>) CK(cudaFuncSetAttribute(kGemmLn<MODE>, attr, kLnSmem));
+  else CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE>, attr, LnSmem::kBytes));
+  CK(cudaFuncSetAttribute(attention_kernel<MODE>, attr, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes));
   return LDM_OK;
 }
 
@@ -695,19 +702,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (cudaDeviceSynchronize() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(cudaGetLastError())); }
   free_staging(h);
 
-  if (h->mode == OP_BF16X3) {
-    TRY(set_smem(kGemmQkv<OP_BF16X3>, kPlainSmem<OP_BF16X3>)); TRY(set_smem(kGemmFf1<OP_BF16X3>, kPlainSmem<OP_BF16X3>));
-    TRY(set_smem(kGemmHead<OP_BF16X3>, kHeadSmem)); TRY(set_smem(kGemmLn<OP_BF16X3>, kLnSmem));
-    TRY(set_smem(attention_kernel<OP_BF16X3>, kAttSmemBytesSplit));
-  } else if (h->mode == OP_BF16) {
-    TRY(set_smem(kGemmQkv<OP_BF16>, kPlainSmem<OP_BF16>)); TRY(set_smem(kGemmFf1<OP_BF16>, kPlainSmem<OP_BF16>));
-    TRY(set_smem(kGemmHead<OP_BF16>, kHeadSmem)); TRY(set_smem(gemm_ln_kernel<OP_BF16>, LnSmem::kBytes));
-    TRY(set_smem(attention_kernel<OP_BF16>, kAttSmemBytes));
-  } else {
-    TRY(set_smem(kGemmQkv<OP_F16>, kPlainSmem<OP_F16>)); TRY(set_smem(kGemmFf1<OP_F16>, kPlainSmem<OP_F16>));
-    TRY(set_smem(kGemmHead<OP_F16>, kHeadSmem)); TRY(set_smem(gemm_ln_kernel<OP_F16>, LnSmem::kBytes));
-    TRY(set_smem(attention_kernel<OP_F16>, kAttSmemBytes));
-  }
+  TRY(h->mode == OP_BF16X3 ? set_smem<OP_BF16X3>() : h->mode == OP_BF16 ? set_smem<OP_BF16>() : set_smem<OP_F16>());
 #undef TRY
   *out = h;
   return LDM_OK;

@@ -32,10 +32,13 @@ def main():
         if "posterior_sample" in name: return "posterior_sample"
         if "gemm_tc_kernel" in name:
             a = [x.strip().replace("(int)", "").replace("(bool)", "") for x in name[name.index("<") + 1:name.index(">")].split(",")]
-            epi, stages = int(a[3]), int(a[2])
-            return {0: "qkv_gemm", 1: "ff1_gemm", 2: "head_gemm"}.get(epi, "outproj_gemm" if stages <= 3 else "ff2_gemm")
+            return {0: "qkv_gemm", 1: "ff1_gemm", 2: "head_gemm", 3: "ln_gemm"}[int(a[3])]   # <width, WG_M, stages, epilogue, mode>
+        if "gemm_ln_kernel" in name: return "ln_gemm"
         return name[:24]
     roles = [role_of(r[cols[0]]) for r in data]
+    # the out-projection and FF2 run the same LN GEMM kernel: the out-projection follows attention, FF2 follows FF1 (the window
+    # is one whole step, so the first launch's predecessor is the last one)
+    roles = [{"attention": "outproj_gemm", "ff1_gemm": "ff2_gemm"}[roles[i - 1]] if r == "ln_gemm" else r for i, r in enumerate(roles)]
     assert sorted(roles) == sorted(ORDER), f"launch window is not one whole step: {roles}"
     os.makedirs(os.path.join(REPO, "profiles"), exist_ok=True)
     with open(os.path.join(REPO, "profiles", f"{tag}_ncu_full_summary.csv"), "w", newline="") as f:
