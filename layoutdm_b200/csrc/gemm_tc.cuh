@@ -2,30 +2,24 @@
 //
 //   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 * n_layouts (one 128-row block = one layout)
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
-//   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; see below
+//   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; 16-bit outputs are written as (hi, lo) pairs (out, out_lo)
 //
-// One kernel template, 384 threads; CTA b runs tiles b, b + gridDim.x, ... (the column tile varies fastest, so consecutive
-// tiles share their A row block in L2).  The GEMMs with TMA-staged stores are launched persistent (min(tiles, SMs) CTAs),
-// the others with one CTA per tile:
-//   warps 0..7  : two consumer warpgroups (setmaxnreg: 232 registers).  Each issues m64 x BN_WG x k16 wgmmas from the
-//                 shared-memory ring (fp32 accumulators in registers) and runs the epilogue on its own accumulator fragment.
-//   warps 8..11 : producer warpgroup (setmaxnreg: 40 registers), one lane issues the TMA loads: cp.async.bulk.tensor 2-D
-//                 tiles with the 128-byte swizzle into a STAGES-deep ring, completion on mbarriers (full: TMA bytes landed,
-//                 empty: both warpgroups' MMAs have read the stage).  Ring slot and phase run on across tiles, so the
-//                 producer fills the ring with the next tile while the consumers run this tile's epilogue.
-// Stores: the 16-bit QKV / FF1 epilogues (one-plane modes) write the fragment into a shared-memory staging tile and one
-// thread per warpgroup stores it with TMA; the consumers go on to the next tile while the store drains.  The other epilogues
-// store straight from the fragment.
-// Tile shapes:
+// Both kernels run one operand ring (Ring): a shared-memory ring of k-block stages that one producer lane fills with TMA 2-D
+// boxes and two consumer warpgroups drain with m64 x N x k16 wgmmas into fp32 register accumulators (full / empty mbarriers).
+// CTA b runs tiles b, b + gridDim.x, ..., the column tile fastest (consecutive tiles share their A row block in L2); the ring
+// slot and phase run on from tile to tile, so the producer fills the ring with the next tile during this tile's epilogue.  A
+// split-mode stage holds both planes of a 32-element k-block, A_hi | A_lo | W_hi | W_lo: the bytes (and so the stage counts) of
+// the one-plane 64-element stage.  Each of its k16 steps is three wgmmas: a_lo w_hi, a_hi w_lo, a_hi w_hi.
+//
+// gemm_tc_kernel adds the epilogue on the consumers' own accumulator fragment.  Tile shapes:
 //   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (QKV, FF1: 256 columns; vocabulary head: 160)
 //   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the LN epilogue: 2 x 232 = 464 =
 //              d_model, so a CTA holds whole rows and the LayerNorm row statistics are combined in shared memory.
 // Epilogues:  QKV (bias, q-scale, 16-bit) | RELU (FF1: bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
 //             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused).
-//
-// Split mode: a ring stage holds four boxes, A_hi | A_lo | W_hi | W_lo, of a 32-element k-block with the 64-byte swizzle, so a
-// stage keeps the bytes (and the GEMMs their stage counts) of the 64-element one-plane k-block.  Each k16 step issues three
-// wgmmas into the accumulator: a_lo w_hi, a_hi w_lo, a_hi w_hi.  16-bit outputs are written as (hi, lo) pairs (out, out_lo).
+// The 16-bit QKV / FF1 epilogues of the one-plane modes write the fragment into a staging tile that one thread per warpgroup
+// stores with TMA while the consumers go on to the next tile (kStagedStore); the others store from the fragment.
+// gemm_ln_kernel (out-projection, FF2 in fp16 / bf16) adds a tile buffer and epilogue warps of its own (see there).
 //
 // Reference ops replaced: nn.Linear / nn.MultiheadAttention projections / nn.LayerNorm / AdaLayerNorm in
 // T/models/transformer_utils.py:79-83,165-210 and T/models/common/nn_lib.py:187-189,235.
@@ -35,11 +29,12 @@
 namespace ldm {
 
 constexpr int kBM = 128;       // rows of one layout tile (125 tokens + 3 pad rows)
-constexpr int kBK = 64;        // K elements per smem stage (= 128 B = one swizzle row)
-constexpr int kBKSplit = 32;   // split mode: K elements per stage and plane (= 64 B = one 64-byte swizzle row)
 constexpr int kWgK = 16;       // K per wgmma (16-bit operands)
 constexpr int kGemmConsumers = 256;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // persistent block: 128 x 40 + 256 x 232 <= the SM's 64 K registers
+
+// K elements per ring k-block of gemm_tc_kernel: 64 with one plane, 32 per plane in the split mode (the stage keeps its bytes)
+constexpr int gemm_kb(bool split) { return split ? 32 : 64; }
 
 enum : int { EPI_QKV = 0, EPI_RELU = 1, EPI_F32 = 2, EPI_LN = 3 };
 
@@ -65,6 +60,110 @@ struct GemmParams {
   void* out_lo;           // split mode: lo plane of the 16-bit output (same layout as out)
 };
 
+template <bool BF16, int N>
+LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 256) wgmma_ss_n256<BF16>(d, da, db, accumulate);
+  else if constexpr (N == 232) wgmma_ss_n232<BF16>(d, da, db, accumulate);
+  else if constexpr (N == 160) wgmma_ss_n160<BF16>(d, da, db, accumulate);
+  else { static_assert(N == 128, "unsupported wgmma width"); wgmma_ss_n128<BF16>(d, da, db, accumulate); }
+}
+
+// The operand ring: STAGES stages, each [A rows][KB] per plane | [B_ROWS weight rows][KB] per plane and column warpgroup.
+// One smem row is one swizzle row of 2 KB bytes: the operand maps' boxes are KB columns with the (2 KB)-byte swizzle, read by
+// make_smem_desc<2 KB>.  K_TAIL: K may end in a partial k-block (K % KB is 0 or 16: K = 464, 512, 1856); a k-block that runs
+// past K issues a single k16 step.  Each role keeps its own cursor (slot s, pass phase) and passes it in.
+template <int KB, int PLANES, int A_ROWS, int B_ROWS, int WG_N, int STAGES, bool K_TAIL = true>
+struct Ring {
+  static constexpr int kKB = KB, kStages = STAGES, kWgN = WG_N;
+  static constexpr int kRowBytes = 2 * KB;
+  static constexpr int kAPlane = A_ROWS * kRowBytes;
+  static constexpr int kABytes = PLANES * kAPlane;                  // A_hi (| A_lo)
+  static constexpr int kBBytes = B_ROWS * kRowBytes;                // one warpgroup's weight rows of one plane
+  static constexpr int kStageBytes = kABytes + PLANES * WG_N * kBBytes;   // ... | W_hi blocks (| W_lo blocks)
+  static constexpr int kBytes = STAGES * kStageBytes;
+  static_assert(kAPlane % (8 * kRowBytes) == 0 && kBBytes % (8 * kRowBytes) == 0, "boxes must keep the swizzle atom's alignment");
+
+  uint8_t* stages;
+  uint64_t* full;                                                   // [STAGES] the stage's TMA bytes have landed
+  uint64_t* empty;                                                  // [STAGES] both warpgroups' MMAs have read the stage
+
+  LDM_DEVINL Ring(uint8_t* smem, uint64_t* bars) : stages(smem), full(bars), empty(bars + STAGES) {}
+  static LDM_DEVINL int num_kb(int K) { return K_TAIL ? (K + KB - 1) / KB : K / KB; }
+
+  template <int MODE>
+  static LDM_DEVINL void prefetch(const OpMaps<MODE>& a, const OpMaps<MODE>& b) {
+    tma_prefetch_desc(&a.hi);
+    tma_prefetch_desc(&b.hi);
+    if constexpr (kOpSplit<MODE>) { tma_prefetch_desc(&a.lo); tma_prefetch_desc(&b.lo); }
+  }
+  LDM_DEVINL void init() const {
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
+  }
+  static LDM_DEVINL void advance(int& s, uint32_t& phase) { if (++s == STAGES) { s = 0; phase ^= 1; } }
+  LDM_DEVINL void release_prev(int s) const { mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]); }
+
+  // producer lane: the num_kb k-blocks of one tile, A rows m0.., weight block wn's rows n0 + wn * B_ROWS..
+  template <int MODE>
+  LDM_DEVINL void load_tile(int& s, uint32_t& phase, const OpMaps<MODE>& a, const OpMaps<MODE>& b, int num_kb, int m0, int n0) const {
+    static_assert(PLANES == (kOpSplit<MODE> ? 2 : 1), "one operand map per plane");
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&empty[s], phase ^ 1);
+      uint8_t* st = stages + s * kStageBytes;
+      mbar_arrive_expect_tx(&full[s], kStageBytes);              // out-of-bounds box parts are zero-filled and still counted
+      tma_load_2d(st, &a.hi, &full[s], kb * KB, m0);
+#pragma unroll
+      for (int wn = 0; wn < WG_N; ++wn) tma_load_2d(st + kABytes + wn * kBBytes, &b.hi, &full[s], kb * KB, n0 + wn * B_ROWS);
+      if constexpr (PLANES == 2) {
+        tma_load_2d(st + kAPlane, &a.lo, &full[s], kb * KB, m0);
+#pragma unroll
+        for (int wn = 0; wn < WG_N; ++wn)
+          tma_load_2d(st + kABytes + (WG_N + wn) * kBBytes, &b.lo, &full[s], kb * KB, n0 + wn * B_ROWS);
+      }
+      advance(s, phase);
+    }
+  }
+
+  // consumer warpgroup (A rows wm * 64.., weight block wn): the MMAs of one tile's num_kb k-blocks into acc.  A k-block's MMAs
+  // stay in flight while the next k-block's are issued; once they have retired its stage goes back to the producer.  The
+  // tile's last stage goes back before the epilogue, so the producer refills it with the next tile meanwhile.
+  template <int MODE>
+  LDM_DEVINL void mma_tile(int& s, uint32_t& phase, float (&acc)[B_ROWS / 2], int wm, int wn, int num_kb, int K) const {
+    static_assert(PLANES == (kOpSplit<MODE> ? 2 : 1), "one operand map per plane");
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[s], phase);
+      const uint32_t st = smem_u32(stages + s * kStageBytes);
+      const uint64_t da = make_smem_desc<kRowBytes>(st + wm * 64 * kRowBytes), da_lo = make_smem_desc<kRowBytes>(st + kAPlane + wm * 64 * kRowBytes);
+      const uint64_t db = make_smem_desc<kRowBytes>(st + kABytes + wn * kBBytes);
+      const uint64_t db_lo = make_smem_desc<kRowBytes>(st + kABytes + (WG_N + wn) * kBBytes);
+      wgmma_fence();
+      // k16 step k: +32 B (>>4 = 2); two planes: three wgmmas, the small terms first
+      const auto step = [&](int k) {
+        if constexpr (PLANES == 2) {
+          wgmma_ss<true, B_ROWS>(acc, da_lo + 2 * k, db + 2 * k, (kb | k) != 0);
+          wgmma_ss<true, B_ROWS>(acc, da + 2 * k, db_lo + 2 * k, 1);
+          wgmma_ss<true, B_ROWS>(acc, da + 2 * k, db + 2 * k, 1);
+        } else {
+          wgmma_ss<kOpBf16<MODE>, B_ROWS>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        }
+      };
+      // two-plane stages issue their first step ahead of the K-tail branch, one-plane stages inside it: other shapes of the same
+      // rule change ptxas's wgmma schedule.  Without K_TAIL there is no branch (ptxas serialises the LN kernel's wgmmas around one)
+      const bool whole = !K_TAIL || kb * KB + KB <= K;
+      if (PLANES == 2 || !whole) step(0);
+      if (whole) {
+#pragma unroll
+        for (int k = PLANES == 2 ? 1 : 0; k < KB / kWgK; ++k) step(k);
+      }
+      wgmma_commit();
+      if (kb > 0) { wgmma_wait<1>(); release_prev(s); }
+      advance(s, phase);
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    release_prev(s);
+  }
+};
+
 // TMA-staged stores: the 16-bit plain epilogues of the one-plane modes (the split mode's (hi, lo) pair outputs would need two
 // staging tiles, which leave too few ring stages).  These GEMMs are the persistent ones: 384 threads (producer warpgroup),
 // min(tiles, SMs) CTAs.  The others store from the fragment, have nothing to overlap their epilogue with, and run one tile per
@@ -76,21 +175,13 @@ constexpr int kGemmThreads = kStagedStore<EPI, kOpSplit<MODE>> ? 384 : 288;
 
 template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false, bool STAGED = false>
 struct GemmSmem {
-  static constexpr int kWgN = 3 - WG_M;                          // warpgroups along N
-  static constexpr int kPlanes = SPLIT ? 2 : 1;
-  static constexpr int kKB = SPLIT ? kBKSplit : kBK;             // K elements per stage
-  static constexpr int kRowBytes = kKB * 2;                      // one smem row = one swizzle row (128 B, split: 64 B)
-  static constexpr int kAPlane = 64 * WG_M * kRowBytes;
-  static constexpr int kABytes = kPlanes * kAPlane;              // A_hi (| A_lo)
-  static constexpr int kBBytes = BN_WG * kRowBytes;              // one warpgroup's weight rows of one plane
-  static constexpr int kStageBytes = kABytes + kPlanes * kWgN * kBBytes;   // ... | W_hi blocks (| W_lo blocks)
-  static_assert(kBBytes % (SPLIT ? 512 : 1024) == 0, "weight block must keep the swizzle atom's alignment");
+  using R = Ring<gemm_kb(SPLIT), SPLIT ? 2 : 1, 64 * WG_M, BN_WG, 3 - WG_M, STAGES>;
   // staging tile of a 16-bit output tile: [column block of 64][row][128 B] with the 128-byte swizzle, so warpgroup wm's rows of
   // column block cb are one TMA store box (64 columns x 64 rows) at cb * kStoreCb + wm * 8 KB
   static constexpr int kStoreCb = 64 * WG_M * 128;
-  static constexpr int kStoreBytes = STAGED ? (kWgN * BN_WG / 64) * kStoreCb : 0;
+  static constexpr int kStoreBytes = STAGED ? (R::kWgN * BN_WG / 64) * kStoreCb : 0;
   static_assert(!STAGED || BN_WG % 64 == 0, "staged stores go out in 64-column boxes");
-  static constexpr int kOffStore = STAGES * kStageBytes;
+  static constexpr int kOffStore = R::kBytes;
   static constexpr int kOffBars = kOffStore + kStoreBytes;
   static constexpr int kOffStat = kOffBars + 256;                // LN: per-row sum, then sum of squared deviations, of each warpgroup's columns
   static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
@@ -98,47 +189,59 @@ struct GemmSmem {
   static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
 };
 
-template <bool BF16, int N>
-LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (N == 256) wgmma_ss_n256<BF16>(d, da, db, accumulate);
-  else if constexpr (N == 232) wgmma_ss_n232<BF16>(d, da, db, accumulate);
-  else if constexpr (N == 160) wgmma_ss_n160<BF16>(d, da, db, accumulate);
-  else { static_assert(N == 128, "unsupported wgmma width"); wgmma_ss_n128<BF16>(d, da, db, accumulate); }
+// bias (q-scale | ReLU) of n8 block j of a plain epilogue's fragment: v = rows rw, rw + 8 x columns c, c + 1
+template <int EPI, int N>
+LDM_DEVINL void bias_act(const float (&acc)[N], int j, const float* bias, int c, float scale, float (&v)[4]) {
+  const float2 b = bias != nullptr ? __ldg(reinterpret_cast<const float2*>(bias + c)) : make_float2(0.0f, 0.0f);
+  v[0] = acc[4 * j] + b.x; v[1] = acc[4 * j + 1] + b.y; v[2] = acc[4 * j + 2] + b.x; v[3] = acc[4 * j + 3] + b.y;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    if constexpr (EPI == EPI_QKV) v[e] *= scale;
+    if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
+  }
+}
+
+// the LayerNorm's (gamma, beta) rows of the tile at row m0 and the offset added to gamma (AdaLN: gamma = 1 + scale)
+struct LnAffine { const float* gam; const float* bet; float gadd; };
+LDM_DEVINL LnAffine ln_affine(const float* scale, const float* shift, int adaln, const int* t_layout, int n_layouts, int m0, int N) {
+  LnAffine a{scale, shift, adaln ? 1.0f : 0.0f};
+  if (t_layout != nullptr) {                                 // per-layout timesteps: this layout's AdaLN (scale, shift) row
+    const int layout = m0 / kBM;
+    const int tl = layout < n_layouts ? __ldg(t_layout + layout) : 0;
+    a.gam = scale + static_cast<size_t>(tl) * 2 * N; a.bet = a.gam + N; a.gadd = 1.0f;
+  }
+  return a;
 }
 
 // grid: staged (persistent): up to tiles = n_tiles * M / (64 WG_M) CTAs, otherwise exactly one CTA per tile; map_out: the TMA
 // store map of a staged epilogue (box 64 x 64 rows)
 template <int BN_WG, int WG_M, int STAGES, int EPI, int MODE>
 __global__ void __launch_bounds__(kGemmThreads<EPI, MODE>, 1)
-gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x 64 WG_M rows*/,
-               const __grid_constant__ OpMaps<MODE> map_b /*box 64 (split: 32) x BN_WG rows*/,
+gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M rows*/,
+               const __grid_constant__ OpMaps<MODE> map_b /*box KB x BN_WG rows*/,
                const __grid_constant__ CUtensorMap map_out, const GemmParams p) {
-  constexpr bool BF16 = kOpBf16<MODE>, SPLIT = kOpSplit<MODE>, STAGED = kStagedStore<EPI, SPLIT>;
+  constexpr bool SPLIT = kOpSplit<MODE>, STAGED = kStagedStore<EPI, SPLIT>;
   using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT, STAGED>;
   using O = OpT<MODE>;
-  constexpr int kKB = SM::kKB;
   constexpr int kBMt = 64 * WG_M, kAcc = BN_WG / 2;
   static_assert(EPI != EPI_LN || (WG_M == 1 && BN_WG == 232), "LN epilogue is laid out for 464 = 2 x 232 columns");
   static_assert(EPI == EPI_LN || WG_M == 2, "plain epilogues use 128-row tiles");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
-  uint64_t* empty = full + STAGES;
+  typename SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int num_kb = (p.K + kKB - 1) / kKB;
+  const int num_kb = SM::R::num_kb(p.K);
   const int n_mblk = p.M / kBMt, n_work = n_mblk * p.n_tiles;
   // tile t: row block t / n_tiles (walked from the last one down when rev), column tile t % n_tiles
   const auto tile_m0 = [&](int t) { const int mb = t / p.n_tiles; return (p.rev ? n_mblk - 1 - mb : mb) * kBMt; };
-  const auto tile_n0 = [&](int t) { return (t % p.n_tiles) * BN_WG * SM::kWgN; };
+  const auto tile_n0 = [&](int t) { return (t % p.n_tiles) * BN_WG * SM::R::kWgN; };
 
   if (threadIdx.x == kGemmConsumers) {
-    tma_prefetch_desc(&map_a.hi);
-    tma_prefetch_desc(&map_b.hi);
-    if constexpr (SPLIT) { tma_prefetch_desc(&map_a.lo); tma_prefetch_desc(&map_b.lo); }
+    ring.prefetch(map_a, map_b);
     if constexpr (STAGED) tma_prefetch_desc(&map_out);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
+    ring.init();
     fence_mbar_init();
   }
   __syncthreads();
@@ -151,22 +254,7 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
       int s = 0;
       uint32_t phase = 0;                                    // ring slot and pass, carried from tile to tile
       for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-        const int m0 = tile_m0(t), n0 = tile_n0(t);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[s], phase ^ 1);
-          uint8_t* st = smem + s * SM::kStageBytes;
-          mbar_arrive_expect_tx(&full[s], SM::kStageBytes);    // out-of-bounds box parts are zero-filled and still counted
-          tma_load_2d(st, &map_a.hi, &full[s], kb * kKB, m0);
-#pragma unroll
-          for (int wn = 0; wn < SM::kWgN; ++wn) tma_load_2d(st + SM::kABytes + wn * SM::kBBytes, &map_b.hi, &full[s], kb * kKB, n0 + wn * BN_WG);
-          if constexpr (SPLIT) {
-            tma_load_2d(st + SM::kAPlane, &map_a.lo, &full[s], kb * kKB, m0);
-#pragma unroll
-            for (int wn = 0; wn < SM::kWgN; ++wn)
-              tma_load_2d(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes, &map_b.lo, &full[s], kb * kKB, n0 + wn * BN_WG);
-          }
-          if (++s == STAGES) { s = 0; phase ^= 1; }
-        }
+        ring.load_tile(s, phase, map_a, map_b, num_kb, tile_m0(t), tile_n0(t));
         if constexpr (!STAGED) break;                        // one tile per CTA
       }
     }
@@ -184,43 +272,7 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
   uint32_t phase = 0;
   for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
     const int m0 = tile_m0(t), n0 = tile_n0(t);
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full[s], phase);
-      const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
-      if constexpr (!SPLIT) {
-        const uint64_t da = make_smem_desc<128>(st + wm * 64 * 128);
-        const uint64_t db = make_smem_desc<128>(st + SM::kABytes + wn * SM::kBBytes);
-        wgmma_fence();
-        if (kb * kBK + kBK <= p.K) {
-#pragma unroll
-          for (int k = 0; k < kBK / kWgK; ++k) wgmma_ss<BF16, BN_WG>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step (>>4 = 2)
-        } else {                                              // K tail of 16 (K % 64 is 0 or 16, checked at create): one k-step
-          wgmma_ss<BF16, BN_WG>(acc, da, db, kb != 0);
-        }
-      } else {
-        const uint64_t da = make_smem_desc<64>(st + wm * 64 * SM::kRowBytes), da_lo = make_smem_desc<64>(st + SM::kAPlane + wm * 64 * SM::kRowBytes);
-        const uint64_t db = make_smem_desc<64>(st + SM::kABytes + wn * SM::kBBytes);
-        const uint64_t db_lo = make_smem_desc<64>(st + SM::kABytes + (SM::kWgN + wn) * SM::kBBytes);
-        wgmma_fence();
-        // K % 32 is 0 or 16 (d = 464: 16): the tail k-block is a single k-step
-        const int nk = kb * kKB + kKB <= p.K ? kKB / kWgK : 1;
-#pragma unroll
-        for (int k = 0; k < kKB / kWgK; ++k) {
-          if (k < nk) {                                       // +32 B per k-step (>>4 = 2); the small terms first
-            wgmma_ss<true, BN_WG>(acc, da_lo + 2 * k, db + 2 * k, (kb | k) != 0);
-            wgmma_ss<true, BN_WG>(acc, da + 2 * k, db_lo + 2 * k, 1);
-            wgmma_ss<true, BN_WG>(acc, da + 2 * k, db + 2 * k, 1);
-          }
-        }
-      }
-      wgmma_commit();
-      // keep this k-block's MMAs in flight; once the previous k-block's have retired its stage goes back to the producer
-      if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]); }
-      if (++s == STAGES) { s = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    fence_acc(acc);
-    mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]);         // the tile's last stage: refilled with the next tile during the epilogue
+    ring.template mma_tile<MODE>(s, phase, acc, wm, wn, num_kb, p.K);
 
     const int rw = (warp & 3) * 16 + (lane >> 2);           // fragment rows rw and rw + 8 of the warpgroup's 64
     const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
@@ -242,13 +294,8 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
       for (int j = 0; j < BN_WG / 8; ++j) {
         const int c = col0 + 8 * j;
         if (c >= p.N) continue;                               // columns past N: the TMA store clips them
-        const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
-        float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          if constexpr (EPI == EPI_QKV) v[e] *= scale;
-          if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
-        }
+        float v[4];
+        bias_act<EPI>(acc, j, p.bias, c, scale, v);
         const uint32_t blk = stage_u32 + (j >> 3) * SM::kStoreCb + ((((j & 7) << 4) ^ sw) | (4 * (lane & 3)));
         st_shared_u32(blk + rw * 128, O::pack(v[0], v[1]));
         st_shared_u32(blk + (rw + 8) * 128, O::pack(v[2], v[3]));
@@ -268,13 +315,8 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
       for (int j = 0; j < BN_WG / 8; ++j) {
         const int c = col0 + 8 * j;
         if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
-        const float2 b = p.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.0f, 0.0f);
-        float v[4] = {acc[4 * j] + b.x, acc[4 * j + 1] + b.y, acc[4 * j + 2] + b.x, acc[4 * j + 3] + b.y};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          if constexpr (EPI == EPI_QKV) v[e] *= scale;
-          if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
-        }
+        float v[4];
+        bias_act<EPI>(acc, j, p.bias, c, scale, v);
         if constexpr (EPI == EPI_F32) {
           float* o = static_cast<float*>(p.out);
           *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
@@ -349,21 +391,14 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
       named_bar_sync(1, kGemmConsumers);
       const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
       const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
-      const float* gam = p.ln_scale;
-      const float* bet = p.ln_shift;
-      float gadd = p.adaln ? 1.0f : 0.0f;
-      if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
-        const int layout = m0 / kBM;
-        const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
-        gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
-      }
+      const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
       typename O::T* out16 = static_cast<typename O::T*>(p.out);
 #pragma unroll
       for (int j = 0; j < BN_WG / 8; ++j) {
         const int c = col0 + 8 * j;
-        const float2 g = __ldg(reinterpret_cast<const float2*>(gam + c)), h = __ldg(reinterpret_cast<const float2*>(bet + c));
-        const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + gadd) + h.y;
-        const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + gadd) + h.y;
+        const float2 g = __ldg(reinterpret_cast<const float2*>(a.gam + c)), h = __ldg(reinterpret_cast<const float2*>(a.bet + c));
+        const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + a.gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + a.gadd) + h.y;
+        const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + a.gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + a.gadd) + h.y;
         if constexpr (SPLIT) {
           typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
           O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
@@ -407,17 +442,13 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 64 (split: 32) x
 // contractions (y - mean is one fma(-sum, 1/N, y - piv), the output fma(d * rstd, gamma + gadd, beta)).
 constexpr int kLnThreads = 384, kLnEpiThreads = 96;
 struct LnSmem {
-  static constexpr int kRows = 64, kWgCols = 232, kCols = 2 * kWgCols, kStages = 3;
-  static constexpr int kKB = kBKSplit;                           // 32-element k-blocks, 64-byte swizzle rows
-  static constexpr int kABytes = kRows * kKB * 2;
-  static constexpr int kBBytes = kWgCols * kKB * 2;              // one MMA warpgroup's weight rows
-  static constexpr int kStageBytes = kABytes + 2 * kBBytes;
-  static_assert(kABytes % 512 == 0 && kBBytes % 512 == 0, "boxes must keep the 64-byte swizzle atom's alignment");
+  static constexpr int kRows = 64, kWgCols = 232, kCols = 2 * kWgCols;
+  using R = Ring<32, 1, kRows, kWgCols, 2, 3, false>;          // K = 512, 1856 (checked at create)
   // tile buffer [64][kLd] fp32: the 8-float pad puts the 8 rows of a fragment access in distinct 32-byte bank groups and
   // keeps every row 16-byte aligned for the bulk copies
   static constexpr int kLd = kCols + 8;
-  static constexpr int kOffBuf = kStages * kStageBytes;
-  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // full[3], empty[3], res_full, buf_full
+  static constexpr int kOffBuf = R::kBytes;
+  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // ring full[3], empty[3]; res_full, buf_full
   static constexpr int kOffStat = kOffBars + 64;                 // per row: pivot, row sum of y - pivot, rstd
   static constexpr int kBytes = kOffStat + 3 * kRows * 4 + 1024 /*align slack*/;
   static_assert(kLd * 4 % 16 == 0, "bulk copies need 16-byte aligned rows");
@@ -426,10 +457,9 @@ struct LnSmem {
 
 template <int MODE>
 __global__ void __launch_bounds__(kLnThreads, 1)
-gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-byte swizzle*/,
-               const __grid_constant__ CUtensorMap map_b /*box 32 x 232 rows, 64-byte swizzle*/, const GemmParams p) {
+gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 64 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 232 rows*/,
+               const GemmParams p) {
   static_assert(!kOpSplit<MODE>, "the split mode runs the fragment-epilogue LN GEMM");
-  constexpr bool BF16 = kOpBf16<MODE>;
   using SM = LnSmem;
   using O = OpT<MODE>;
   constexpr int kRows = SM::kRows, kWgCols = SM::kWgCols, kLd = SM::kLd, kAcc = kWgCols / 2;
@@ -437,9 +467,8 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
-  uint64_t* empty = full + SM::kStages;
-  uint64_t* res_full = empty + SM::kStages;                      // the tile's residual rows have landed in the buffer
+  SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
+  uint64_t* res_full = ring.empty + SM::R::kStages;             // the tile's residual rows have landed in the buffer
   uint64_t* buf_full = res_full + 1;                             // the MMA warpgroups wrote y into the buffer
   float* buf = reinterpret_cast<float*>(smem + SM::kOffBuf);
   float* s_piv = reinterpret_cast<float*>(smem + SM::kOffStat);
@@ -448,14 +477,13 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int N = p.N;
-  const int num_kb = p.K / SM::kKB;                             // K % 32 == 0 (checked at create)
+  const int num_kb = SM::R::num_kb(p.K);
   const int n_work = p.M / kRows;
   const auto tile_m0 = [&](int t) { return (p.rev ? n_work - 1 - t : t) * kRows; };
 
   if (threadIdx.x == kProducer) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
-    for (int i = 0; i < SM::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
+    ring.prefetch(map_a, map_b);
+    ring.init();
     mbar_init(res_full, 1);
     mbar_init(buf_full, kGemmConsumers);
     fence_mbar_init();
@@ -466,20 +494,9 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
   if (threadIdx.x >= kProducer) {
     // ===================== TMA producer =====================
     if (threadIdx.x == kProducer) {
-      int s = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-        const int m0 = tile_m0(t);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[s], phase ^ 1);
-          uint8_t* st = smem + s * SM::kStageBytes;
-          mbar_arrive_expect_tx(&full[s], SM::kStageBytes);
-          tma_load_2d(st, &map_a, &full[s], kb * SM::kKB, m0);
-          tma_load_2d(st + SM::kABytes, &map_b, &full[s], kb * SM::kKB, 0);
-          tma_load_2d(st + SM::kABytes + SM::kBBytes, &map_b, &full[s], kb * SM::kKB, kWgCols);
-          if (++s == SM::kStages) { s = 0; phase ^= 1; }
-        }
-      }
+      int s = 0;
+      for (int t = blockIdx.x; t < n_work; t += gridDim.x) ring.load_tile(s, phase, map_a, map_b, num_kb, tile_m0(t), 0);
     }
     return;
   }
@@ -543,14 +560,7 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
       if (copier) bulk_wait_group_read<0>();                 // the y rows are out of the buffer before it is overwritten
       named_bar_sync(1, kLnEpiThreads);
       // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a bulk store
-      const float* gam = p.ln_scale;
-      const float* bet = p.ln_shift;
-      float gadd = p.adaln ? 1.0f : 0.0f;
-      if (p.t_layout != nullptr) {                             // per-layout timesteps: this layout's AdaLN (scale, shift) row
-        const int layout = m0 / kBM;
-        const int tl = layout < p.n_layouts ? __ldg(p.t_layout + layout) : 0;
-        gam = p.ln_scale + static_cast<size_t>(tl) * 2 * N; bet = gam + N; gadd = 1.0f;
-      }
+      const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
       typename O::T* out16 = static_cast<typename O::T*>(p.out);
       const bool keep32 = p.out32 != nullptr;
 #pragma unroll 6
@@ -559,10 +569,10 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
         if (i >= kTotal) continue;
         float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
         const float4 y = *bp;
-        const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), b = __ldg(reinterpret_cast<const float4*>(bet + c));
+        const float4 g = __ldg(reinterpret_cast<const float4*>(a.gam + c)), b = __ldg(reinterpret_cast<const float4*>(a.bet + c));
         const float piv = s_piv[r], s = s_sum[r], rstd = s_rstd[r];
-        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + gadd, b.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + gadd, b.y),
-                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + gadd, b.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + gadd, b.w));
+        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, b.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, b.y),
+                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, b.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, b.w));
         *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
         if (keep32) *bp = v;
       }
@@ -588,21 +598,7 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap map_a /*box 32 x 64 rows, 64-
   const int cw = wn * kWgCols + 2 * (lane & 3);              // + 8 j: columns c, c + 1 of n8 block j
   float* bw = buf + rw * kLd + cw;
   for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full[s], phase);
-      const uint32_t st = smem_u32(smem + s * SM::kStageBytes);
-      const uint64_t da = make_smem_desc<64>(st);
-      const uint64_t db = make_smem_desc<64>(st + SM::kABytes + wn * SM::kBBytes);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < SM::kKB / kWgK; ++k) wgmma_ss<BF16, kWgCols>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);   // +32 B per k-step
-      wgmma_commit();
-      if (kb > 0) { wgmma_wait<1>(); mbar_arrive(&empty[s == 0 ? SM::kStages - 1 : s - 1]); }
-      if (++s == SM::kStages) { s = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    fence_acc(acc);
-    mbar_arrive(&empty[s == 0 ? SM::kStages - 1 : s - 1]);
+    ring.mma_tile<MODE>(s, phase, acc, 0, wn, num_kb, p.K);
     // y = acc + (bias + resid) over the residual rows in the buffer; the pivot bias[0] + resid[row][0] of rows rw, rw + 8
     mbar_wait(res_full, bphase);
     if (cw == 0) { const float b0 = __ldg(p.bias); s_piv[rw] = b0 + bw[0]; s_piv[rw + 8] = b0 + bw[8 * kLd]; }

@@ -52,7 +52,9 @@ constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 
 // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue).  fp16 / bf16: gemm_ln_kernel (persistent, epilogue
 // warps, 32-element k-blocks: K = 512 and 1856 have no tail); the split mode: the fragment-epilogue kernel below
 constexpr int kLnBN = 232, kLnStages = 3;
-static_assert(LnSmem::kWgCols == kLnBN && kAttN % LnSmem::kKB == 0 && 4 * kDModel % LnSmem::kKB == 0, "persistent LN GEMM shapes");
+// k-block of the LN GEMMs' operands (the TMA box columns) in every mode: the persistent kernel's, which is the split mode's
+constexpr int kLnKB = LnSmem::R::kKB;
+static_assert(LnSmem::kWgCols == kLnBN && kAttN % kLnKB == 0 && 4 * kDModel % kLnKB == 0 && gemm_kb(true) == kLnKB, "LN GEMM shapes");
 template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_QKV, MODE>;
 template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_RELU, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
@@ -64,7 +66,7 @@ constexpr int kLnSmem = GemmSmem<kLnBN, 1, kLnStages>::kBytes;
 // the split mode's stage (two planes of a 32-element k-block) has the bytes of the one-plane 64-element stage, so the head and
 // LN GEMMs keep their stage counts in every mode (the plain GEMMs trade the staging tile for a fourth stage)
 static_assert(GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem && GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem &&
-              GemmSmem<kPlainBN, 2, 4, true>::kStageBytes == GemmSmem<kPlainBN, 2, 4>::kStageBytes,
+              GemmSmem<kPlainBN, 2, 4, true>::R::kStageBytes == GemmSmem<kPlainBN, 2, 4>::R::kStageBytes,
               "split-mode ring stages must keep the one-plane sizes");
 static_assert(kStagedStore<EPI_QKV, false> == kStagedStore<EPI_RELU, false> && kStagedStore<EPI_QKV, true> == kStagedStore<EPI_RELU, true>,
               "QKV and FF1 share one shared-memory size");
@@ -84,15 +86,15 @@ int load_encode() {
   return LDM_OK;
 }
 
-// 2-D row-major [rows][cols] 16-bit tensor, box = box_rows x 64 columns, 128-byte swizzle, zero OOB fill (TMA operand loads).
-// sw64: box_rows x 32 columns with the 64-byte swizzle (the split-mode GEMM operands).
-int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16, bool sw64 = false) {
+// 2-D row-major [rows][cols] 16-bit tensor, box = box_rows x kb columns with the (2 kb)-byte swizzle (kb = 64 or 32: one box row
+// is one swizzle row, the layout of a ring k-block), zero OOB fill
+int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, int kb, bool bf16) {
   const cuuint64_t dims[2] = {cols, rows};
   const cuuint64_t strides[1] = {cols * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(sw64 ? kBKSplit : kBK), box_rows};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kb), box_rows};
   const cuuint32_t estr[2] = {1, 1};
   CUresult r = g_encode(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims,
-                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                        strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, kb == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu box_rows=%u", (int)r,
                                      (unsigned long long)rows, (unsigned long long)cols, box_rows);
@@ -149,10 +151,8 @@ struct LdmHandle {
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
-  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs (m_att16: 64-byte swizzle;
-                                                                             // m_hid16: FF1's store map, FF2's A operand in the split mode)
-  CUtensorMap m_hid16_k32;                                                   // fp16 / bf16: FF2's A operand (64 rows x 32 columns, 64-byte swizzle)
-  CUtensorMap m_qkv16_st;                                                    // 64-row boxes: the QKV GEMM's TMA stores (one-plane modes)
+  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
+  CUtensorMap m_qkv16_st, m_hid16_st;                                        // 64-row boxes: the QKV / FF1 GEMMs' TMA stores (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
@@ -217,13 +217,12 @@ int pack16(LdmHandle* h, void** dst, void** dst_lo, const float* src_dev, const 
   return LDM_OK;
 }
 
-// TMA descriptor(s) of one GEMM operand plane pair: 128-byte swizzle, split mode: both planes with the 64-byte swizzle.
-// sw64: the 64-byte swizzle in every mode (the LN GEMMs' operands: the persistent LN GEMM's ring holds 32-element k-blocks)
+// TMA descriptor(s) of one 16-bit operand (split mode: both planes), boxes of box_rows x kb elements
 int make_op_maps(const LdmHandle* h, CUtensorMap* m, CUtensorMap* m_lo, const void* base, const void* base_lo, uint64_t rows, uint64_t cols,
-                 uint32_t box_rows, bool sw64 = false) {
-  int rc = make_map(m, base, rows, cols, box_rows, h->bf16, h->split || sw64);
+                 uint32_t box_rows, int kb) {
+  int rc = make_map(m, base, rows, cols, box_rows, kb, h->bf16);
   if (rc || !h->split) return rc;
-  return make_map(m_lo, base_lo, rows, cols, box_rows, h->bf16, true);
+  return make_map(m_lo, base_lo, rows, cols, box_rows, kb, h->bf16);
 }
 
 template <int MODE>
@@ -363,14 +362,16 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   h->cap = n_layouts;
   h->ws_generation++;
   int rc;
-  if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM))) return rc;
-  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64, true))) return rc;   // the out-projection's A operand
-  if ((rc = make_map(&h->m_qkv16, h->qkv16, M, kQkvN, kBM, h->bf16))) return rc;  // attention's Q / K / V head tiles (128-byte swizzle in every mode)
-  if (h->split && (rc = make_map(&h->m_qkv16_lo, h->qkv16_lo, M, kQkvN, kBM, h->bf16))) return rc;
-  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, 64, h->bf16))) return rc;
-  if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM))) return rc;
-  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64))) return rc;
-  if (!h->split && (rc = make_map(&h->m_hid16_k32, h->hid16, M, ff, 64, h->bf16, true))) return rc;
+  const int kb = gemm_kb(h->split);
+  if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM, kb))) return rc;
+  if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM, kb))) return rc;
+  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64, kLnKB))) return rc;
+  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64, kLnKB))) return rc;
+  // attention's Q / K / V head tiles: 128 rows x one padded head, in every mode
+  if ((rc = make_op_maps(h, &h->m_qkv16, &h->m_qkv16_lo, h->qkv16, h->qkv16_lo, M, kQkvN, kBM, kHeadPad))) return rc;
+  // the staged stores: 64 x 64 boxes of the staging tile (128-byte swizzle)
+  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, 64, 64, h->bf16))) return rc;
+  if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16, M, ff, 64, 64, h->bf16))) return rc;
   return LDM_OK;
 }
 
@@ -388,9 +389,14 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     if (!persistent) return dim3(tiles);
     return dim3(std::min({tiles, h->num_sms, h->gemm_ctas > 0 ? h->gemm_ctas : tiles}));
   };
-  const int ln_tiles = M / 64;            // LN GEMMs: 64 whole rows per tile
   const CUtensorMap no_store{};            // map_out of the epilogues that store from the fragment
   constexpr bool kStaged = kStagedStore<EPI_QKV, kOpSplit<MODE>>;
+  // the LN GEMMs (out-projection, FF2), 64 whole rows per tile: the fragment-epilogue kernel in the split mode, the persistent
+  // LN kernel otherwise
+  const auto ln_gemm = [&](const OpMaps<MODE>& a, const OpMaps<MODE>& w, const GemmParams& p) {
+    if constexpr (kOpSplit<MODE>) return launch_step(h, kGemmLn<MODE>, grid(M / 64, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, a, w, no_store, p);
+    else return launch_step(h, gemm_ln_kernel<MODE>, grid(M / 64, true), kLnThreads, LnSmem::kBytes, st, a, w, p);
+  };
   int done = 0;
   // alternating sweep direction: every kernel walks the row blocks opposite to its predecessor (GemmParams::rev); the embedding /
   // draw kernels run their blocks in ascending order, so the first GEMM starts from the end.  LDM_SWEEP=0: always ascending
@@ -424,10 +430,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
       p.rev = next_rev(); p.out_lo = h->z16_lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      if constexpr (kOpSplit<MODE>)
-        CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), no_store, p));
-      else
-        CK(launch_step(h, gemm_ln_kernel<MODE>, grid(ln_tiles, true), kLnThreads, LnSmem::kBytes, st, h->m_att16, h->m_wo[l], p));
+      CK(ln_gemm(maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
@@ -435,7 +438,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       p.rev = next_rev(); p.out_lo = h->hid16_lo;
       ProfScope ps(h, CAT_FF1, st);
       CK(launch_step(h, kGemmFf1<MODE>, grid(p.n_tiles * n, kStaged), kGemmThreads<EPI_RELU, MODE>, kPlainSmem<MODE>, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]),
-                     kStaged ? h->m_hid16 : no_store, p));
+                     kStaged ? h->m_hid16_st : no_store, p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
@@ -449,10 +452,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      if constexpr (kOpSplit<MODE>)
-        CK(launch_step(h, kGemmLn<MODE>, grid(ln_tiles, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), no_store, p));
-      else
-        CK(launch_step(h, gemm_ln_kernel<MODE>, grid(ln_tiles, true), kLnThreads, LnSmem::kBytes, st, h->m_hid16_k32, h->m_w2[l], p));
+      CK(ln_gemm(maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), p));
     }
     LDM_STAGE_DONE();
   }
@@ -672,10 +672,10 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(dev_upload(h, &h->b2[l], w->linear2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2w[l], w->norm2_w + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
     TRY(dev_upload(h, &h->ln2b[l], w->norm2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN));   // one warpgroup's weight rows per box
-    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, true));
-    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN));
-    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, true));
+    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN, gemm_kb(h->split)));   // one warpgroup's weight rows per box
+    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, kLnKB));
+    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN, gemm_kb(h->split)));
+    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, kLnKB));
   }
   {
     float* tmp = nullptr;
@@ -685,7 +685,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     int* hmap_dev = nullptr;
     TRY(dev_upload(h, &hmap_dev, hmap.data(), hmap.size()));
     TRY(pack16(h, &h->whead, &h->whead_lo, tmp, hmap_dev, kLogitLd, d, d));
-    TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN));
+    TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN, gemm_kb(h->split)));
   }
   {
     std::vector<float> sch(static_cast<size_t>(h->G) * 8 * (T + 1));

@@ -1,11 +1,14 @@
-"""GPU (-m gpu): the persistent GEMM schedule computes every output element the same way whatever the CTA count.
+"""GPU (-m gpu): the persistent GEMMs compute every output element the same way whatever the CTA count.
 
-QKV and FF1 in fp16 / bf16 are persistent: min(tiles, SMs) CTAs, each walking tiles b, b + gridDim.x, ... with one
-shared-memory ring whose slot and phase carry over from tile to tile, and a staging tile that the previous tile's TMA store
-may still be reading.  LDM_GEMM_CTAS caps their CTA count: with 1 CTA a single ring runs through every tile of a launch
-(hundreds of tiles, 8 k-blocks each over 3 stages), with 7 the tiles of a row block spread over CTAs in a ragged last round.
-Every other GEMM (and every GEMM of the split mode) runs one CTA per tile whatever the cap.  Each GEMM's tapped output must
-be bitwise equal to the uncapped run's, in every operand mode."""
+The persistent GEMMs run min(tiles, SMs) CTAs, each walking tiles b, b + gridDim.x, ... through one shared-memory operand ring
+whose slot and phase carry over from tile to tile:
+- QKV and FF1 in fp16 / bf16, with a staging tile that the previous tile's TMA store may still be reading;
+- the out-projection and FF2 in fp16 / bf16 (bias + residual + LayerNorm / AdaLN epilogue), with a tile buffer that takes the
+  next tile's residual rows while the MMA warpgroups compute it.  At per-layout timesteps (predict_start) FF2's AdaLN reloads
+  the (scale, shift) row of the tile's own layout, so a CTA's consecutive tiles normalise with different rows.
+LDM_GEMM_CTAS caps their CTA count: with 1 CTA a single ring runs through every tile of a launch (hundreds of tiles), with 7 the
+tiles of a row block spread over CTAs in a ragged last round.  Every other GEMM (and every GEMM of the split mode) runs one CTA
+per tile whatever the cap.  Each GEMM's tapped output must be bitwise equal to the uncapped run's."""
 import pytest
 import torch
 
@@ -20,15 +23,9 @@ LAYERS = 2
 T = 20
 
 
-def taps(split):
-    """launch count to stop after -> the buffers that launch's GEMM writes (0: the whole pass, ending with the head).
-    Launch 1 is the embedding; layer l's launches are 2 + 5 l: QKV, attention, out-projection, FF1, FF2"""
-    lo = (lambda names: names + [n + "_lo" for n in names if n.endswith("16")]) if split else (lambda names: names)
-    last_ff2 = 1 + 5 * LAYERS
-    return {2: lo(["qkv16"]), 4: lo(["y32", "z16"]), 5: lo(["hid16"]), 6: lo(["x32", "x16"]), last_ff2: lo(["z16"]), 0: ["logits"]}
-
-
-def run(monkeypatch, dtype, cap, sd, ids):
+def run(monkeypatch, dtype, cap, sd, taps, call):
+    """taps: launch count to stop after -> the buffers that launch's GEMM writes (0: the whole pass).  Launch 1 is the
+    embedding; layer l's launches are 2 + 5 l: QKV, attention, out-projection, FF1, FF2.  call(engine) runs the pass."""
     from layoutdm_b200 import Engine, Vocab
     vo = O.RICO25
     if cap is None:
@@ -39,9 +36,9 @@ def run(monkeypatch, dtype, cap, sd, ids):
     bits = lambda t: t.view(torch.int16 if t.element_size() == 2 else torch.int32).clone()
     out = {}
     try:
-        for n, names in taps(dtype == "bf16x3").items():
+        for n, names in taps.items():
             G.set_stop_after(eng, n)
-            eng.step(ids, 7, 7, {"name": "deterministic"})
+            call(eng)
             torch.cuda.synchronize()
             for k in names:
                 out[(n, k)] = bits(G.debug_read(eng, k, B, raw=True))
@@ -51,13 +48,31 @@ def run(monkeypatch, dtype, cap, sd, ids):
     return out
 
 
+def check_caps(monkeypatch, dtype, sd, taps, call, what):
+    ref = run(monkeypatch, dtype, None, sd, taps, call)
+    for cap in (1, 7):
+        got = run(monkeypatch, dtype, cap, sd, taps, call)
+        bad = [f"launch {n} {k}" for (n, k), v in ref.items() if not torch.equal(v, got[(n, k)])]
+        assert not bad, f"{dtype}, LDM_GEMM_CTAS={cap}{what}: not bitwise equal to the uncapped run: {bad}"
+
+
 @pytest.mark.parametrize("dtype", ["fp16", "bf16", "bf16x3"])
 def test_gemm_outputs_independent_of_cta_count(monkeypatch, dtype):
     vo, spec = O.RICO25, O.ModelSpec(layers=LAYERS, T=T)
     sd = O.make_weights(vo, spec, seed=5, scale=2.0)
     ids = mixed_ids(B, vo, B).cuda()
-    ref = run(monkeypatch, dtype, None, sd, ids)
-    for cap in (1, 7):
-        got = run(monkeypatch, dtype, cap, sd, ids)
-        bad = [f"launch {n} {k}" for (n, k), v in ref.items() if not torch.equal(v, got[(n, k)])]
-        assert not bad, f"{dtype}, LDM_GEMM_CTAS={cap}: not bitwise equal to the uncapped run: {bad}"
+    lo = (lambda names: names + [n + "_lo" for n in names if n.endswith("16")]) if dtype == "bf16x3" else (lambda names: names)
+    taps = {2: lo(["qkv16"]), 4: lo(["y32", "z16"]), 5: lo(["hid16"]), 6: lo(["x32", "x16"]), 1 + 5 * LAYERS: lo(["z16"]), 0: ["logits"]}
+    check_caps(monkeypatch, dtype, sd, taps, lambda eng: eng.step(ids, 7, 7, {"name": "deterministic"}), "")
+
+
+@pytest.mark.parametrize("dtype", ["fp16", "bf16"])
+def test_ln_gemm_outputs_independent_of_cta_count_per_layout_t(monkeypatch, dtype):
+    vo, spec = O.RICO25, O.ModelSpec(layers=LAYERS, T=T)
+    sd = O.make_weights(vo, spec, seed=6, scale=2.0)
+    ids = mixed_ids(B, vo, 13).cuda()
+    t = torch.randint(0, T, (B,), generator=torch.Generator().manual_seed(8))
+    t[0], t[1] = 0, T - 1
+    t = t.cuda()
+    taps = {4: ["y32", "z16"], 6: ["x32", "x16"], 4 + 5 * (LAYERS - 1): ["y32", "z16"], 1 + 5 * LAYERS: ["z16"]}
+    check_caps(monkeypatch, dtype, sd, taps, lambda eng: eng.predict_start(ids, t), ", per-layout timesteps")
