@@ -107,6 +107,25 @@ typedef struct {
   int32_t top_k;
 } LdmSampling;
 
+/* Where a draw's noise comes from (DESIGN.md §7).
+ *   LDM_NOISE_CONTRACT : the project's Philox contract keyed by (seed, step_ctr, global layout, token, class); offset and
+ *                        total_layouts are not read.
+ *   LDM_NOISE_TORCH    : the numbers torch's CUDA generator with this seed and offset would give the reference's draw
+ *                        (helpers/sampling.py:81-130 on a (total_layouts, C, S) batch: rand_like for name="gumbel", then
+ *                        multinomial's exponential_), so a seeded run reproduces the reference on the GPU.  Step k of a call
+ *                        draws at offset + k * (one step's advance, ldm_noise_advance); layouts [b_global0, b_global0 + B) of
+ *                        total_layouts get the slice of the whole batch's draw.  offset must be a multiple of 4 (torch's
+ *                        offsets are) and total_layouts * S * C < 2^31 (LDM_ERR_UNSUPPORTED otherwise: torch splits larger
+ *                        draws).  Tied to torch's distribution kernels (ATen/native/cuda/DistributionTemplates.h). */
+#define LDM_NOISE_CONTRACT 0
+#define LDM_NOISE_TORCH 1
+typedef struct {
+  int32_t kind;
+  uint64_t seed;
+  uint64_t offset;
+  int64_t total_layouts;
+} LdmNoise;
+
 /* Build a handle: uploads and repacks the weights (per-head padded QKV, 16-bit operands, AdaLN table for all t,
  * schedule tables, TMA descriptors).  Replaces model construction + .to(device) for the sampling path. */
 int ldm_create(const LdmModelDesc* desc, const LdmWeights* weights, LdmHandle** out);
@@ -126,6 +145,14 @@ int ldm_step(LdmHandle* h, int32_t B, const int64_t* ids_in_dev, int32_t t_model
              const LdmCond* cond, const LdmSampling* sampling, uint64_t seed, uint32_t step_ctr, int64_t b_global0,
              int64_t* ids_out_dev, float* logits_out_dev, float* logprob_out_dev,
              const float* logits_in_dev, const float* logprob_in_dev, void* stream);
+/* ldm_step with the noise described by `noise` (step_ctr: the contract's counter; torch noise draws at noise->offset) */
+int ldm_step_noise(LdmHandle* h, int32_t B, const int64_t* ids_in_dev, int32_t t_model, int32_t t_post,
+                   const LdmCond* cond, const LdmSampling* sampling, const LdmNoise* noise, uint32_t step_ctr, int64_t b_global0,
+                   int64_t* ids_out_dev, float* logits_out_dev, float* logprob_out_dev,
+                   const float* logits_in_dev, const float* logprob_in_dev, void* stream);
+/* How far a call of n_steps steps on a batch of total_layouts layouts moves torch's generator offset (0 for deterministic,
+ * one draw per step, two for gumbel); < 0: LDM_ERR_*.  The one place that knows torch's launch policy. */
+int64_t ldm_noise_advance(const LdmHandle* h, int64_t total_layouts, const LdmSampling* sampling, int32_t n_steps);
 
 /* The whole loop == BaseMaskAndReplaceDiffusion.sample (base.py:293-371) for a precomputed timestep plan.
  *   t_model_host / t_post_host : n_steps entries each (host).
@@ -135,6 +162,10 @@ int ldm_step(LdmHandle* h, int32_t B, const int64_t* ids_in_dev, int32_t t_model
 int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model_host, const int32_t* t_post_host,
                     const LdmCond* cond, const LdmSampling* sampling, uint64_t seed, int64_t b_global0,
                     const int64_t* ids_init_dev, int64_t* ids_out_dev, int64_t* ids_trace_dev, void* stream);
+/* ldm_sample_loop with the noise described by `noise`; a replayed CUDA graph takes the new seed / offset */
+int ldm_sample_loop_noise(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model_host, const int32_t* t_post_host,
+                          const LdmCond* cond, const LdmSampling* sampling, const LdmNoise* noise, int64_t b_global0,
+                          const int64_t* ids_init_dev, int64_t* ids_out_dev, int64_t* ids_trace_dev, void* stream);
 
 /* Same loop with HOST buffers (what `LayoutDM.sample()` does around the core: H2D of cond, D2H of ids;
  * base.py:328-330,371): copies the inputs host->device, runs the loop, copies ids_out device->host and
@@ -217,6 +248,10 @@ int ldm_profile_end(LdmHandle* h, float* ms_per_category, int64_t* launches_per_
  * ("x32","y32","x16","z16","att16","qkv16","hid16","logits"; operand_dtype 2 also the lo planes "x16_lo","z16_lo","att16_lo",
  * "qkv16_lo","hid16_lo") of the first n_layouts layouts to host; returns bytes (< 0: unknown name). */
 int ldm_debug_set_stop_after(LdmHandle* h, int32_t n_launches);
+/* test tap of LDM_NOISE_TORCH: out_dev[numel] = the float32 values torch's CUDA generator (this seed / offset, the handle's
+ * device) gives exponential_ (which = 1) or rand (which = 0) of a contiguous tensor of numel < 2^31 elements, computed by
+ * the device code the draw kernels use */
+int ldm_debug_torch_noise(const LdmHandle* h, int64_t numel, uint64_t seed, uint64_t offset, int32_t which, float* out_dev, void* stream);
 int64_t ldm_debug_read(const LdmHandle* h, const char* name, void* dst_host, int64_t capacity_bytes, int32_t n_layouts);
 
 const char* ldm_last_error(void);

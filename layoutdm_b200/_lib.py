@@ -41,6 +41,14 @@ class LdmSampling(C.Structure):
     _fields_ = [("mode", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float), ("top_k", C.c_int32)]
 
 
+# LdmNoise.kind: the project's Philox contract, or the numbers torch's CUDA generator would give the reference's draw
+NOISE_KINDS = {"contract": 0, "torch": 1}
+
+
+class LdmNoise(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("seed", C.c_uint64), ("offset", C.c_uint64), ("total_layouts", C.c_int64)]
+
+
 # every symbol include/ldm_b200.h declares: (restype, argtypes)
 SIGNATURES = {
     "ldm_create": (C.c_int, [C.POINTER(LdmModelDesc), C.POINTER(LdmWeights), C.POINTER(C.c_void_p)]),
@@ -49,6 +57,13 @@ SIGNATURES = {
                            C.c_uint64, C.c_uint32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ldm_sample_loop": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(LdmCond),
                                   C.POINTER(LdmSampling), C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ldm_step_noise": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(LdmCond), C.POINTER(LdmSampling),
+                                 C.POINTER(LdmNoise), C.c_uint32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p]),
+    "ldm_sample_loop_noise": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(LdmCond),
+                                        C.POINTER(LdmSampling), C.POINTER(LdmNoise), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
+    "ldm_noise_advance": (C.c_int64, [C.c_void_p, C.c_int64, C.POINTER(LdmSampling), C.c_int32]),
     "ldm_sample_host": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(LdmSampling), C.c_uint64, C.c_int64, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -71,6 +86,7 @@ SIGNATURES = {
     "ldm_profile_begin": (C.c_int, [C.c_void_p]),
     "ldm_profile_end": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.c_int32]),
     "ldm_debug_set_stop_after": (C.c_int, [C.c_void_p, C.c_int32]),
+    "ldm_debug_torch_noise": (C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p]),
     "ldm_debug_read": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int32]),
     "ldm_last_error": (C.c_char_p, []),
     "ldm_version": (C.c_char_p, []),

@@ -305,6 +305,78 @@ struct TokenNoise {
     w[0] = word_of(a, 4 * lane); w[1] = word_of(a, 4 * lane + 1); w[2] = word_of(a, 4 * lane + 2); w[3] = word_of(a, 4 * lane + 3);
     w[4] = word_of(b, 128 + lane);
   }
+  // what draw_class needs of the contract: the lane's classes must be able to win by at least this much (in units of the
+  // temperature) for the classes outside a vocabulary group to be unreachable; see posterior_sample_group_kernel
+  static constexpr float kGroupMargin = 40.0f;
+};
+
+// The draw's view of TokenNoise: words(stream, w) fills the lane's N words of a stream; Gumbel noise (added to the lane's
+// log-probabilities) from stream 1, Exp(1) variates from stream 0.  Every slot is drawn whatever `on` says: the words come in Philox blocks of four classes.
+template <int N, class Words>
+struct ContractDraw {
+  Words words;
+  LDM_DEVINL void add_gumbel(const bool (&)[N], float (&lg)[N]) const {
+    uint32_t w[N];
+    words(1u, w);
+#pragma unroll
+    for (int j = 0; j < N; ++j) lg[j] += gumbel_of(u01_from_bits(w[j]));
+  }
+  LDM_DEVINL void exponential(const bool (&)[N], float (&e)[N]) const {
+    uint32_t w[N];
+    words(0u, w);
+#pragma unroll
+    for (int j = 0; j < N; ++j) e[j] = -logf(u01_from_bits(w[j]));
+  }
+};
+template <int N, class Words>
+LDM_DEVINL ContractDraw<N, Words> contract_draw(Words w) { return ContractDraw<N, Words>{w}; }
+
+// ------------------------------------------------------------------------------------------------------------
+// The second noise contract: the numbers torch's CUDA generator gives `exponential_` / `uniform_` on a contiguous tensor of
+// numel < 2^31 elements (ATen/native/cuda/DistributionTemplates.h, distribution_elementwise_grid_stride_kernel with
+// curand_uniform4; tthr = 256 * grid threads of calc_execution_policy).  Element i is word (i / tthr) & 3 of the
+// Philox4x32-10 block with counter offset / 4 + i / (4 tthr) in words 0-1 and subsequence i % tthr in words 2-3,
+// key = seed (curand_init(seed, i % tthr, offset)).
+// ------------------------------------------------------------------------------------------------------------
+struct TorchNoise {
+  uint2 key; unsigned long long ctr0; uint32_t tthr;
+  __host__ __device__ __forceinline__ TorchNoise(unsigned long long seed, unsigned long long offset, uint32_t tthr_) : ctr0(offset >> 2), tthr(tthr_) {
+    key = make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  }
+  LDM_DEVINL uint32_t word(uint32_t i) const {
+    const uint32_t q = i / tthr, sub = i - q * tthr;
+    const unsigned long long ctr = ctr0 + (q >> 2);
+    return TokenNoise::word_of(philox4x32_10(make_uint4(static_cast<uint32_t>(ctr), static_cast<uint32_t>(ctr >> 32), sub, 0u), key), q & 3);
+  }
+  // curand_uniform: w 2^-32 + 2^-33, in (0, 1]
+  static LDM_DEVINL float uniform(uint32_t w) { return __fmaf_rn(__uint2float_rn(w), 0x1p-32f, 0x1p-33f); }
+  // uniform_ on [0, 1) (uniform_kernel: 1 -> 0)
+  static LDM_DEVINL float rand(uint32_t w) { const float u = uniform(w); return u == 1.0f ? 0.0f : u; }
+  // exponential_(1) (ATen/core/TransformationHelper.h, transformation::exponential): -log(u), -log -> eps / 2 near 1; at::log
+  // of a float is the fast __logf on the device (ATen/NumericUtils.h)
+  static LDM_DEVINL float exponential(uint32_t w) { const float u = uniform(w); return u >= 1.0f - 0x1p-24f ? 0x1p-24f : -__logf(u); }
+  // a class outside a group has p ~ 1e-30 / temperature: it cannot win unless exp(margin) < e_max / e_min * Gumbel spread
+  // = (22.9 / 2^-24) * exp(16.7 + 4.3), exp(40.7); the margin of the contract would not do
+  static constexpr float kGroupMargin = 48.0f;
+};
+
+// The draw's view of TorchNoise for one token (b, s) of an (n_total, S, C) batch, b global: multinomial over the (B S, C)
+// probabilities draws exponential_ at `exp`'s offset into empty_like(probs), in memory order: element (b S + s) C + c of the
+// contiguous copy the rearrange makes for n_total > 1, element c S + s for n_total == 1, where the rearrange is a view with
+// strides (1, S) that empty_like keeps (i_exp + exp_cs * c).  name="gumbel" first draws element (b C + c) S + s of rand_like on
+// the contiguous (B, C, S) log-probabilities at `gum`'s offset.  One Philox block per class, and only for the slots with `on`
+// (classes that can win).
+template <int N>
+struct TorchDraw {
+  TorchNoise exp, gum; uint32_t i_exp, exp_cs, i_gum, S; const int (&cls)[N];
+  LDM_DEVINL void add_gumbel(const bool (&on)[N], float (&lg)[N]) const {
+#pragma unroll
+    for (int j = 0; j < N; ++j) if (on[j]) lg[j] += gumbel_of(TorchNoise::rand(gum.word(i_gum + static_cast<uint32_t>(cls[j]) * S)));
+  }
+  LDM_DEVINL void exponential(const bool (&on)[N], float (&e)[N]) const {
+#pragma unroll
+    for (int j = 0; j < N; ++j) e[j] = on[j] ? TorchNoise::exponential(exp.word(i_exp + exp_cs * static_cast<uint32_t>(cls[j]))) : 1.0f;
+  }
 };
 
 LDM_DEVINL float ex2_approx(float x) {

@@ -161,13 +161,14 @@ struct LdmHandle {
   int use_graph = 1;           // env LDM_GRAPH=0: plain stream launches
   int sweep = 1;               // env LDM_SWEEP=0: every kernel walks its row blocks in ascending order (no alternating directions)
   int num_sms = 0;             // the persistent GEMMs run at most one CTA per SM
+  int max_threads_sm = 0;      // with num_sms: the launch policy of torch's distribution kernels (LDM_NOISE_TORCH)
   int gemm_ctas = 0;           // env LDM_GEMM_CTAS=n (n >= 1): at most n CTAs in a persistent GEMM launch; 0: no cap
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
                                // The split mode always launches it: the draw kernels write one 16-bit plane only
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   uint64_t graph_key = 0;
-  unsigned long long* call_block = nullptr;   // device {seed, b_global0}
+  unsigned long long* call_block = nullptr;   // device {seed, b_global0, torch offset, tthr, delta, total_layouts} (StepParams::call)
   uint64_t ws_generation = 0;  // bumped when the workspace is reallocated (captured pointers die)
   int64_t graph_launches = 0;  // kernel launches inside the captured graph
   std::vector<void*> staging;  // ldm_create: fp32 uploads that only feed the packing kernels, released once those have run
@@ -487,6 +488,34 @@ int validate_common(LdmHandle* h, int B, const LdmSampling* s) {
   return LDM_OK;
 }
 
+// torch's launch policy for a draw of numel < 2^31 elements (calc_execution_policy, ATen/native/cuda/DistributionTemplates.h):
+// 256-thread blocks, at most as many as the device holds at once; tthr threads in all, each running curand_uniform4 until the
+// elements are covered, and the generator's offset advances by 4 per such call (delta)
+struct TorchPolicy { uint32_t tthr, delta; };
+TorchPolicy torch_policy(const LdmHandle* h, int64_t numel) {
+  const int64_t grid = std::min<int64_t>(static_cast<int64_t>(h->num_sms) * (h->max_threads_sm / 256), (numel + 255) / 256);
+  const int64_t tthr = 256 * grid;
+  return {static_cast<uint32_t>(tthr), static_cast<uint32_t>(((numel - 1) / (tthr * 4) + 1) * 4)};
+}
+int64_t torch_numel(const LdmHandle* h, int64_t total_layouts) { return total_layouts * h->S * h->C; }
+// total_layouts * S * C < 2^31, checked without forming the product
+bool torch_batch_fits(const LdmHandle* h, int64_t total_layouts) {
+  return total_layouts <= ((int64_t(1) << 31) - 1) / (static_cast<int64_t>(h->S) * h->C);
+}
+
+int validate_noise(const LdmHandle* h, int B, int64_t b_global0, const LdmNoise* nz) {
+  if (!nz) return fail(LDM_ERR_INVALID, "null noise description");
+  if (nz->kind != LDM_NOISE_CONTRACT && nz->kind != LDM_NOISE_TORCH) return fail(LDM_ERR_INVALID, "unknown noise kind %d", nz->kind);
+  if (nz->kind == LDM_NOISE_TORCH) {
+    if (b_global0 < 0 || nz->total_layouts < b_global0 + B)
+      return fail(LDM_ERR_INVALID, "total_layouts=%lld must cover layouts [%lld, %lld)", (long long)nz->total_layouts, (long long)b_global0, (long long)(b_global0 + B));
+    if (!torch_batch_fits(h, nz->total_layouts))
+      return fail(LDM_ERR_UNSUPPORTED, "torch-generator noise needs total_layouts * S * C < 2^31 (torch splits larger draws)");
+    if (nz->offset % 4) return fail(LDM_ERR_INVALID, "a torch generator offset is a multiple of 4 (got %llu)", (unsigned long long)nz->offset);
+  }
+  return LDM_OK;
+}
+
 StepParams base_step_params(const LdmHandle* h, int B) {
   StepParams p{};
   p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr;
@@ -502,8 +531,9 @@ StepParams base_step_params(const LdmHandle* h, int B) {
   return p;
 }
 
+// noise: its kind selects the draw kernels' contract; step t_step of a call draws at the torch offset advanced by t_step steps
 int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_post, const LdmCond* cond, const LdmSampling* samp,
-              uint64_t seed, uint32_t step_ctr, int64_t b_global0, long long* ids_out, float* logits_out, float* logprob_out,
+              const LdmNoise& noise, uint32_t step_ctr, int t_step, int64_t b_global0, long long* ids_out, float* logits_out, float* logprob_out,
               const float* logits_in, const float* logprob_in, cudaStream_t st, const unsigned long long* call = nullptr,
               bool skip_embed = false, int t_next = -1) {
   if (t_model < 0 || t_model >= h->T || t_post < 0 || t_post >= h->T)
@@ -532,7 +562,14 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
                    ((cond->seq_orig && cond->refine_table) ? COND_REFINE : 0);
   }
   p.mode = samp->mode; p.temperature = samp->temperature; p.top_p = samp->top_p; p.top_k = samp->top_k;
-  p.seed = seed; p.step_ctr = step_ctr; p.b_global0 = b_global0; p.call = call;
+  p.seed = noise.seed; p.step_ctr = step_ctr; p.b_global0 = b_global0; p.call = call;
+  const bool torch_noise = noise.kind == LDM_NOISE_TORCH;
+  if (torch_noise) {
+    const TorchPolicy tp = torch_policy(h, torch_numel(h, noise.total_layouts));
+    p.t_offset = noise.offset; p.t_tthr = tp.tthr; p.t_delta = tp.delta; p.t_step = t_step; p.t_total = noise.total_layouts;
+  }
+  const auto generic = torch_noise ? posterior_sample_kernel<TorchNoise> : posterior_sample_kernel<TokenNoise>;
+  const auto group = torch_noise ? posterior_sample_group_kernel<TorchNoise> : posterior_sample_group_kernel<TokenNoise>;
   p.ids_out = ids_out; p.logprob_out = logprob_out;
   if (t_next >= 0) {     // the loop: this draw also writes the next step's embedding + AdaLN_0(t_next) rows
     p.emb_cat = h->cat_emb; p.emb_pos = h->pos; p.emb_adaln = h->adaln + static_cast<size_t>(t_next) * 2 * h->desc.d_model;
@@ -551,7 +588,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
     p1.cond_flags &= ~COND_PAD_DISABLE; p1.logprob_out = h->rel_lp; p1.emb_adaln = nullptr;    // its draw is discarded: no embedding
     {
       ProfScope ps(h, CAT_EPILOGUE, st);
-      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p1));
+      CK(launch_step(h, generic, blocks, 256, 0, st, p1));
     }
     RelationParams r{};
     r.n_layouts = B; r.S = h->S; r.C = h->C; r.n_attr = h->desc.n_attr; r.n_elem = h->desc.n_elem; r.n_cat = h->desc.n_cat;
@@ -568,15 +605,15 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
     p2.logprob_out = logprob_out;            // tap: the adjusted log-probs after PAD-disable (what sample() sees, base.py:287)
     {
       ProfScope ps(h, CAT_EPILOGUE, st);
-      CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p2));
+      CK(launch_step(h, generic, blocks, 256, 0, st, p2));
     }
     CK(cudaGetLastError());
     return LDM_OK;
   }
   {
     ProfScope ps(h, CAT_EPILOGUE, st);
-    if (group_kernel_applies(p)) CK(launch_step(h, posterior_sample_group_kernel, blocks, 256, 0, st, p));
-    else CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p));
+    if (group_kernel_applies(p)) CK(launch_step(h, group, blocks, 256, 0, st, p));
+    else CK(launch_step(h, generic, blocks, 256, 0, st, p));
   }
   CK(cudaGetLastError());
   return LDM_OK;
@@ -619,6 +656,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (h->split) h->fuse_embed = 0;
   if (const char* e = getenv("LDM_SWEEP")) h->sweep = atoi(e);
   h->num_sms = prop.multiProcessorCount;
+  h->max_threads_sm = prop.maxThreadsPerMultiProcessor;
   if (const char* e = getenv("LDM_GEMM_CTAS")) h->gemm_ctas = std::max(1, atoi(e));
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
@@ -695,7 +733,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     }
     TRY(dev_upload(h, &h->sched, sch.data(), sch.size()));
     TRY(dev_alloc(h, &h->lae, static_cast<size_t>(h->G) * (T + 1) * 4));
-    TRY(dev_alloc(h, &h->call_block, static_cast<size_t>(2)));
+    TRY(dev_alloc(h, &h->call_block, static_cast<size_t>(6)));
     lae_table_kernel<<<(h->G * (T + 1) + 127) / 128, 128>>>(h->sched, h->lae, h->G, T + 1);
     if (cudaGetLastError() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "lae_table_kernel launch failed"); }
   }
@@ -722,22 +760,50 @@ int ldm_destroy(LdmHandle* h) {
   return LDM_OK;
 }
 
+int ldm_step_noise(LdmHandle* h, int32_t B, const int64_t* ids_in, int32_t t_model, int32_t t_post, const LdmCond* cond,
+                   const LdmSampling* sampling, const LdmNoise* noise, uint32_t step_ctr, int64_t b_global0, int64_t* ids_out,
+                   float* logits_out, float* logprob_out, const float* logits_in, const float* logprob_in, void* stream) {
+  int rc = validate_common(h, B, sampling);
+  if (rc) return rc;
+  if ((rc = validate_noise(h, B, b_global0, noise))) return rc;
+  if (!ids_in || !ids_out) return fail(LDM_ERR_INVALID, "ids_in / ids_out must not be null");
+  CK(cudaSetDevice(h->desc.device));
+  return step_impl(h, B, reinterpret_cast<const long long*>(ids_in), t_model, t_post, cond, sampling, *noise, step_ctr, 0, b_global0,
+                   reinterpret_cast<long long*>(ids_out), logits_out, logprob_out, logits_in, logprob_in, static_cast<cudaStream_t>(stream));
+}
+
 int ldm_step(LdmHandle* h, int32_t B, const int64_t* ids_in, int32_t t_model, int32_t t_post, const LdmCond* cond,
              const LdmSampling* sampling, uint64_t seed, uint32_t step_ctr, int64_t b_global0, int64_t* ids_out,
              float* logits_out, float* logprob_out, const float* logits_in, const float* logprob_in, void* stream) {
-  int rc = validate_common(h, B, sampling);
-  if (rc) return rc;
-  if (!ids_in || !ids_out) return fail(LDM_ERR_INVALID, "ids_in / ids_out must not be null");
+  const LdmNoise noise{LDM_NOISE_CONTRACT, seed, 0, 0};
+  return ldm_step_noise(h, B, ids_in, t_model, t_post, cond, sampling, &noise, step_ctr, b_global0, ids_out, logits_out, logprob_out,
+                        logits_in, logprob_in, stream);
+}
+
+int64_t ldm_noise_advance(const LdmHandle* h, int64_t total_layouts, const LdmSampling* sampling, int32_t n_steps) {
+  if (!h || !sampling || total_layouts <= 0 || n_steps < 0) return fail(LDM_ERR_INVALID, "bad ldm_noise_advance arguments");
+  if (!torch_batch_fits(h, total_layouts))
+    return fail(LDM_ERR_UNSUPPORTED, "torch-generator noise needs total_layouts * S * C < 2^31 (torch splits larger draws)");
+  if (sampling->mode == LDM_SAMPLING_DETERMINISTIC) return 0;
+  const int64_t per_step = static_cast<int64_t>(torch_policy(h, torch_numel(h, total_layouts)).delta) * (sampling->mode == LDM_SAMPLING_GUMBEL ? 2 : 1);
+  return per_step * n_steps;
+}
+
+int ldm_debug_torch_noise(const LdmHandle* h, int64_t numel, uint64_t seed, uint64_t offset, int32_t which, float* out, void* stream) {
+  if (!h || !out || numel <= 0 || numel >= (int64_t(1) << 31) || offset % 4 || (which != 0 && which != 1))
+    return fail(LDM_ERR_INVALID, "bad ldm_debug_torch_noise arguments");
   CK(cudaSetDevice(h->desc.device));
-  return step_impl(h, B, reinterpret_cast<const long long*>(ids_in), t_model, t_post, cond, sampling, seed, step_ctr, b_global0,
-                   reinterpret_cast<long long*>(ids_out), logits_out, logprob_out, logits_in, logprob_in, static_cast<cudaStream_t>(stream));
+  const TorchPolicy tp = torch_policy(h, numel);
+  torch_noise_tap_kernel<<<1024, 256, 0, static_cast<cudaStream_t>(stream)>>>(TorchNoise(seed, offset, tp.tthr), static_cast<uint32_t>(numel), which, out);
+  CK(cudaGetLastError());
+  return LDM_OK;
 }
 
 namespace {
 
 // the plain loop: fill / pick the start state, then n_steps x step_impl on stream st
 int run_loop(LdmHandle* h, int B, int n_steps, const int32_t* t_model, const int32_t* t_post, const LdmCond* cond, const LdmSampling* sampling,
-             uint64_t seed, int64_t b_global0, const long long* ids_init, long long* ids_out, long long* ids_trace, cudaStream_t st,
+             const LdmNoise& noise, int64_t b_global0, const long long* ids_init, long long* ids_out, long long* ids_trace, cudaStream_t st,
              const unsigned long long* call) {
   const size_t nid = static_cast<size_t>(B) * h->S;
   const long long* cur = nullptr;
@@ -754,7 +820,7 @@ int run_loop(LdmHandle* h, int B, int n_steps, const int32_t* t_model, const int
     else if (i == n_steps - 1) dst = ids_out;
     else dst = (cur == h->ids[0]) ? h->ids[1] : h->ids[0];
     const bool fuse = h->fuse_embed != 0;
-    int rc = step_impl(h, B, cur, t_model[i], t_post[i], cond, sampling, seed, static_cast<uint32_t>(i), b_global0, dst, nullptr, nullptr, nullptr, nullptr, st, call,
+    int rc = step_impl(h, B, cur, t_model[i], t_post[i], cond, sampling, noise, static_cast<uint32_t>(i), i, b_global0, dst, nullptr, nullptr, nullptr, nullptr, st, call,
                        fuse && i > 0, (fuse && i + 1 < n_steps) ? t_model[i + 1] : -1);
     if (rc) return rc;
     cur = dst;
@@ -771,11 +837,12 @@ uint64_t fnv1a(uint64_t hsh, const void* data, size_t n) {
 
 }  // namespace
 
-int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model, const int32_t* t_post, const LdmCond* cond,
-                    const LdmSampling* sampling, uint64_t seed, int64_t b_global0, const int64_t* ids_init, int64_t* ids_out,
-                    int64_t* ids_trace, void* stream) {
+int ldm_sample_loop_noise(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model, const int32_t* t_post, const LdmCond* cond,
+                          const LdmSampling* sampling, const LdmNoise* noise, int64_t b_global0, const int64_t* ids_init, int64_t* ids_out,
+                          int64_t* ids_trace, void* stream) {
   int rc = validate_common(h, B, sampling);
   if (rc) return rc;
+  if ((rc = validate_noise(h, B, b_global0, noise))) return rc;
   if (n_steps < 1 || !t_model || !t_post || !ids_out) return fail(LDM_ERR_INVALID, "bad loop arguments");
   for (int i = 0; i < n_steps; ++i) {
     if (t_model[i] < 0 || t_model[i] >= h->T || t_post[i] < 0 || t_post[i] >= h->T)
@@ -789,7 +856,7 @@ int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
   const size_t nid = static_cast<size_t>(B) * h->S;
   const bool has_cond = cond && cond->seq;
   if (!h->use_graph || h->prof || ids_trace || h->debug_stop_after || (has_cond && cond->rel_adj))
-    return run_loop(h, B, n_steps, t_model, t_post, has_cond ? cond : nullptr, sampling, seed, b_global0, reinterpret_cast<const long long*>(ids_init),
+    return run_loop(h, B, n_steps, t_model, t_post, has_cond ? cond : nullptr, sampling, *noise, b_global0, reinterpret_cast<const long long*>(ids_init),
                     reinterpret_cast<long long*>(ids_out), reinterpret_cast<long long*>(ids_trace), st, nullptr);
 
   // ---- CUDA-graph replay: the static T-step plan (n_steps x 23 launches with programmatic edges) is captured once; what changes
@@ -812,11 +879,15 @@ int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
     gc.pad_disable = cond->pad_disable;
   }
   if (ids_init && reinterpret_cast<const long long*>(ids_init) != h->ids[1]) CK(cudaMemcpyAsync(h->ids[1], ids_init, nid * 8, cudaMemcpyDeviceToDevice, st));
-  const unsigned long long blk[2] = {seed, static_cast<unsigned long long>(b_global0)};
+  // the noise words the captured kernels read (StepParams::call); the contract reads the first two
+  const TorchPolicy tp = noise->kind == LDM_NOISE_TORCH ? torch_policy(h, torch_numel(h, noise->total_layouts)) : TorchPolicy{0, 0};
+  const unsigned long long blk[6] = {noise->seed, static_cast<unsigned long long>(b_global0), noise->offset, tp.tthr, tp.delta,
+                                     static_cast<unsigned long long>(noise->total_layouts)};
   CK(cudaMemcpyAsync(h->call_block, blk, sizeof(blk), cudaMemcpyHostToDevice, st));   // pageable source: staged by the driver before the call returns
 
   uint64_t key = 1469598103934665603ull;
-  const int32_t head[6] = {B, n_steps, has_cond ? 1 + (gc.mask ? 2 : 0) + (gc.seq_orig ? 4 : 0) + (gc.pad_disable ? 8 : 0) : 0, ids_init ? 1 : 0, h->pdl, h->fuse_embed};
+  const int32_t head[7] = {B, n_steps, has_cond ? 1 + (gc.mask ? 2 : 0) + (gc.seq_orig ? 4 : 0) + (gc.pad_disable ? 8 : 0) : 0, ids_init ? 1 : 0, h->pdl, h->fuse_embed,
+                           noise->kind};
   key = fnv1a(key, head, sizeof(head));
   key = fnv1a(key, t_model, sizeof(int32_t) * n_steps);
   key = fnv1a(key, t_post, sizeof(int32_t) * n_steps);
@@ -831,7 +902,8 @@ int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
     bool ok = cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     cudaGraph_t g = nullptr;
     if (ok) {
-      rc = run_loop(h, B, n_steps, t_model, t_post, has_cond ? &gc : nullptr, sampling, 0, 0, ids_init ? h->ids[1] : nullptr, h->ids_final, nullptr,
+      const LdmNoise staged{noise->kind, 0, 0, noise->total_layouts};     // every noise word the kernels read comes from call_block
+      rc = run_loop(h, B, n_steps, t_model, t_post, has_cond ? &gc : nullptr, sampling, staged, 0, ids_init ? h->ids[1] : nullptr, h->ids_final, nullptr,
                     h->cap_stream, h->call_block);
       ok = cudaStreamEndCapture(h->cap_stream, &g) == cudaSuccess && g != nullptr && rc == LDM_OK;
       h->graph_launches = h->launches - l0;
@@ -842,7 +914,7 @@ int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
     if (!ok) {
       cudaGetLastError();
       h->graph_exec = nullptr; h->use_graph = 0;
-      return run_loop(h, B, n_steps, t_model, t_post, has_cond ? &gc : nullptr, sampling, seed, b_global0, ids_init ? h->ids[1] : nullptr,
+      return run_loop(h, B, n_steps, t_model, t_post, has_cond ? &gc : nullptr, sampling, *noise, b_global0, ids_init ? h->ids[1] : nullptr,
                       reinterpret_cast<long long*>(ids_out), nullptr, st, nullptr);
     }
     h->graph_key = key;
@@ -851,6 +923,13 @@ int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_m
   h->launches += h->graph_launches;
   if (reinterpret_cast<long long*>(ids_out) != h->ids_final) CK(cudaMemcpyAsync(ids_out, h->ids_final, nid * 8, cudaMemcpyDeviceToDevice, st));
   return LDM_OK;
+}
+
+int ldm_sample_loop(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model, const int32_t* t_post, const LdmCond* cond,
+                    const LdmSampling* sampling, uint64_t seed, int64_t b_global0, const int64_t* ids_init, int64_t* ids_out,
+                    int64_t* ids_trace, void* stream) {
+  const LdmNoise noise{LDM_NOISE_CONTRACT, seed, 0, 0};
+  return ldm_sample_loop_noise(h, B, n_steps, t_model, t_post, cond, sampling, &noise, b_global0, ids_init, ids_out, ids_trace, stream);
 }
 
 int ldm_sample_host(LdmHandle* h, int32_t B, int32_t n_steps, const int32_t* t_model, const int32_t* t_post,
@@ -970,7 +1049,7 @@ int ldm_predict_start(LdmHandle* h, int32_t B, const int64_t* xt_ids, const int3
   StepParams p = base_step_params(h, B);
   p.ids_in = reinterpret_cast<const long long*>(xt_ids); p.t_layout = t_dev; p.lx0_out = log_x0_out;   // ids_out == nullptr: no draw
   const int blocks = (B * h->S * 32 + 255) / 256;
-  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p)); }
+  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel<>, blocks, 256, 0, st, p)); }
   CK(cudaGetLastError());
   return LDM_OK;
 }
@@ -982,7 +1061,7 @@ int ldm_q_posterior(LdmHandle* h, int32_t B, const float* log_x_start, const int
   StepParams p = base_step_params(h, B);
   p.ids_in = reinterpret_cast<const long long*>(xt_ids); p.t_layout = t_dev; p.lx0_in = log_x_start; p.logprob_out = out;
   const int blocks = (B * h->S * 32 + 255) / 256;
-  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel, blocks, 256, 0, st, p)); }
+  { ProfScope ps(h, CAT_EPILOGUE, st); CK(launch_step(h, posterior_sample_kernel<>, blocks, 256, 0, st, p)); }
   CK(cudaGetLastError());
   return LDM_OK;
 }

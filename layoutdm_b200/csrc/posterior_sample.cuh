@@ -8,7 +8,11 @@
 //   sample()                      T/helpers/sampling.py:81-130 ; torch.multinomial(p,1) == argmax(p / Exp(1))
 // Class ownership inside a warp (lane_classes): lane l holds classes 4l..4l+3 (one float4 of logits, one Philox block) and
 // class 128+l; TokenNoise::lane_words draws the noise words of exactly these classes.
+// The draw kernels take the noise contract as a template parameter: TokenNoise (the default, DESIGN.md §7) or TorchNoise
+// (the numbers torch's CUDA generator would give the reference's draw).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "embed.cuh"
 
@@ -36,14 +40,17 @@ struct StepParams {
   int cond_flags;
   int mode; float temperature; float top_p; int top_k;
   unsigned long long seed; unsigned int step_ctr; long long b_global0;
-  const unsigned long long* call;        // nullptr, or device words {seed, b_global0} that override the two fields above: a captured
-                                         // CUDA graph of the loop stays valid while the noise key changes from call to call
+  const unsigned long long* call;        // nullptr, or device words {seed, b_global0, t_offset, t_tthr, t_delta, t_total} that override those
+                                         // fields: a captured CUDA graph of the loop stays valid while the noise changes from call to call
   long long* ids_out;                    // [n_layouts][S]
   float* logprob_out;                    // [n_layouts][S][C] or nullptr
   // the front of the NEXT denoising step, fused behind the draw (the loop API only): the warp that drew a token also writes that
   // token's embedding + AdaLN_0(t_next) row, which saves the embed launch and overlaps its write stream with this issue-bound kernel
   const float* emb_cat; const float* emb_pos; const float* emb_adaln;   // cat_emb [C][d], pos [S][d], AdaLN row [2d] of (layer 0, t_next); emb_adaln == nullptr: off
   float* emb_x32; void* emb_x16; int emb_d, emb_bf16;
+  // TorchNoise: the generator offset of the call's first step, the threads of torch's launch and the offset one draw advances;
+  // step t_step of the call draws at t_offset + t_step * (1 or 2 draws) * t_delta; t_total: the layouts of the whole batch
+  unsigned long long t_offset; unsigned int t_tthr, t_delta; int t_step; long long t_total;
 };
 
 LDM_DEVINL float log_add_exp(float a, float b) {   // util.py:19-21
@@ -108,6 +115,21 @@ LDM_DEVINL int warp_argmax_first(const float (&v)[N], const int (&cls)[N], const
 LDM_DEVINL TokenNoise step_noise(const StepParams& p, const int b, const int s) {
   const unsigned long long seed = p.call ? __ldg(p.call) : p.seed, bg0 = p.call ? __ldg(p.call + 1) : static_cast<unsigned long long>(p.b_global0);
   return TokenNoise(seed, bg0, b, p.S, s);
+}
+
+// the torch-generator noise of token (b, s) of this call's step p.t_step, slot j holding class cls[j] (the same override)
+template <int N>
+LDM_DEVINL TorchDraw<N> torch_draw(const StepParams& p, const int b, const int s, const int (&cls)[N]) {
+  const unsigned long long* w = p.call;
+  const unsigned long long seed = w ? __ldg(w) : p.seed, bg0 = w ? __ldg(w + 1) : static_cast<unsigned long long>(p.b_global0);
+  const unsigned long long off0 = w ? __ldg(w + 2) : p.t_offset;
+  const uint32_t tthr = w ? static_cast<uint32_t>(__ldg(w + 3)) : p.t_tthr, delta = w ? static_cast<uint32_t>(__ldg(w + 4)) : p.t_delta;
+  const bool single = (w ? static_cast<long long>(__ldg(w + 5)) : p.t_total) == 1;   // see TorchDraw
+  const bool gum = p.mode == SAMP_GUMBEL;       // rand_like at the step's offset, then multinomial one draw later
+  const unsigned long long off = off0 + static_cast<unsigned long long>(p.t_step) * (gum ? 2u : 1u) * delta;
+  const uint32_t bg = static_cast<uint32_t>(bg0 + b), S = static_cast<uint32_t>(p.S), C = static_cast<uint32_t>(p.C);
+  return TorchDraw<N>{TorchNoise(seed, off + (gum ? delta : 0u), tthr), TorchNoise(seed, off, tthr), single ? static_cast<uint32_t>(s) : (bg * S + s) * C,
+                      single ? S : 1u, bg * C * S + s, S, cls};
 }
 
 // predict_start (base.py:127-146): the float64 log-sum-exp over the C-1 non-MASK logits of one token's row (lane classes);
@@ -203,16 +225,12 @@ LDM_DEVINL void posterior_token_logprob(const StepParams& p, const int s, const 
 }
 
 // The draw from lg = log-probs / temperature (top-k / top-p already applied), the same for any slot layout: Gumbel noise for
-// name="gumbel" (stream 1), then probs = softmax(lg) and multinomial(probs, 1) = argmax(probs / e), e ~ Exp(1) (stream 0).
-// words(stream, w) returns the noise words of the lane's N slots.
-template <int N, class Words>
-LDM_DEVINL int draw_class(const StepParams& p, float (&lg)[N], const int (&cls)[N], const bool (&on)[N], Words words) {
-  uint32_t w[N];
-  if (p.mode == SAMP_GUMBEL) {
-    words(1u, w);
-#pragma unroll
-    for (int j = 0; j < N; ++j) lg[j] += gumbel_of(u01_from_bits(w[j]));
-  }
+// name="gumbel", then probs = softmax(lg) and multinomial(probs, 1) = argmax(probs / e), e ~ Exp(1).  The noise contract's
+// draw view (ContractDraw, TorchDraw) maps the lane's N slots to their Gumbel noise and Exp(1) variates; a slot with zero
+// probability scores 0 whatever its e, so it needs none.
+template <int N, class Draw>
+LDM_DEVINL int draw_class(const StepParams& p, float (&lg)[N], const int (&cls)[N], const bool (&on)[N], const Draw& nz) {
+  if (p.mode == SAMP_GUMBEL) nz.add_gumbel(on, lg);
   float m = -INFINITY;
 #pragma unroll
   for (int j = 0; j < N; ++j) m = fmaxf(m, lg[j]);
@@ -221,17 +239,19 @@ LDM_DEVINL int draw_class(const StepParams& p, float (&lg)[N], const int (&cls)[
 #pragma unroll
   for (int j = 0; j < N; ++j) { ex[j] = on[j] ? expf(lg[j] - m) : 0.0f; sm += ex[j]; }
   sm = warp_sum(sm);
-  words(0u, w);
+  bool live[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) live[j] = on[j] && ex[j] > 0.0f;
+  float e[N];
+  nz.exponential(live, e);
   float score[N];
 #pragma unroll
-  for (int j = 0; j < N; ++j) {
-    const float e = -logf(u01_from_bits(w[j]));
-    score[j] = on[j] ? (ex[j] / sm) / e : -INFINITY;
-  }
+  for (int j = 0; j < N; ++j) score[j] = on[j] ? (ex[j] / sm) / e[j] : -INFINITY;
   return warp_argmax_first<N>(score, cls, on);
 }
 
 // One token, every class (lane classes): any q_type, any sampling mode, log-prob in / out.
+template <class Noise>
 LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, const int lane) {
   const int b = token / p.S, s = token % p.S;
   const int C = p.C;
@@ -347,18 +367,23 @@ LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, co
         for (int j = 0; j < 5; ++j) if (valid[j] && lg[j] < thr) lg[j] = -INFINITY;
       }
     }
-    const TokenNoise nz = step_noise(p, b, s);
-    best_c = draw_class<5>(p, lg, cls, valid, [&](uint32_t stream, uint32_t (&w)[5]) { nz.lane_words(lane, noise_ctr(p.step_ctr, stream), w); });
+    if constexpr (std::is_same_v<Noise, TokenNoise>) {
+      const TokenNoise nz = step_noise(p, b, s);
+      best_c = draw_class<5>(p, lg, cls, valid, contract_draw<5>([&](uint32_t stream, uint32_t (&w)[5]) { nz.lane_words(lane, noise_ctr(p.step_ctr, stream), w); }));
+    } else {
+      best_c = draw_class<5>(p, lg, cls, valid, torch_draw<5>(p, b, s, cls));
+    }
   }
   if (lane == 0) p.ids_out[token] = best_c;
   embed_next(p, b, s, best_c, lane);
 }
 
+template <class Noise = TokenNoise>
 __global__ void __launch_bounds__(256) posterior_sample_kernel(const StepParams p) {
   const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (token >= p.n_layouts * p.S) return;
   pdl_sync();
-  posterior_token_generic(p, token, lane);
+  posterior_token_generic<Noise>(p, token, lane);
 }
 
 // Group-centric variant for the constrained (per-attribute) diffusion: outside the token's vocabulary group (plus PAD and
@@ -368,6 +393,7 @@ __global__ void __launch_bounds__(256) posterior_sample_kernel(const StepParams 
 // input / output, every group <= 32 classes.  A token whose best in-group log-probability is not far enough above
 // log(1e-30) for the out-of-group classes to be unreachable takes posterior_token_generic instead (warp-uniform), so
 // the result is the generic kernel's in every case.
+template <class Noise = TokenNoise>
 __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepParams p) {
   const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (token >= p.n_layouts * p.S) return;
@@ -420,11 +446,11 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
     float tmax = 0.0f;
 #pragma unroll
     for (int j = 0; j < 5; ++j) if (lvalid[j] && !in_group(p, g, lcls[j])) tmax = fmaxf(tmax, __ldg(trow + lcls[j]));
-    if (warp_max(tmax) > 0.0f) { posterior_token_generic(p, token, lane); return; }
+    if (warp_max(tmax) > 0.0f) { posterior_token_generic<Noise>(p, token, lane); return; }
   }
   // every class outside the group sits at log(1e-30): it must be out of reach of the draw (see the header comment)
-  const float margin = p.mode == SAMP_DETERMINISTIC ? 0.0f : 40.0f * p.temperature;
-  if (!(lmax - kLogEps > margin)) { posterior_token_generic(p, token, lane); return; }
+  const float margin = p.mode == SAMP_DETERMINISTIC ? 0.0f : Noise::kGroupMargin * p.temperature;
+  if (!(lmax - kLogEps > margin)) { posterior_token_generic<Noise>(p, token, lane); return; }
 
   int best_c;
   if (p.mode == SAMP_DETERMINISTIC) {
@@ -462,25 +488,36 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
 #pragma unroll
       for (int j = 0; j < 2; ++j) if (on[j] && n_before[j] > 0 && static_cast<float>(cum[j]) > p.top_p) lg[j] = -INFINITY;
     }
-    // One Philox evaluation per noise stream serves the whole token: lanes 0..8 compute the (at most 9) blocks of the group,
-    // lanes 9 / 10 the blocks of PAD / MASK, then every lane fetches its words.
-    const TokenNoise nz = step_noise(p, b, s);
-    const int b0 = TokenNoise::block_of(gst);
-    const int my_block = lane < 9 ? b0 + lane : TokenNoise::block_of(lane == 9 ? p.pad_id : p.mask_id);
-    const int src0 = TokenNoise::block_of(cls[0]) - b0, src1 = lane == 0 ? 9 : 10;
-    best_c = draw_class<2>(p, lg, cls, on, [&](uint32_t stream, uint32_t (&w)[2]) {
-      const uint4 r = nz.block(my_block, noise_ctr(p.step_ctr, stream));
+    if constexpr (std::is_same_v<Noise, TokenNoise>) {
+      // One Philox evaluation per noise stream serves the whole token: lanes 0..8 compute the (at most 9) blocks of the group,
+      // lanes 9 / 10 the blocks of PAD / MASK, then every lane fetches its words.
+      const TokenNoise nz = step_noise(p, b, s);
+      const int b0 = TokenNoise::block_of(gst);
+      const int my_block = lane < 9 ? b0 + lane : TokenNoise::block_of(lane == 9 ? p.pad_id : p.mask_id);
+      const int src0 = TokenNoise::block_of(cls[0]) - b0, src1 = lane == 0 ? 9 : 10;
+      best_c = draw_class<2>(p, lg, cls, on, contract_draw<2>([&](uint32_t stream, uint32_t (&w)[2]) {
+        const uint4 r = nz.block(my_block, noise_ctr(p.step_ctr, stream));
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int src = j == 0 ? src0 : src1;
-        const uint4 rs = make_uint4(__shfl_sync(0xffffffffu, r.x, src), __shfl_sync(0xffffffffu, r.y, src),
-                                    __shfl_sync(0xffffffffu, r.z, src), __shfl_sync(0xffffffffu, r.w, src));
-        w[j] = TokenNoise::word_of(rs, cls[j]);
-      }
-    });
+        for (int j = 0; j < 2; ++j) {
+          const int src = j == 0 ? src0 : src1;
+          const uint4 rs = make_uint4(__shfl_sync(0xffffffffu, r.x, src), __shfl_sync(0xffffffffu, r.y, src),
+                                      __shfl_sync(0xffffffffu, r.z, src), __shfl_sync(0xffffffffu, r.w, src));
+          w[j] = TokenNoise::word_of(rs, cls[j]);
+        }
+      }));
+    } else {
+      best_c = draw_class<2>(p, lg, cls, on, torch_draw<2>(p, b, s, cls));   // the group's classes only
+    }
   }
   if (lane == 0) p.ids_out[token] = best_c;
   embed_next(p, b, s, best_c, lane);
+}
+
+// test tap of the torch-generator contract: out[i] = element i of one exponential_ (which = 1) or rand (which = 0) draw of
+// `n` elements, through the TorchNoise the draw kernels use
+__global__ void torch_noise_tap_kernel(const TorchNoise nz, const uint32_t n, const int which, float* __restrict__ out) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    out[i] = which ? TorchNoise::exponential(nz.word(i)) : TorchNoise::rand(nz.word(i));
 }
 
 // the preconditions of posterior_sample_group_kernel (its header comment)

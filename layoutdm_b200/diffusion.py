@@ -17,6 +17,7 @@ from typing import Any, Dict, List, Optional, Union
 import torch
 import torch.nn.functional as F
 
+from . import _lib
 from .engine import Engine, sampling_struct
 from .vocab import Vocab, decode_ids, group_full_ids, linear_centers, refinement_table, relation_edge_table, timestep_plan
 
@@ -48,7 +49,14 @@ def duplicate_cond(cond: Dict, batch_size: int) -> Dict:
 
 
 class FusedMaskAndReplaceDiffusion:
-    def __init__(self, engine: Engine, tokenizer=None, bbox_centers=None):
+    """noise="contract": the draws use the project's Philox contract keyed by a seed (drawn from torch's generator unless
+    given).  noise="torch": they are the numbers torch's CUDA generator gives the reference's `sample` on the same GPU, and
+    every call advances that generator as the reference's would, so a seeded run reproduces the reference's samples."""
+
+    def __init__(self, engine: Engine, tokenizer=None, bbox_centers=None, noise: str = "contract"):
+        if noise not in _lib.NOISE_KINDS:
+            raise ValueError(f"noise must be one of {', '.join(_lib.NOISE_KINDS)}, got {noise!r}")
+        self.noise = noise
         self.engine = engine
         self.vocab: Vocab = engine.vocab
         self.num_classes = self.vocab.C
@@ -95,6 +103,20 @@ class FusedMaskAndReplaceDiffusion:
                 cond[k] = cond[k].to(self.device)                              # base.py:328-330
         return cond
 
+    def _with_torch_noise(self, total_layouts: int, sampling_cfg, n_steps: int, seed: Optional[int], call):
+        """call(noise) with the noise of n_steps steps from torch's CUDA generator of this device (its seed and current offset);
+        once the call has succeeded the generator is advanced past its draws, where the reference would leave it"""
+        if seed is not None:
+            raise ValueError("seed= selects the Philox contract; with noise='torch' the draws come from torch's CUDA generator")
+        if torch.cuda.is_current_stream_capturing():
+            raise ValueError("noise='torch' reads and advances torch's CUDA generator, which cannot be done during a CUDA graph capture")
+        gen = torch.cuda.default_generators[self.device.index]
+        offset = gen.get_offset()
+        advance = self.engine.noise_advance(total_layouts, sampling_cfg, n_steps)
+        out = call(_lib.LdmNoise(_lib.NOISE_KINDS["torch"], gen.initial_seed(), offset, total_layouts))
+        gen.set_offset(offset + advance)
+        return out
+
     @staticmethod
     def _new_seed() -> int:
         # the reference draws from torch's global generator, so `set_seed` / torch.manual_seed keeps controlling
@@ -103,39 +125,53 @@ class FusedMaskAndReplaceDiffusion:
 
     # ---- reference API -------------------------------------------------------------------------------
     def sample(self, batch_size: Optional[int] = 1, cond: Optional[Dict] = None, sampling_cfg=None,
-               get_intermediate_results: bool = False, seed: Optional[int] = None, b_global0: int = 0, **kwargs
-               ) -> Union[torch.LongTensor, List[torch.LongTensor]]:
-        """base.py:293-371"""
+               get_intermediate_results: bool = False, seed: Optional[int] = None, b_global0: int = 0,
+               total_layouts: Optional[int] = None, **kwargs) -> Union[torch.LongTensor, List[torch.LongTensor]]:
+        """base.py:293-371.  total_layouts: the whole batch when this call samples layouts [b_global0, b_global0 + batch_size)
+        of it (noise="torch": the draws are that slice of the whole batch's, and the generator advances as for the whole batch)"""
+        total = b_global0 + batch_size if total_layouts is None else int(total_layouts)
         T_eval = _cfg_get(sampling_cfg, "num_timesteps", self.num_timesteps)
         plan = timestep_plan(self.num_timesteps, T_eval, float(_cfg_get(sampling_cfg, "time_difference", 0.0)))
         cond_d = self._prepare_cond(cond, batch_size, sampling_cfg)
         if cond_d is not None:
             assert cond_d["seq"].shape[0] == batch_size
             assert cond_d["seq"].max().item() < self.num_classes
-        seed = self._new_seed() if seed is None else seed
+        if self.noise == "torch" and seed is not None:
+            raise ValueError("seed= selects the Philox contract; with noise='torch' the draws come from torch's CUDA generator")
+        seed = self._new_seed() if seed is None and self.noise == "contract" else seed
         if cond_d is not None and cond_d.get("type") == "relation" and "rel_adj" not in cond_d and self.logit_adjust_fn is not None:
             # an external (Python) logit adjustment between posterior and draw: per-step host loop through the log-prob taps
-            return self._sample_stepwise(batch_size, plan, cond_d, sampling_cfg, seed, b_global0, get_intermediate_results)
-        res = self.engine.sample_loop(batch_size, plan, sampling_cfg, cond_d, seed=seed, b_global0=b_global0, trace=get_intermediate_results)
+            return self._sample_stepwise(batch_size, plan, cond_d, sampling_cfg, seed, b_global0, get_intermediate_results, total)
+        loop = lambda noise: self.engine.sample_loop(batch_size, plan, sampling_cfg, cond_d, seed=seed or 0, b_global0=b_global0,
+                                                     trace=get_intermediate_results, noise=noise)
+        res = self._with_torch_noise(total, sampling_cfg, len(plan), None, loop) if self.noise == "torch" else loop(None)
         if get_intermediate_results:
             return [r for r in res[1].cpu()]
         return res.cpu()
 
-    def _sample_stepwise(self, B, plan, cond, sampling_cfg, seed, b_global0, trace):
+    def _sample_stepwise(self, B, plan, cond, sampling_cfg, seed, b_global0, trace, total=None):
         """per-step host loop: needed when a Python hook edits the log-probs between posterior and draw (cond=relation)"""
         ids = cond["seq"].clone() if cond else torch.full((B, self.max_token_length), self.vocab.mask_id, device=self.device)
         results = []
         for i, (t_model, t_post) in enumerate(plan):
-            ids = self._step_ids(ids, t_model, t_post, sampling_cfg, cond, seed, i, b_global0)
+            ids = self._step_ids(ids, t_model, t_post, sampling_cfg, cond, seed, i, b_global0, total)
             if trace:
                 results.append(ids.cpu())
         return results if trace else ids.cpu()
 
-    def _step_ids(self, ids, t_model, t_post, sampling_cfg, cond, seed, step_ctr, b_global0=0):
+    def _step_ids(self, ids, t_model, t_post, sampling_cfg, cond, seed, step_ctr, b_global0=0, total=None):
+        # noise="torch": the generator is read right before the step's draw (after the hook, which may draw from it as well)
+        def draw(**kw):
+            step = lambda noise: self.engine.step(ids, t_model, t_post, sampling_cfg, cond, seed, step_ctr, b_global0, noise=noise, **kw)[0]
+            if self.noise != "torch":
+                return step(None)
+            return self._with_torch_noise(b_global0 + ids.shape[0] if total is None else total, sampling_cfg, 1, None, step)
+        seed = seed or 0
         if cond is not None and cond.get("type") == "relation" and "rel_adj" not in cond and self.logit_adjust_fn is not None:
             # base.py:243-284 order: strong mask -> update() -> PAD-disable -> draw.  The first call returns the log-probs with the
             # strong mask only (PAD-disable off: `update` must see what the reference's sees), the hook edits them, PAD-disable
-            # is applied here, the second call draws from the result.  `t` is an int like in the reference (base.py:262).
+            # is applied here, the second call draws from the result.  `t` is an int like in the reference (base.py:262).  The first
+            # call's draw is discarded: it takes the contract's noise and leaves torch's generator alone.
             pre = dict(cond); pre["_pad_disable"] = False
             _, _, lp = self.engine.step(ids, t_model, t_post, sampling_cfg, pre, seed, step_ctr, b_global0, want_logprob=True)
             lp = self.logit_adjust_fn(int(t_model), cond, lp.permute(0, 2, 1).contiguous(), sampling_cfg)      # (B,C,S) like the reference
@@ -143,10 +179,8 @@ class FusedMaskAndReplaceDiffusion:
             S = ids.shape[1]
             pad_mask = (torch.arange(S, device=ids.device)[None] % self.vocab.n_attr != 0) & (cond["seq"] != self.vocab.pad_id)
             lp[..., self.vocab.pad_id] = torch.where(pad_mask, torch.full_like(lp[..., 0], -69.07755278982137), lp[..., self.vocab.pad_id])
-            out, _, _ = self.engine.step(ids, t_model, t_post, sampling_cfg, cond, seed, step_ctr, b_global0, logprob_in=lp)
-            return out
-        out, _, _ = self.engine.step(ids, t_model, t_post, sampling_cfg, cond, seed, step_ctr, b_global0)
-        return out
+            return draw(logprob_in=lp)
+        return draw()
 
     def _sample_single_step(self, log_z: torch.Tensor, model_t: torch.Tensor, skip_step: int, sampling_cfg=None,
                             cond: Optional[Dict] = None) -> torch.Tensor:
@@ -164,6 +198,9 @@ class FusedMaskAndReplaceDiffusion:
             cond_d = {k: (v.to(self.device) if isinstance(v, torch.Tensor) else v) for k, v in cond.items()}
             if cond_d.get("type") == "refinement" and "refine_table" not in cond_d:
                 cond_d = self._prepare_cond(cond_d, ids.shape[0], sampling_cfg)
+        if self.noise == "torch":      # one step's draws from torch's CUDA generator
+            out = self._step_ids(ids, t_model, t_post, sampling_cfg, cond_d, None, 0)
+            return index_to_log_onehot(out, self.num_classes)
         # noise key: like the reference, the draws come from torch's global generator -- a new key is derived from it at the start
         # of every trajectory (timesteps strictly decrease inside one), unless reset_noise(seed) pinned one
         if self._seed is None or (self._last_t is not None and t_model >= self._last_t and not self._pinned):
@@ -235,11 +272,16 @@ class FusedMaskAndReplaceDiffusion:
         return index_to_log_onehot((xt[..., None] == ids).long().argmax(-1), ids.numel())
 
     def sample_logits(self, logits: torch.Tensor, sampling_cfg, seed: Optional[int] = None) -> torch.Tensor:
-        """helpers/sampling.py:81-130 `sample(logits, sampling_cfg)`: (B,C,S) logits -> (B,1,S) ids"""
+        """helpers/sampling.py:81-130 `sample(logits, sampling_cfg)`: (B,C,S) logits -> (B,1,S) ids.  noise="torch": the draw of
+        the reference's `sample` on contiguous (B,C,S) logits, one step of torch's CUDA generator"""
         B = logits.shape[0]
         dummy = torch.zeros(B, self.vocab.S, dtype=torch.long, device=self.device)
-        out, _, _ = self.engine.step(dummy, 0, 0, sampling_cfg, None, self._new_seed() if seed is None else seed, 0,
-                                     logprob_in=logits.to(self.device).permute(0, 2, 1))
+        lp = logits.to(self.device).permute(0, 2, 1)
+        if self.noise == "torch":
+            out = self._with_torch_noise(B, sampling_cfg, 1, seed, lambda noise: self.engine.step(dummy, 0, 0, sampling_cfg, None, 0, 0, logprob_in=lp,
+                                                                                                   noise=noise)[0])
+        else:
+            out = self.engine.step(dummy, 0, 0, sampling_cfg, None, self._new_seed() if seed is None else seed, 0, logprob_in=lp)[0]
         return out[:, None, :]
 
     def q_sample(self, log_x_start: torch.Tensor, t: torch.Tensor, key: Optional[str] = None, seed: Optional[int] = None) -> torch.Tensor:
@@ -333,25 +375,29 @@ class FusedMaskAndReplaceDiffusion:
 class LayoutDMB200:
     """LayoutDM wrapper (models/layoutdm.py:26-97): `.sample()` returns decoded layouts on the CPU."""
 
-    def __init__(self, engine: Engine, tokenizer=None, bbox_centers=None):
-        self.model = FusedMaskAndReplaceDiffusion(engine, tokenizer, bbox_centers)
+    def __init__(self, engine: Engine, tokenizer=None, bbox_centers=None, noise: str = "contract"):
+        self.model = FusedMaskAndReplaceDiffusion(engine, tokenizer, bbox_centers, noise=noise)
         self.tokenizer = tokenizer
         self.vocab = engine.vocab
         self._centers = bbox_centers
 
     @classmethod
     def from_state_dict(cls, sd, dataset: str = "rico25", num_timesteps: int = 100, q_type: str = "constrained",
-                        operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None) -> "LayoutDMB200":
+                        operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None, noise: str = "contract") -> "LayoutDMB200":
+        """noise: "contract" (the project's Philox contract) or "torch" (torch's CUDA generator, FusedMaskAndReplaceDiffusion)"""
         vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else Vocab.for_dataset(dataset)
         eng = Engine.from_state_dict(sd, vocab, num_timesteps=num_timesteps, q_type=q_type, operand_dtype=operand_dtype, device=device)
-        return cls(eng, tokenizer, bbox_centers)
+        return cls(eng, tokenizer, bbox_centers, noise=noise)
 
     def eval(self):
         return self
 
-    def sample(self, batch_size: Optional[int] = 1, cond: Optional[Dict] = None, sampling_cfg=None, **kwargs) -> Dict[str, torch.Tensor]:
+    def sample(self, batch_size: Optional[int] = 1, cond: Optional[Dict] = None, sampling_cfg=None, total_layouts: Optional[int] = None,
+               **kwargs) -> Dict[str, torch.Tensor]:
         """layoutdm.py:77-88 (extra kwargs such as cond_type= / device= are swallowed like the reference does)"""
         kw = {k: v for k, v in kwargs.items() if k in ("seed", "b_global0", "get_intermediate_results")}
+        if total_layouts is not None:
+            kw["total_layouts"] = total_layouts
         ids = self.model.sample(batch_size=batch_size, cond=cond, sampling_cfg=sampling_cfg, **kw)
         if self.tokenizer is not None:
             return self.tokenizer.decode(ids)
@@ -389,17 +435,18 @@ class LayoutDMB200:
         return sampling_cfg
 
 
-def patch_reference_model(model, operand_dtype: str = "fp16", device=None):
+def patch_reference_model(model, operand_dtype: str = "fp16", device=None, noise: str = "contract"):
     """Drop-in for a live reference `trainer.models.layoutdm.LayoutDM`: after `load_state_dict`, call
     `patch_reference_model(model)`; `model.sample(...)` (layoutdm.py:77) and `model.model.sample(...)` /
-    `_sample_single_step(...)` then run on the sm_90a library.  Training `forward` is untouched."""
+    `_sample_single_step(...)` then run on the sm_90a library.  Training `forward` is untouched.
+    noise="torch": the draws come from torch's CUDA generator like the unpatched model's on the same GPU."""
     core = model.model.module if hasattr(model.model, "module") else model.model
     tok = model.tokenizer
     vocab = Vocab.from_tokenizer(tok)
     q_type = "vanilla" if type(core).__name__.startswith("Vanilla") else "constrained"
     eng = Engine.from_state_dict(model.state_dict(), vocab, num_timesteps=core.num_timesteps, q_type=q_type,
                                  operand_dtype=operand_dtype, device=device)
-    fused = FusedMaskAndReplaceDiffusion(eng, tok)
+    fused = FusedMaskAndReplaceDiffusion(eng, tok, noise=noise)
     # cond=relation: the reference's own gradient update (logit_adjustment.py:88-126) runs between the posterior and the draw.
     # `model` is a live reference object, so its package is importable; an import failure is an error, not a silent downgrade.
     import importlib

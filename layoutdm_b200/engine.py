@@ -172,10 +172,22 @@ class Engine:
             c.pad_disable = 1 if cond["_pad_disable"] else 0
         return c, keep
 
+    def noise_advance(self, total_layouts: int, sampling, n_steps: int) -> int:
+        """how far `n_steps` steps on a batch of `total_layouts` layouts move torch's CUDA generator (ldm_noise_advance)"""
+        s = sampling if isinstance(sampling, _lib.LdmSampling) else sampling_struct(sampling)
+        adv = int(self.lib.ldm_noise_advance(self._h, int(total_layouts), C.byref(s), int(n_steps)))
+        _lib.check(adv if adv < 0 else _lib.LDM_OK)
+        return adv
+
+    @staticmethod
+    def _noise(noise: Optional[_lib.LdmNoise], seed: int) -> _lib.LdmNoise:
+        return _lib.LdmNoise(_lib.NOISE_KINDS["contract"], seed, 0, 0) if noise is None else noise
+
     def step(self, ids_in: torch.Tensor, t_model: int, t_post: int, sampling, cond: Optional[dict] = None, seed: int = 0,
              step_ctr: int = 0, b_global0: int = 0, want_logits: bool = False, want_logprob: bool = False,
-             logits_in: Optional[torch.Tensor] = None, logprob_in: Optional[torch.Tensor] = None):
-        """one `_sample_single_step` on ids; returns (ids_out, logits | None, logprob | None), all on the GPU."""
+             logits_in: Optional[torch.Tensor] = None, logprob_in: Optional[torch.Tensor] = None, noise: Optional[_lib.LdmNoise] = None):
+        """one `_sample_single_step` on ids; returns (ids_out, logits | None, logprob | None), all on the GPU.
+        noise: an LdmNoise (torch-generator noise); None: the contract keyed by seed / step_ctr."""
         B, S = ids_in.shape
         assert S == self.vocab.S and ids_in.is_cuda and ids_in.dtype == torch.int64
         assert int(ids_in.max()) < self.vocab.C, f"Error: {int(ids_in.max())} >= {self.vocab.C}"     # util.py:35
@@ -187,15 +199,16 @@ class Engine:
         s = sampling if isinstance(sampling, _lib.LdmSampling) else sampling_struct(sampling)
         li = None if logits_in is None else logits_in.to(self.device, torch.float32).contiguous()
         pi = None if logprob_in is None else logprob_in.to(self.device, torch.float32).contiguous()
-        rc = self.lib.ldm_step(self._h, B, _ptr(ids_in), int(t_model), int(t_post), C.byref(c) if c else None, C.byref(s),
-                               C.c_uint64(seed), C.c_uint32(step_ctr), C.c_int64(b_global0), _ptr(out), _ptr(lg), _ptr(lp), _ptr(li), _ptr(pi),
-                               self._stream())
+        rc = self.lib.ldm_step_noise(self._h, B, _ptr(ids_in), int(t_model), int(t_post), C.byref(c) if c else None, C.byref(s),
+                                     C.byref(self._noise(noise, seed)), C.c_uint32(step_ctr), C.c_int64(b_global0), _ptr(out), _ptr(lg),
+                                     _ptr(lp), _ptr(li), _ptr(pi), self._stream())
         _lib.check(rc)
         return out, lg, lp
 
     def sample_loop(self, B: int, plan: Sequence[Tuple[int, int]], sampling, cond: Optional[dict] = None, seed: int = 0,
-                    b_global0: int = 0, ids_init: Optional[torch.Tensor] = None, trace: bool = False):
-        """whole T-step loop on the device; returns ids (B,S) [and the (n_steps,B,S) trace] as CUDA tensors."""
+                    b_global0: int = 0, ids_init: Optional[torch.Tensor] = None, trace: bool = False, noise: Optional[_lib.LdmNoise] = None):
+        """whole T-step loop on the device; returns ids (B,S) [and the (n_steps,B,S) trace] as CUDA tensors.
+        noise: an LdmNoise (torch-generator noise, step k at its offset + k steps); None: the contract keyed by seed."""
         n = len(plan)
         tm = (C.c_int32 * n)(*[p[0] for p in plan])
         tp = (C.c_int32 * n)(*[p[1] for p in plan])
@@ -205,8 +218,8 @@ class Engine:
         s = sampling if isinstance(sampling, _lib.LdmSampling) else sampling_struct(sampling)
         if ids_init is not None:
             ids_init = ids_init.to(self.device, torch.int64).contiguous()
-        rc = self.lib.ldm_sample_loop(self._h, B, n, tm, tp, C.byref(c) if c else None, C.byref(s), C.c_uint64(seed), C.c_int64(b_global0),
-                                      _ptr(ids_init), _ptr(out), _ptr(tr), self._stream())
+        rc = self.lib.ldm_sample_loop_noise(self._h, B, n, tm, tp, C.byref(c) if c else None, C.byref(s), C.byref(self._noise(noise, seed)),
+                                            C.c_int64(b_global0), _ptr(ids_init), _ptr(out), _ptr(tr), self._stream())
         _lib.check(rc)
         return (out, tr) if trace else out
 

@@ -4,6 +4,7 @@ noise is keyed by the GLOBAL layout index so the result does not depend on the n
 collective is one all-gather of the final ids (NCCL over NVLink on GPUs, gloo in the CPU tests)."""
 from __future__ import annotations
 
+import inspect
 from typing import Callable, Dict, Optional, Tuple
 
 import torch
@@ -46,8 +47,12 @@ def all_gather_ids(local: torch.Tensor, total: int, group=None) -> torch.Tensor:
 
 
 def sample_sharded(sample_fn: Callable[..., torch.Tensor], total: int, cond: Optional[Dict] = None, group=None, **kw) -> torch.Tensor:
-    """sample_fn(batch_size=, cond=, b_global0=, **kw) -> (b, S) ids on this rank's device; returns all `total` layouts."""
+    """sample_fn(batch_size=, cond=, b_global0=, **kw) -> (b, S) ids on this rank's device; returns all `total` layouts.
+    A sample_fn with a `total_layouts` parameter gets the global batch size: torch-generator noise draws each shard's slice of
+    the whole batch's draw."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     lo, hi = shard_bounds(total, world, rank)
+    if "total_layouts" in inspect.signature(sample_fn).parameters:
+        kw["total_layouts"] = total
     local = sample_fn(batch_size=hi - lo, cond=shard_cond(cond, lo, hi), b_global0=lo, **kw)
     return all_gather_ids(local, total, group)
