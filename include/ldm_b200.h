@@ -54,7 +54,7 @@ typedef struct {
   double att_1, att_T, ctt_1, ctt_T;  /* alpha_schedule() endpoints, util.py:47-49 */
 } LdmModelDesc;
 
-/* fp32 host arrays in the reference's own parameter layout (state_dict, SURVEY.md 8a-a5), layers stacked on dim 0.
+/* fp32 arrays (host for ldm_create, device for ldm_load_weights) in the reference's own parameter layout (state_dict, SURVEY.md 8a-a5), layers stacked on dim 0.
  * C = n_cat + 4*n_bins + 2, S = n_elem*n_attr, d = d_model, f = d_ff, L = n_layers, T = num_timesteps. */
 typedef struct {
   const float* cat_emb;      /* [C][d]        transformer.cat_emb.weight */
@@ -130,6 +130,14 @@ typedef struct {
  * schedule tables, TMA descriptors).  Replaces model construction + .to(device) for the sampling path. */
 int ldm_create(const LdmModelDesc* desc, const LdmWeights* weights, LdmHandle** out);
 int ldm_destroy(LdmHandle* h);
+/* Repack new weights into the handle's existing buffers on `stream` (what ldm_create does with its host arrays), so that a
+ * handle follows a model being trained or given another checkpoint.  w: fp32 DEVICE pointers on the handle's device, in the
+ * LdmWeights layout and the shapes of the handle's LdmModelDesc (a different shape is a new handle, not a reload).  No
+ * allocation and no synchronisation; tensor maps and a captured loop graph stay valid (the addresses do not change).  Work
+ * already queued on `stream` sees the old weights, later work the new ones; work on other streams must be ordered by the
+ * caller, as for every call on a handle.  The arrays must stay valid until the work queued here has run.
+ * A null handle, a null field or a pointer that is not device memory of the handle's device: LDM_ERR_INVALID. */
+int ldm_load_weights(LdmHandle* h, const LdmWeights* weights_dev, void* stream);
 
 /* One denoising step == BaseMaskAndReplaceDiffusion._sample_single_step (base.py:205-291) on token ids:
  *   ids_in_dev [B][S] (x_t)  ->  ids_out_dev [B][S] (x_{t-1}).

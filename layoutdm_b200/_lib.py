@@ -53,6 +53,7 @@ class LdmNoise(C.Structure):
 SIGNATURES = {
     "ldm_create": (C.c_int, [C.POINTER(LdmModelDesc), C.POINTER(LdmWeights), C.POINTER(C.c_void_p)]),
     "ldm_destroy": (C.c_int, [C.c_void_p]),
+    "ldm_load_weights": (C.c_int, [C.c_void_p, C.POINTER(LdmWeights), C.c_void_p]),
     "ldm_step": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(LdmCond), C.POINTER(LdmSampling),
                            C.c_uint64, C.c_uint32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ldm_sample_loop": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(LdmCond),

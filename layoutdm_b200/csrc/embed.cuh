@@ -1,5 +1,5 @@
 // Front of the denoiser: token + positional embedding and the first block's timestep-adaptive LayerNorm;
-// plus the one-off precomputation of the AdaLN (scale, shift) table.
+// plus the weight packing (AdaLN (scale, shift) table, 16-bit operands, padded QKV bias) of ldm_create / ldm_load_weights.
 //   h  = cat_emb[id] + pos[s]                                   T/models/common/nn_lib.py:204,220 (+ :112-127)
 //   x  = LN(h) * (1 + scale_t) + shift_t                        T/models/transformer_utils.py:79-83
 // One warp per token row; pad rows (s >= 125 of each 128-row layout tile) are written as zeros so that every
@@ -42,6 +42,16 @@ __global__ void pack_weight_kernel(const float* __restrict__ src, void* __restri
     if constexpr (kOpSplit<MODE>) O::from_pair(v, dst[i], static_cast<typename O::T*>(dst_lo)[i]);
     else dst[i] = O::from(v);
   }
+}
+
+// per-head padded QKV bias: dst[r] = src[row_map[r]] (0 where row_map[r] < 0), except column v_col of every V head (rows
+// r >= v_first), which is 1: with its zero weight row it makes the attention kernel's PV MMA deliver the softmax denominator
+__global__ void qkv_bias_kernel(const float* __restrict__ src, const int* __restrict__ row_map, float* __restrict__ dst, int n, int v_first,
+                                int head_pad, int v_col) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const int sr = row_map[r];
+  dst[r] = (r >= v_first && (r - v_first) % head_pad == v_col) ? 1.0f : (sr >= 0 ? src[sr] : 0.0f);
 }
 
 // one token row: h = cat_emb[id] + pos[s]; x = LN(h) * (1 + scale_t) + shift_t -> fp32 residual row + 16-bit operand row (whole warp;

@@ -142,6 +142,7 @@ struct LdmHandle {
   CUtensorMap m_wqkv[kMaxLayers], m_wo[kMaxLayers], m_w1[kMaxLayers], m_w2[kMaxLayers], m_whead;
   void *wqkv_lo[kMaxLayers] = {}, *wo_lo[kMaxLayers] = {}, *w1_lo[kMaxLayers] = {}, *w2_lo[kMaxLayers] = {}, *whead_lo = nullptr;
   CUtensorMap m_wqkv_lo[kMaxLayers], m_wo_lo[kMaxLayers], m_w1_lo[kMaxLayers], m_w2_lo[kMaxLayers], m_whead_lo;
+  int *qmap = nullptr, *amap = nullptr, *hmap = nullptr;   // source row / column maps of the padded QKV, out-projection and head weights
   // workspace (device), sized for cap layouts
   int cap = 0;
   void *x16 = nullptr, *qkv16 = nullptr, *att16 = nullptr, *z16 = nullptr, *hid16 = nullptr;
@@ -203,19 +204,72 @@ void free_staging(LdmHandle* h) {
   h->staging.clear();
 }
 
-// 16-bit weight (split mode: the hi plane in dst, the lo plane in dst_lo)
-int pack16(LdmHandle* h, void** dst, void** dst_lo, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
-           const int* col_map_dev = nullptr) {
-  const size_t bytes = static_cast<size_t>(dst_rows) * dst_cols * 2;
+// 16-bit weight buffer of rows x cols (split mode: the hi plane in dst, the lo plane in dst_lo)
+int alloc16(LdmHandle* h, void** dst, void** dst_lo, int rows, int cols) {
+  const size_t bytes = static_cast<size_t>(rows) * cols * 2;
   CK(cudaMalloc(dst, bytes));
   h->owned.push_back(*dst);
   if (h->split) { CK(cudaMalloc(dst_lo, bytes)); h->owned.push_back(*dst_lo); }
+  return LDM_OK;
+}
+
+// fp32 weight -> the 16-bit operand in dst (split mode: both planes), on stream st
+int pack16(const LdmHandle* h, void* dst, void* dst_lo, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
+           cudaStream_t st, const int* col_map_dev = nullptr) {
   const int blocks = 512;
-  if (h->mode == OP_BF16X3) pack_weight_kernel<OP_BF16X3><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, *dst_lo);
-  else if (h->mode == OP_BF16) pack_weight_kernel<OP_BF16><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
-  else pack_weight_kernel<OP_F16><<<blocks, 256>>>(src_dev, *dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
+  if (h->mode == OP_BF16X3) pack_weight_kernel<OP_BF16X3><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, dst_lo);
+  else if (h->mode == OP_BF16) pack_weight_kernel<OP_BF16><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
+  else pack_weight_kernel<OP_F16><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
   CK(cudaGetLastError());
   return LDM_OK;
+}
+
+// the fields of LdmWeights with their element counts for the handle's shapes
+struct WeightField { const float* LdmWeights::*member; const char* name; size_t n; };
+std::vector<WeightField> weight_fields(const LdmHandle* h) {
+  const size_t d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T, C = h->C, S = h->S;
+  return {{&LdmWeights::cat_emb, "cat_emb", C * d},         {&LdmWeights::pos_table, "pos_table", S * d},
+          {&LdmWeights::in_proj_w, "in_proj_w", L * 3 * d * d}, {&LdmWeights::in_proj_b, "in_proj_b", L * 3 * d},
+          {&LdmWeights::out_proj_w, "out_proj_w", L * d * d},   {&LdmWeights::out_proj_b, "out_proj_b", L * d},
+          {&LdmWeights::linear1_w, "linear1_w", L * ff * d},    {&LdmWeights::linear1_b, "linear1_b", L * ff},
+          {&LdmWeights::linear2_w, "linear2_w", L * d * ff},    {&LdmWeights::linear2_b, "linear2_b", L * d},
+          {&LdmWeights::norm1_emb, "norm1_emb", L * T * d},     {&LdmWeights::norm1_w, "norm1_w", L * 2 * d * d},
+          {&LdmWeights::norm1_b, "norm1_b", L * 2 * d},         {&LdmWeights::norm2_w, "norm2_w", L * d},
+          {&LdmWeights::norm2_b, "norm2_b", L * d},             {&LdmWeights::head_ln_w, "head_ln_w", d},
+          {&LdmWeights::head_ln_b, "head_ln_b", d},             {&LdmWeights::head_w, "head_w", C * d}};
+}
+
+// Repacks fp32 DEVICE weights in the LdmWeights layout into the handle's parameter buffers, on stream st: ldm_create runs it on
+// its staged host arrays, ldm_load_weights on the caller's.  The kernels are plain launches (no programmatic dependent launch),
+// so each starts only once all earlier work of st has completed; every step kernel reads a weight only after its pdl_sync()
+// (common.cuh), so a step queued after this routine reads the new weights (DESIGN.md, "Weights").
+int pack_weights(LdmHandle* h, const LdmWeights& w, cudaStream_t st) {
+  const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
+  const auto copy = [&](float* dst, const float* src, size_t n) { return cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st); };
+  CK(copy(h->cat_emb, w.cat_emb, static_cast<size_t>(h->C) * d));
+  CK(copy(h->pos, w.pos_table, static_cast<size_t>(h->S) * d));
+  CK(copy(h->hlnw, w.head_ln_w, d));
+  CK(copy(h->hlnb, w.head_ln_b, d));
+  // AdaLN (scale, shift) for every (layer, t)
+  adaln_table_kernel<<<dim3(T, L), 256, d * sizeof(float), st>>>(w.norm1_emb, w.norm1_w, w.norm1_b, h->adaln, T, d);
+  CK(cudaGetLastError());
+  int rc;
+  for (int l = 0; l < L; ++l) {
+    const size_t dd = static_cast<size_t>(d) * d;
+    if ((rc = pack16(h, h->wqkv[l], h->wqkv_lo[l], w.in_proj_w + l * 3 * dd, h->qmap, kQkvN, d, d, st))) return rc;
+    qkv_bias_kernel<<<(kQkvN + 255) / 256, 256, 0, st>>>(w.in_proj_b + static_cast<size_t>(l) * 3 * d, h->qmap, h->bqkv[l], kQkvN,
+                                                        2 * 8 * kHeadPad, kHeadPad, d / h->desc.n_heads);
+    CK(cudaGetLastError());
+    if ((rc = pack16(h, h->wo[l], h->wo_lo[l], w.out_proj_w + l * dd, nullptr, d, kAttN, d, st, h->amap))) return rc;   // K = 512: head h occupies columns h*64 .. h*64+57
+    CK(copy(h->bo[l], w.out_proj_b + static_cast<size_t>(l) * d, d));
+    if ((rc = pack16(h, h->w1[l], h->w1_lo[l], w.linear1_w + l * ff * static_cast<size_t>(d), nullptr, ff, d, d, st))) return rc;
+    CK(copy(h->b1[l], w.linear1_b + static_cast<size_t>(l) * ff, ff));
+    if ((rc = pack16(h, h->w2[l], h->w2_lo[l], w.linear2_w + l * ff * static_cast<size_t>(d), nullptr, d, ff, ff, st))) return rc;
+    CK(copy(h->b2[l], w.linear2_b + static_cast<size_t>(l) * d, d));
+    CK(copy(h->ln2w[l], w.norm2_w + static_cast<size_t>(l) * d, d));
+    CK(copy(h->ln2b[l], w.norm2_b + static_cast<size_t>(l) * d, d));
+  }
+  return pack16(h, h->whead, h->whead_lo, w.head_w, h->hmap, kLogitLd, d, d, st);
 }
 
 // TMA descriptor(s) of one 16-bit operand (split mode: both planes), boxes of box_rows x kb elements
@@ -660,21 +714,30 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (const char* e = getenv("LDM_GEMM_CTAS")) h->gemm_ctas = std::max(1, atoi(e));
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
-  TRY(dev_upload(h, &h->cat_emb, w->cat_emb, static_cast<size_t>(C) * d));
-  TRY(dev_upload(h, &h->pos, w->pos_table, static_cast<size_t>(S) * d));
-  TRY(dev_upload(h, &h->hlnw, w->head_ln_w, static_cast<size_t>(d)));
-  TRY(dev_upload(h, &h->hlnb, w->head_ln_b, static_cast<size_t>(d)));
-
-  // AdaLN (scale, shift) for every (layer, t)
-  {
-    float *emb = nullptr, *lw = nullptr, *lb = nullptr;
-    TRY(dev_upload_tmp(h, &emb, w->norm1_emb, static_cast<size_t>(L) * T * d));
-    TRY(dev_upload_tmp(h, &lw, w->norm1_w, static_cast<size_t>(L) * 2 * d * d));
-    TRY(dev_upload_tmp(h, &lb, w->norm1_b, static_cast<size_t>(L) * 2 * d));
-    TRY(dev_alloc(h, &h->adaln, static_cast<size_t>(L) * T * 2 * d));
-    adaln_table_kernel<<<dim3(T, L), 256, d * sizeof(float)>>>(emb, lw, lb, h->adaln, T, d);
-    if (cudaGetLastError() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "adaln_table_kernel launch failed"); }
+  // parameter buffers and the TMA descriptors of the 16-bit weights
+  TRY(dev_alloc(h, &h->cat_emb, static_cast<size_t>(C) * d));
+  TRY(dev_alloc(h, &h->pos, static_cast<size_t>(S) * d));
+  TRY(dev_alloc(h, &h->hlnw, static_cast<size_t>(d)));
+  TRY(dev_alloc(h, &h->hlnb, static_cast<size_t>(d)));
+  TRY(dev_alloc(h, &h->adaln, static_cast<size_t>(L) * T * 2 * d));
+  for (int l = 0; l < L; ++l) {
+    TRY(alloc16(h, &h->wqkv[l], &h->wqkv_lo[l], kQkvN, d));
+    TRY(alloc16(h, &h->wo[l], &h->wo_lo[l], d, kAttN));
+    TRY(alloc16(h, &h->w1[l], &h->w1_lo[l], ff, d));
+    TRY(alloc16(h, &h->w2[l], &h->w2_lo[l], d, ff));
+    TRY(dev_alloc(h, &h->bqkv[l], static_cast<size_t>(kQkvN)));
+    TRY(dev_alloc(h, &h->bo[l], static_cast<size_t>(d)));
+    TRY(dev_alloc(h, &h->b1[l], static_cast<size_t>(ff)));
+    TRY(dev_alloc(h, &h->b2[l], static_cast<size_t>(d)));
+    TRY(dev_alloc(h, &h->ln2w[l], static_cast<size_t>(d)));
+    TRY(dev_alloc(h, &h->ln2b[l], static_cast<size_t>(d)));
+    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN, gemm_kb(h->split)));   // one warpgroup's weight rows per box
+    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, kLnKB));
+    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN, gemm_kb(h->split)));
+    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, kLnKB));
   }
+  TRY(alloc16(h, &h->whead, &h->whead_lo, kLogitLd, d));
+  TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN, gemm_kb(h->split)));
 
   // per-head padded QKV row map: dst row = which*512 + head*64 + j  <-  src row which*d + head*58 + j (j < 58)
   const int dh = d / desc->n_heads;
@@ -683,48 +746,22 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     const int which = r / (8 * kHeadPad), hh = (r % (8 * kHeadPad)) / kHeadPad, j = r % kHeadPad;
     qmap[r] = j < dh ? which * d + hh * dh + j : -1;
   }
-  int* qmap_dev = nullptr;
-  TRY(dev_upload(h, &qmap_dev, qmap.data(), qmap.size()));
+  TRY(dev_upload(h, &h->qmap, qmap.data(), qmap.size()));
   std::vector<int> amap(kAttN);
   for (int c = 0; c < kAttN; ++c) amap[c] = (c % kHeadPad) < dh ? (c / kHeadPad) * dh + (c % kHeadPad) : -1;
-  int* amap_dev = nullptr;
-  TRY(dev_upload(h, &amap_dev, amap.data(), amap.size()));
+  TRY(dev_upload(h, &h->amap, amap.data(), amap.size()));
+  std::vector<int> hmap(kLogitLd);
+  for (int r = 0; r < kLogitLd; ++r) hmap[r] = r < C ? r : -1;
+  TRY(dev_upload(h, &h->hmap, hmap.data(), hmap.size()));
 
-  for (int l = 0; l < L; ++l) {
-    float* tmp = nullptr;
-    TRY(dev_upload_tmp(h, &tmp, w->in_proj_w + static_cast<size_t>(l) * 3 * d * d, static_cast<size_t>(3) * d * d));
-    TRY(pack16(h, &h->wqkv[l], &h->wqkv_lo[l], tmp, qmap_dev, kQkvN, d, d));
-    std::vector<float> bq(kQkvN, 0.0f);
-    for (int r = 0; r < kQkvN; ++r) if (qmap[r] >= 0) bq[r] = w->in_proj_b[static_cast<size_t>(l) * 3 * d + qmap[r]];
-    // column dh of every V head = 1 (zero weight row + unit bias): the attention kernel reads the softmax denominator from it
-    for (int hh = 0; hh < desc->n_heads; ++hh) bq[2 * 8 * kHeadPad + hh * kHeadPad + dh] = 1.0f;
-    TRY(dev_upload(h, &h->bqkv[l], bq.data(), bq.size()));
-    TRY(dev_upload_tmp(h, &tmp, w->out_proj_w + static_cast<size_t>(l) * d * d, static_cast<size_t>(d) * d));
-    TRY(pack16(h, &h->wo[l], &h->wo_lo[l], tmp, nullptr, d, kAttN, d, amap_dev));      // K = 512: head h occupies columns h*64 .. h*64+57
-    TRY(dev_upload(h, &h->bo[l], w->out_proj_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(dev_upload_tmp(h, &tmp, w->linear1_w + static_cast<size_t>(l) * ff * d, static_cast<size_t>(ff) * d));
-    TRY(pack16(h, &h->w1[l], &h->w1_lo[l], tmp, nullptr, ff, d, d));
-    TRY(dev_upload(h, &h->b1[l], w->linear1_b + static_cast<size_t>(l) * ff, static_cast<size_t>(ff)));
-    TRY(dev_upload_tmp(h, &tmp, w->linear2_w + static_cast<size_t>(l) * d * ff, static_cast<size_t>(d) * ff));
-    TRY(pack16(h, &h->w2[l], &h->w2_lo[l], tmp, nullptr, d, ff, ff));
-    TRY(dev_upload(h, &h->b2[l], w->linear2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(dev_upload(h, &h->ln2w[l], w->norm2_w + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(dev_upload(h, &h->ln2b[l], w->norm2_b + static_cast<size_t>(l) * d, static_cast<size_t>(d)));
-    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN, gemm_kb(h->split)));   // one warpgroup's weight rows per box
-    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, kLnKB));
-    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN, gemm_kb(h->split)));
-    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, kLnKB));
+  // the host arrays, staged on the device, then packed as ldm_load_weights packs device arrays
+  LdmWeights staged{};
+  for (const WeightField& f : weight_fields(h)) {
+    float* p = nullptr;
+    TRY(dev_upload_tmp(h, &p, w->*f.member, f.n));
+    staged.*f.member = p;
   }
-  {
-    float* tmp = nullptr;
-    TRY(dev_upload_tmp(h, &tmp, w->head_w, static_cast<size_t>(C) * d));
-    std::vector<int> hmap(kLogitLd);
-    for (int r = 0; r < kLogitLd; ++r) hmap[r] = r < C ? r : -1;
-    int* hmap_dev = nullptr;
-    TRY(dev_upload(h, &hmap_dev, hmap.data(), hmap.size()));
-    TRY(pack16(h, &h->whead, &h->whead_lo, tmp, hmap_dev, kLogitLd, d, d));
-    TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN, gemm_kb(h->split)));
-  }
+  TRY(pack_weights(h, staged, nullptr));
   {
     std::vector<float> sch(static_cast<size_t>(h->G) * 8 * (T + 1));
     for (int g = 0; g < h->G; ++g) {
@@ -758,6 +795,23 @@ int ldm_destroy(LdmHandle* h) {
   if (h->c_tbl) cudaFree(h->c_tbl);
   delete h;
   return LDM_OK;
+}
+
+int ldm_load_weights(LdmHandle* h, const LdmWeights* w, void* stream) {
+  if (!h || !w) return fail(LDM_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(h->desc.device));
+  for (const WeightField& f : weight_fields(h)) {
+    const float* p = w->*f.member;
+    if (!p) return fail(LDM_ERR_INVALID, "LdmWeights.%s is null", f.name);
+    // a host or other-device pointer would fault in the packing kernels: reject it here
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) ||
+        a.device != h->desc.device) {
+      cudaGetLastError();
+      return fail(LDM_ERR_INVALID, "LdmWeights.%s is not device memory of device %d", f.name, h->desc.device);
+    }
+  }
+  return pack_weights(h, *w, static_cast<cudaStream_t>(stream));
 }
 
 int ldm_step_noise(LdmHandle* h, int32_t B, const int64_t* ids_in, int32_t t_model, int32_t t_post, const LdmCond* cond,

@@ -12,10 +12,12 @@ exactly where the reference returns CPU tensors.
 from __future__ import annotations
 
 import copy
+import weakref
 from typing import Any, Dict, List, Optional, Union
 
 import torch
 import torch.nn.functional as F
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import _lib
 from .engine import Engine, sampling_struct
@@ -48,6 +50,62 @@ def duplicate_cond(cond: Dict, batch_size: int) -> Dict:
     return cond
 
 
+_FOLLOWERS: "weakref.WeakSet[WeightFollower]" = weakref.WeakSet()
+_STEP_HOOK = None
+
+
+def _optimizer_stepped(optimizer, args, kwargs):
+    """optimizer step post-hook: marks the followers of the parameters it stepped dirty.  A fused AdamW step writes the
+    parameters without bumping their version counters, so the fingerprint alone would miss it."""
+    stepped = None
+    for f in list(_FOLLOWERS):
+        if stepped is None:
+            stepped = {id(p) for g in optimizer.param_groups for p in g["params"]}
+        if not stepped.isdisjoint(f.param_ids):
+            f.dirty = True
+
+
+class WeightFollower:
+    """Keeps a target's packed weights equal to a live module's parameters.  target: anything with `load_weights(dict)` (the
+    `Engine.pack_state_dict` dict), `vocab` and `device`, i.e. an Engine.
+
+    `check()` reloads when the parameters may have changed since the last load: a parameter's storage (`data_ptr`: a
+    parameter replaced, `model.cpu()` / `.cuda()`) or version counter (in-place writes such as `load_state_dict` or a foreach
+    optimizer step) differs, or an optimizer stepped one of them (the dirty flag, set by a step post-hook).  Writes through
+    `.data` bypass all of these; call `reload()` after them.  An unchanged module costs the fingerprint only."""
+
+    def __init__(self, module: torch.nn.Module, target):
+        global _STEP_HOOK
+        self.module, self.target = module, target
+        self.reloads = 0
+        self.dirty = False
+        self._fp = self._fingerprint()
+        _FOLLOWERS.add(self)
+        if _STEP_HOOK is None:        # one hook for every follower; it holds them only through the weak set
+            _STEP_HOOK = register_optimizer_step_post_hook(_optimizer_stepped)
+
+    def _fingerprint(self):
+        params = list(self.module.parameters())
+        self.param_ids = frozenset(id(p) for p in params)
+        return tuple((p.data_ptr(), p._version) for p in params)
+
+    def check(self) -> bool:
+        """reload if the module may have changed; True if it did"""
+        fp = self._fingerprint()
+        if self.dirty or fp != self._fp:
+            self.reload(fp)
+            return True
+        return False
+
+    def reload(self, fp=None):
+        """repack the module's current parameters into the target unconditionally"""
+        sd = self.module.state_dict()
+        self.target.load_weights(Engine.pack_state_dict(sd, self.target.vocab, device=self.target.device))
+        self._fp = self._fingerprint() if fp is None else fp
+        self.dirty = False
+        self.reloads += 1
+
+
 class FusedMaskAndReplaceDiffusion:
     """noise="contract": the draws use the project's Philox contract keyed by a seed (drawn from torch's generator unless
     given).  noise="torch": they are the numbers torch's CUDA generator gives the reference's `sample` on the same GPU, and
@@ -73,10 +131,32 @@ class FusedMaskAndReplaceDiffusion:
         self._last_t: Optional[int] = None
         self.relation_on_device = True   # cond=relation, relation_mode "average": hand-derived update kernel; False: logit_adjust_fn hook
         self.logit_adjust_fn = None      # optional hook f(t: int, cond, model_log_prob (B,C,S), sampling_cfg) for cond=relation
+        self._weights: Optional[WeightFollower] = None   # the live module whose parameters the engine follows (follow())
 
     @property
     def device(self) -> torch.device:
         return self.engine.device
+
+    # ---- weights -------------------------------------------------------------------------------------
+    def follow(self, module: torch.nn.Module):
+        """take the denoiser's weights from `module` (the reference's CategoricalTransformer, whose state_dict the engine was
+        built from): every call that runs the denoiser first reloads them if they may have changed (WeightFollower)"""
+        self._weights = WeightFollower(module, self.engine)
+
+    def reload_weights(self):
+        """repack the followed module's parameters now: needed after writes through `.data`, which nothing detects"""
+        if self._weights is None:
+            raise ValueError("no weight source: follow(module) first (patch_reference_model does)")
+        self._weights.reload()
+
+    @property
+    def weight_reloads(self) -> int:
+        """how many times the followed module's weights have been repacked"""
+        return 0 if self._weights is None else self._weights.reloads
+
+    def _follow_weights(self):
+        if self._weights is not None:
+            self._weights.check()
 
     # ---- helpers -------------------------------------------------------------------------------------
     def _prepare_cond(self, cond: Optional[Dict], batch_size: int, sampling_cfg) -> Optional[Dict]:
@@ -129,6 +209,7 @@ class FusedMaskAndReplaceDiffusion:
                total_layouts: Optional[int] = None, **kwargs) -> Union[torch.LongTensor, List[torch.LongTensor]]:
         """base.py:293-371.  total_layouts: the whole batch when this call samples layouts [b_global0, b_global0 + batch_size)
         of it (noise="torch": the draws are that slice of the whole batch's, and the generator advances as for the whole batch)"""
+        self._follow_weights()
         total = b_global0 + batch_size if total_layouts is None else int(total_layouts)
         T_eval = _cfg_get(sampling_cfg, "num_timesteps", self.num_timesteps)
         plan = timestep_plan(self.num_timesteps, T_eval, float(_cfg_get(sampling_cfg, "time_difference", 0.0)))
@@ -186,6 +267,7 @@ class FusedMaskAndReplaceDiffusion:
                             cond: Optional[Dict] = None) -> torch.Tensor:
         """base.py:205-291 ; log_z (B,C,S) -> log_z (B,C,S).  Kept for API compatibility (the notebook and subclasses call it);
         `sample()` itself never materialises (B,C,S) tensors."""
+        self._follow_weights()
         ids = log_z.argmax(1).to(self.device)
         t_model = int(model_t[0].item())
         assert bool((model_t == t_model).all())
@@ -218,6 +300,7 @@ class FusedMaskAndReplaceDiffusion:
 
     def predict_start(self, log_x_t: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
         """base.py:127-146: log_x_t (B,C,S) log one-hot, t (B,) -> log p(x0|xt) (B,C,S)"""
+        self._follow_weights()
         return self.engine.predict_start(log_x_t.argmax(1), t).permute(0, 2, 1).contiguous()
 
     def q_posterior(self, log_x_start: torch.Tensor, log_x_t: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
@@ -319,6 +402,7 @@ class FusedMaskAndReplaceDiffusion:
                 seed: Optional[int] = None):
         """constrained.py:232-333 / vanilla.py:177-243, FORWARD ONLY (validation loss; no autograd graph is built -- the optimiser
         step of the reference's training loop stays out of scope).  x (B,S) ids -> ({"probs": (B,C,S)}, {"kl_loss", "aux_loss"})."""
+        self._follow_weights()
         if not hasattr(self, "Lt_history"):
             self.Lt_history = torch.zeros(self.num_timesteps, device=self.device)
             self.Lt_count = torch.zeros(self.num_timesteps, device=self.device)
@@ -367,6 +451,7 @@ class FusedMaskAndReplaceDiffusion:
 
     def predict_logits(self, ids: torch.Tensor, t: int) -> torch.Tensor:
         """CategoricalTransformer.forward (nn_lib.py:191-237): ids (B,S) -> logits (B,S,C) on the GPU"""
+        self._follow_weights()
         s = sampling_struct({"name": "deterministic"})
         _, lg, _ = self.engine.step(ids.to(self.device), t, t, s, want_logits=True)
         return lg
@@ -390,6 +475,12 @@ class LayoutDMB200:
         return cls(eng, tokenizer, bbox_centers, noise=noise)
 
     def eval(self):
+        return self
+
+    def load_state_dict(self, sd) -> "LayoutDMB200":
+        """repack another checkpoint of the same shapes into the engine in place, like the reference's
+        `model.load_state_dict(torch.load(...))` (test.py's load_model); returns self"""
+        self.model.engine.load_state_dict(sd)
         return self
 
     def sample(self, batch_size: Optional[int] = 1, cond: Optional[Dict] = None, sampling_cfg=None, total_layouts: Optional[int] = None,
@@ -436,9 +527,11 @@ class LayoutDMB200:
 
 
 def patch_reference_model(model, operand_dtype: str = "fp16", device=None, noise: str = "contract"):
-    """Drop-in for a live reference `trainer.models.layoutdm.LayoutDM`: after `load_state_dict`, call
-    `patch_reference_model(model)`; `model.sample(...)` (layoutdm.py:77) and `model.model.sample(...)` /
-    `_sample_single_step(...)` then run on the sm_90a library.  Training `forward` is untouched.
+    """Drop-in for a live reference `trainer.models.layoutdm.LayoutDM`: after `patch_reference_model(model)`,
+    `model.sample(...)` (layoutdm.py:77) and `model.model.sample(...)` / `_sample_single_step(...)` run on the sm_90a library.
+    Training `forward` is untouched.  The library follows the model's weights: optimizer steps, `load_state_dict` and device
+    moves after patching are picked up by the next sampling call (WeightFollower); after writes through `.data`, call
+    `model.model.module._ldm_b200.reload_weights()`.
     noise="torch": the draws come from torch's CUDA generator like the unpatched model's on the same GPU."""
     core = model.model.module if hasattr(model.model, "module") else model.model
     tok = model.tokenizer
@@ -447,6 +540,7 @@ def patch_reference_model(model, operand_dtype: str = "fp16", device=None, noise
     eng = Engine.from_state_dict(model.state_dict(), vocab, num_timesteps=core.num_timesteps, q_type=q_type,
                                  operand_dtype=operand_dtype, device=device)
     fused = FusedMaskAndReplaceDiffusion(eng, tok, noise=noise)
+    fused.follow(core.transformer)
     # cond=relation: the reference's own gradient update (logit_adjustment.py:88-126) runs between the posterior and the draw.
     # `model` is a live reference object, so its package is importable; an import failure is an error, not a silent downgrade.
     import importlib

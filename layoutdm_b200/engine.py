@@ -56,6 +56,7 @@ class Engine:
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         self.device = torch.device("cuda", self.device_index)
         L = weights["in_proj_w"].shape[0]
+        self.n_layers, self.d_model, self.d_ff = L, d_model, d_ff
         desc = _lib.LdmModelDesc(vocab.n_cat, vocab.n_bins, vocab.n_elem, vocab.n_attr, d_model, n_heads, d_ff, L, num_timesteps,
                                  {"constrained": 0, "vanilla": 1}[q_type], _lib.OPERAND_DTYPES[operand_dtype], self.device_index,
                                  att_1, att_T, ctt_1, ctt_T)
@@ -76,9 +77,12 @@ class Engine:
         return cls(vocab, cls.pack_state_dict(sd, vocab), num_timesteps=num_timesteps, **kw)
 
     @staticmethod
-    def pack_state_dict(sd, vocab: Vocab) -> Dict[str, torch.Tensor]:
+    def pack_state_dict(sd, vocab: Vocab, device=None) -> Dict[str, torch.Tensor]:
+        """the reference's parameters in the LdmWeights layout, fp32, on `device` (default: the CPU).  Parameters already on
+        `device` are stacked there, with no host round trip."""
         p = _find_prefix(sd)
-        g = lambda k: sd[p + k].detach().float().cpu()
+        device = torch.device("cpu") if device is None else torch.device(device)
+        g = lambda k: sd[p + k].detach().to(device, torch.float32)
         L = 0
         while f"{p}backbone.layers.{L}.linear1.weight" in sd:
             L += 1
@@ -95,6 +99,35 @@ class Engine:
             norm1_emb=st("norm1.emb.weight"), norm1_w=st("norm1.linear.weight"), norm1_b=st("norm1.linear.bias"),
             norm2_w=st("norm2.weight"), norm2_b=st("norm2.bias"),
             head_ln_w=g("head.0.weight"), head_ln_b=g("head.0.bias"), head_w=g("head.1.weight"))
+
+    def weight_shapes(self) -> Dict[str, Tuple[int, ...]]:
+        """the shape of every LdmWeights field for this handle (include/ldm_b200.h)"""
+        C, S, d, f, L, T = self.vocab.C, self.vocab.S, self.d_model, self.d_ff, self.n_layers, self.T
+        return dict(cat_emb=(C, d), pos_table=(S, d), in_proj_w=(L, 3 * d, d), in_proj_b=(L, 3 * d), out_proj_w=(L, d, d),
+                    out_proj_b=(L, d), linear1_w=(L, f, d), linear1_b=(L, f), linear2_w=(L, d, f), linear2_b=(L, d),
+                    norm1_emb=(L, T, d), norm1_w=(L, 2 * d, d), norm1_b=(L, 2 * d), norm2_w=(L, d), norm2_b=(L, d),
+                    head_ln_w=(d,), head_ln_b=(d,), head_w=(C, d))
+
+    def load_weights(self, weights: Dict[str, torch.Tensor]):
+        """Repack new weights (the `pack_state_dict` dict, on any device) into this handle in place (ldm_load_weights), on the
+        current stream: sampling queued before sees the old weights, sampling after the new ones.  The shapes must be the
+        handle's; a captured sampling graph stays valid."""
+        want = self.weight_shapes()
+        stream = torch.cuda.current_stream(self.device)
+        w = _lib.LdmWeights()
+        keep = []
+        for name in _lib._W_FIELDS:
+            t = weights[name].detach().to(self.device, torch.float32).contiguous()
+            if tuple(t.shape) != want[name]:
+                raise ValueError(f"weight {name}: shape {tuple(t.shape)}, the handle was built for {want[name]}")
+            t.record_stream(stream)          # the packing kernels read it after this call returns
+            keep.append(t)
+            setattr(w, name, t.data_ptr())
+        _lib.check(self.lib.ldm_load_weights(self._h, C.byref(w), C.c_void_p(stream.cuda_stream)))
+
+    def load_state_dict(self, sd: Dict[str, torch.Tensor]):
+        """load_weights from a reference LayoutDM `state_dict()` (any of the key prefixes `from_state_dict` takes)"""
+        self.load_weights(self.pack_state_dict(sd, self.vocab, device=self.device))
 
     def close(self):
         if getattr(self, "_h", None):
