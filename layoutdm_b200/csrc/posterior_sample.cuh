@@ -378,26 +378,17 @@ LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, co
   embed_next(p, b, s, best_c, lane);
 }
 
-template <class Noise = TokenNoise>
-__global__ void __launch_bounds__(256) posterior_sample_kernel(const StepParams p) {
-  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (token >= p.n_layouts * p.S) return;
-  pdl_sync();
-  posterior_token_generic<Noise>(p, token, lane);
-}
-
-// Group-centric variant for the constrained (per-attribute) diffusion: outside the token's vocabulary group (plus PAD and
-// MASK) the posterior is the constant log(1e-30), so only the <= 34 classes of the group are evaluated (lane l: class
-// grp_start + l; lanes 0 / 1 additionally PAD / MASK); the float64 log-softmax still runs over all C-1 logits.
-// Preconditions (checked by the host): constrained, mode in {deterministic, random, gumbel, top_p with top_p < 1}, no log-prob
-// input / output, every group <= 32 classes.  A token whose best in-group log-probability is not far enough above
-// log(1e-30) for the out-of-group classes to be unreachable takes posterior_token_generic instead (warp-uniform), so
-// the result is the generic kernel's in every case.
-template <class Noise = TokenNoise>
-__global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepParams p) {
-  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (token >= p.n_layouts * p.S) return;
-  pdl_sync();
+// The group-centric computation of one token of the constrained (per-attribute) diffusion: outside the token's vocabulary
+// group (plus PAD and MASK) the posterior is the constant log(1e-30), so only the <= 34 classes of the group are evaluated
+// (lane l: class grp_start + l; lanes 0 / 1 additionally PAD / MASK); the float64 log-softmax still runs over all C-1 logits.
+// A token whose best in-group log-probability is not far enough above log(1e-30) for the out-of-group classes to be
+// unreachable, or whose refinement row lifts a class outside the group, is not taken: the routine returns false
+// (warp-uniform) having written nothing, and the caller runs posterior_token_generic.  Otherwise it writes the id, the
+// next step's embedding row and, with kTap and logprob_out set, the log-probabilities it drew from: the group's, and
+// log(1e-30) plus the refinement entry outside it.  Both draw kernels run it for every token group_path_applies admits, so
+// the ids do not depend on whether the log-probabilities are requested (DESIGN.md §2).
+template <class Noise, bool kTap>
+LDM_DEVINL bool posterior_token_group(const StepParams& p, const int token, const int lane) {
   const int b = token / p.S, s = token % p.S;
   const int C = p.C;
   const int x_t = static_cast<int>(p.ids_in[token]);
@@ -446,11 +437,22 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
     float tmax = 0.0f;
 #pragma unroll
     for (int j = 0; j < 5; ++j) if (lvalid[j] && !in_group(p, g, lcls[j])) tmax = fmaxf(tmax, __ldg(trow + lcls[j]));
-    if (warp_max(tmax) > 0.0f) { posterior_token_generic<Noise>(p, token, lane); return; }
+    if (warp_max(tmax) > 0.0f) return false;
   }
-  // every class outside the group sits at log(1e-30): it must be out of reach of the draw (see the header comment)
+  // every class outside the group sits at log(1e-30): it must be out of reach of the draw.  A fixed token whose id lies outside
+  // the group leaves every group class at log(1e-30) and so always goes to the all-classes routine.
   const float margin = p.mode == SAMP_DETERMINISTIC ? 0.0f : Noise::kGroupMargin * p.temperature;
-  if (!(lmax - kLogEps > margin)) { posterior_token_generic<Noise>(p, token, lane); return; }
+  if (!(lmax - kLogEps > margin)) return false;
+
+  if constexpr (kTap) {
+    if (p.logprob_out != nullptr) {
+      float* out = p.logprob_out + static_cast<size_t>(token) * C;
+#pragma unroll
+      for (int j = 0; j < 5; ++j) if (lvalid[j] && !in_group(p, g, lcls[j])) out[lcls[j]] = refine ? kLogEps + __ldg(trow + lcls[j]) : kLogEps;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) if (on[j]) out[cls[j]] = lp[j];
+    }
+  }
 
   int best_c;
   if (p.mode == SAMP_DETERMINISTIC) {
@@ -461,7 +463,7 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
     for (int j = 0; j < 2; ++j) lg[j] = on[j] ? lp[j] / p.temperature : -INFINITY;
     if (p.mode == SAMP_TOP_P) {
       // sampling.py:94-109 restricted to the group: the classes outside it carry ~1e-30 of the mass, sit at the tail of the
-      // descending order with a cumulative mass of ~1 > top_p (the host requires top_p < 1) and are dropped in any case.
+      // descending order with a cumulative mass of ~1 > top_p (group_path_applies requires top_p < 0.9999) and are dropped in any case.
       float m = warp_max(fmaxf(lg[0], lg[1]));
       float pr[2], sm = 0.0f;
 #pragma unroll
@@ -511,6 +513,39 @@ __global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepP
   }
   if (lane == 0) p.ids_out[token] = best_c;
   embed_next(p, b, s, best_c, lane);
+  return true;
+}
+
+// The steps posterior_token_group serves: ids drawn from logits (no log-prob or log p(x0) input, no log p(x0) tap, one posterior
+// timestep for the batch), the constrained diffusion, mode in {deterministic, random, gumbel, top_p with top_p < 0.9999}, every
+// group <= 32 classes.  Kernel parameters only: the same answer for every token of a launch.
+__host__ __device__ inline bool group_path_applies(const StepParams& p) {
+  bool ok = p.constrained && p.ids_out != nullptr && p.logprob_in == nullptr && p.lx0_in == nullptr && p.lx0_out == nullptr &&
+            p.t_layout == nullptr &&
+            (p.mode == SAMP_DETERMINISTIC || p.mode == SAMP_RANDOM || p.mode == SAMP_GUMBEL || (p.mode == SAMP_TOP_P && p.top_p < 0.9999f));
+  for (int g = 0; g < p.n_attr; ++g) ok = ok && p.grp_n[g] <= 32;
+  return ok;
+}
+
+// All-classes kernel: any q_type, any sampling mode, log-prob in / out.  A token of a step group_path_applies admits takes
+// posterior_token_group first, exactly as in posterior_sample_group_kernel, and fills the log-prob tap from it.
+template <class Noise = TokenNoise>
+__global__ void __launch_bounds__(256) posterior_sample_kernel(const StepParams p) {
+  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (token >= p.n_layouts * p.S) return;
+  pdl_sync();
+  if (group_path_applies(p) && posterior_token_group<Noise, true>(p, token, lane)) return;
+  posterior_token_generic<Noise>(p, token, lane);
+}
+
+// Group-centric kernel: posterior_token_group for every token, posterior_token_generic for the ones it does not take.  Launched
+// where group_kernel_applies; its ids are the all-classes kernel's in every case, bit for bit.
+template <class Noise = TokenNoise>
+__global__ void __launch_bounds__(256) posterior_sample_group_kernel(const StepParams p) {
+  const int token = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (token >= p.n_layouts * p.S) return;
+  pdl_sync();
+  if (!posterior_token_group<Noise, false>(p, token, lane)) posterior_token_generic<Noise>(p, token, lane);
 }
 
 // test tap of the torch-generator contract: out[i] = element i of one exponential_ (which = 1) or rand (which = 0) draw of
@@ -520,13 +555,8 @@ __global__ void torch_noise_tap_kernel(const TorchNoise nz, const uint32_t n, co
     out[i] = which ? TorchNoise::exponential(nz.word(i)) : TorchNoise::rand(nz.word(i));
 }
 
-// the preconditions of posterior_sample_group_kernel (its header comment)
-inline bool group_kernel_applies(const StepParams& p) {
-  bool ok = p.constrained && p.logprob_in == nullptr && p.logprob_out == nullptr &&
-            (p.mode == SAMP_DETERMINISTIC || p.mode == SAMP_RANDOM || p.mode == SAMP_GUMBEL || (p.mode == SAMP_TOP_P && p.top_p < 0.9999f));
-  for (int g = 0; g < p.n_attr; ++g) ok = ok && p.grp_n[g] <= 32;
-  return ok;
-}
+// where posterior_sample_group_kernel may replace the all-classes kernel: no log-prob tap to fill
+inline bool group_kernel_applies(const StepParams& p) { return group_path_applies(p) && p.logprob_out == nullptr; }
 
 // ---------------------------------------------------------------------------------------------------------
 // Training-side terms of the variational bound, per token: what `forward` computes after x_t has been drawn

@@ -146,7 +146,9 @@ class Serial:
     pad: Dict[int, torch.Tensor] = field(default_factory=dict)
 
 
-def serialized(monkeypatch, wl: Workload, dtype: str, seed: int, b_global0: int, cond, ids_init, keep=(), plan=None, B=None) -> Serial:
+def serialized(monkeypatch, wl: Workload, dtype: str, seed: int, b_global0: int, cond, ids_init, keep=(), plan=None, B=None,
+               want_logprob: bool = False) -> Serial:
+    """want_logprob: every step also fills the log-prob tap, so its draw runs in the all-classes kernel"""
     plan = wl.plan if plan is None else plan
     B = wl.B if B is None else B
     v = wl.vocab
@@ -159,7 +161,8 @@ def serialized(monkeypatch, wl: Workload, dtype: str, seed: int, b_global0: int,
         else:
             x = torch.full((B, v.S), v.mask_id, dtype=torch.int64, device="cuda")
         for i, (tm, tp) in enumerate(plan):
-            x, lg, _ = eng.step(x, tm, tp, wl.sampling, cond, seed=seed, step_ctr=i, b_global0=b_global0, want_logits=i in keep)
+            x, lg, _ = eng.step(x, tm, tp, wl.sampling, cond, seed=seed, step_ctr=i, b_global0=b_global0, want_logits=i in keep,
+                                want_logprob=want_logprob)
             out.ids.append(x.to(torch.int16).cpu())
             if i in keep:
                 out.logits[i] = lg.cpu()
@@ -237,6 +240,18 @@ def test_loop_equals_serialized_steps_under_every_switch(monkeypatch, name, dtyp
     ks = prefixes(len(wl.plan))
     ref = serialized(monkeypatch, wl, dtype, wl.seed, wl.b_global0, cond, ids_init, keep=[k - 1 for k in ks])
     failures = compare_prefixes(monkeypatch, wl, dtype, MATRIX, ks, ref, cond, ids_init)
+    # the serialized steps with the log-prob tap (the all-classes draw kernel, which the oracle tests read log-probs from)
+    tap = serialized(monkeypatch, wl, dtype, wl.seed, wl.b_global0, cond, ids_init, keep=[k - 1 for k in ks], want_logprob=True)
+    for step, (a, b) in enumerate(zip(tap.ids, ref.ids)):
+        d = first_diff(a, b)
+        if d is not None:
+            failures.append(f"serialized steps with the log-prob tap: ids differ at step {step}, first at (layout, token) {d}, "
+                            f"{int((a != b).sum())} tokens")
+            break
+    for step in ref.logits:
+        if first_diff(tap.logits[step], ref.logits[step]) is not None:
+            failures.append(f"serialized steps with the log-prob tap: logits differ at step {step}")
+    print(f"  {'log-prob tap':18s} {'-':9s} {'ok' if not any('log-prob tap' in f for f in failures) else 'FAIL':5s}")
     assert not failures, "\n".join(failures)
 
 
