@@ -109,6 +109,8 @@ LDM_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32
 
 // named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
 LDM_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// counts the calling warp's threads toward the barrier without waiting for it
+LDM_DEVINL void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------
 // wgmma (Hopper warpgroup MMA): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp32 accumulators in registers.

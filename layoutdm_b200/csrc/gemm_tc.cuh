@@ -4,22 +4,21 @@
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
 //   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; 16-bit outputs are written as (hi, lo) pairs (out, out_lo)
 //
-// Both kernels run one operand ring (Ring): a shared-memory ring of k-block stages that one producer lane fills with TMA 2-D
+// Every kernel runs one operand ring (Ring): a shared-memory ring of k-block stages that one producer lane fills with TMA 2-D
 // boxes and two consumer warpgroups drain with m64 x N x k16 wgmmas into fp32 register accumulators (full / empty mbarriers).
-// CTA b runs tiles b, b + gridDim.x, ..., the column tile fastest (consecutive tiles share their A row block in L2); the ring
-// slot and phase run on from tile to tile, so the producer fills the ring with the next tile during this tile's epilogue.  A
-// split-mode stage holds both planes of a 32-element k-block, A_hi | A_lo | W_hi | W_lo: the bytes (and so the stage counts) of
-// the one-plane 64-element stage.  Each of its k16 steps is three wgmmas: a_lo w_hi, a_hi w_lo, a_hi w_hi.
+// In the persistent kernels the ring slot and phase run on from tile to tile, so the producer fills the ring with the next
+// tile during this tile's epilogue.  A split-mode stage holds both planes of a 32-element k-block, A_hi | A_lo | W_hi | W_lo:
+// the bytes (and so the stage counts) of the one-plane 64-element stage.  Each of its k16 steps is three wgmmas: a_lo w_hi,
+// a_hi w_lo, a_hi w_hi.
 //
 // gemm_tc_kernel adds the epilogue on the consumers' own accumulator fragment.  Tile shapes:
-//   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (QKV, FF1: 256 columns; vocabulary head: 160)
+//   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (split-mode QKV, FF1: 256 columns; vocabulary head: 160)
 //   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the LN epilogue: 2 x 232 = 464 =
 //              d_model, so a CTA holds whole rows and the LayerNorm row statistics are combined in shared memory.
 // Epilogues:  QKV (bias, q-scale, 16-bit) | RELU (FF1: bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
 //             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused).
-// The 16-bit QKV / FF1 epilogues of the one-plane modes write the fragment into a staging tile that one thread per warpgroup
-// stores with TMA while the consumers go on to the next tile (kStagedStore); the others store from the fragment.
-// gemm_ln_kernel (out-projection, FF2 in fp16 / bf16) adds a tile buffer and epilogue warps of its own (see there).
+// It stores from the fragment.  gemm_rowblock_kernel (QKV, FF1 in fp16 / bf16) keeps each layout's A rows resident and stores
+// through staging buffers with TMA (see there).  gemm_ln_kernel (out-projection, FF2 in fp16 / bf16) adds a tile buffer and epilogue warps of its own (see there).
 //
 // Reference ops replaced: nn.Linear / nn.MultiheadAttention projections / nn.LayerNorm / AdaLayerNorm in
 // T/models/transformer_utils.py:79-83,165-210 and T/models/common/nn_lib.py:187-189,235.
@@ -58,6 +57,7 @@ struct GemmParams {
   int rev;                // 1: walk the row blocks from the last to the first.  Consecutive kernels alternate the direction, so a consumer starts
                           // with the rows its producer wrote last -- the part of the intermediate that is still in L2
   void* out_lo;           // split mode: lo plane of the 16-bit output (same layout as out)
+  int n_ranges;           // gemm_rowblock_kernel: column ranges each row block is cut into (work items = row blocks x n_ranges)
 };
 
 template <bool BF16, int N>
@@ -68,11 +68,14 @@ LDM_DEVINL void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t a
   else { static_assert(N == 128, "unsupported wgmma width"); wgmma_ss_n128<BF16>(d, da, db, accumulate); }
 }
 
+struct NoKbHook { LDM_DEVINL void operator()(int) const {} };
+
 // The operand ring: STAGES stages, each [A rows][KB] per plane | [B_ROWS weight rows][KB] per plane and column warpgroup.
 // One smem row is one swizzle row of 2 KB bytes: the operand maps' boxes are KB columns with the (2 KB)-byte swizzle, read by
 // make_smem_desc<2 KB>.  K_TAIL: K may end in a partial k-block (K % KB is 0 or 16: K = 464, 512, 1856); a k-block that runs
-// past K issues a single k16 step.  Each role keeps its own cursor (slot s, pass phase) and passes it in.
-template <int KB, int PLANES, int A_ROWS, int B_ROWS, int WG_N, int STAGES, bool K_TAIL = true>
+// past K issues a single k16 step.  Each role keeps its own cursor (slot s, pass phase) and passes it in.  A_ROWS = 0: the
+// stages hold weights only (the row-block GEMM keeps its A rows outside the ring).  CONSUMERS: the threads that release a stage.
+template <int KB, int PLANES, int A_ROWS, int B_ROWS, int WG_N, int STAGES, bool K_TAIL = true, int CONSUMERS = kGemmConsumers>
 struct Ring {
   static constexpr int kKB = KB, kStages = STAGES, kWgN = WG_N;
   static constexpr int kRowBytes = 2 * KB;
@@ -97,24 +100,27 @@ struct Ring {
     if constexpr (kOpSplit<MODE>) { tma_prefetch_desc(&a.lo); tma_prefetch_desc(&b.lo); }
   }
   LDM_DEVINL void init() const {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kGemmConsumers); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMERS); }
   }
   static LDM_DEVINL void advance(int& s, uint32_t& phase) { if (++s == STAGES) { s = 0; phase ^= 1; } }
   LDM_DEVINL void release_prev(int s) const { mbar_arrive(&empty[s == 0 ? STAGES - 1 : s - 1]); }
 
-  // producer lane: the num_kb k-blocks of one tile, A rows m0.., weight block wn's rows n0 + wn * B_ROWS..
-  template <int MODE>
-  LDM_DEVINL void load_tile(int& s, uint32_t& phase, const OpMaps<MODE>& a, const OpMaps<MODE>& b, int num_kb, int m0, int n0) const {
+  // producer lane: the num_kb k-blocks of one tile, A rows m0.., weight block wn's rows n0 + wn * B_ROWS..; on_kb(kb) runs
+  // before k-block kb's stage is claimed
+  template <int MODE, class OnKb = NoKbHook>
+  LDM_DEVINL void load_tile(int& s, uint32_t& phase, const OpMaps<MODE>& a, const OpMaps<MODE>& b, int num_kb, int m0, int n0,
+                            OnKb on_kb = {}) const {
     static_assert(PLANES == (kOpSplit<MODE> ? 2 : 1), "one operand map per plane");
     for (int kb = 0; kb < num_kb; ++kb) {
+      on_kb(kb);
       mbar_wait(&empty[s], phase ^ 1);
       uint8_t* st = stages + s * kStageBytes;
       mbar_arrive_expect_tx(&full[s], kStageBytes);              // out-of-bounds box parts are zero-filled and still counted
-      tma_load_2d(st, &a.hi, &full[s], kb * KB, m0);
+      if constexpr (A_ROWS > 0) tma_load_2d(st, &a.hi, &full[s], kb * KB, m0);
 #pragma unroll
       for (int wn = 0; wn < WG_N; ++wn) tma_load_2d(st + kABytes + wn * kBBytes, &b.hi, &full[s], kb * KB, n0 + wn * B_ROWS);
+      if constexpr (PLANES == 2 && A_ROWS > 0) tma_load_2d(st + kAPlane, &a.lo, &full[s], kb * KB, m0);
       if constexpr (PLANES == 2) {
-        tma_load_2d(st + kAPlane, &a.lo, &full[s], kb * KB, m0);
 #pragma unroll
         for (int wn = 0; wn < WG_N; ++wn)
           tma_load_2d(st + kABytes + (WG_N + wn) * kBBytes, &b.lo, &full[s], kb * KB, n0 + wn * B_ROWS);
@@ -164,25 +170,14 @@ struct Ring {
   }
 };
 
-// TMA-staged stores: the 16-bit plain epilogues of the one-plane modes (the split mode's (hi, lo) pair outputs would need two
-// staging tiles, which leave too few ring stages).  These GEMMs are the persistent ones: 384 threads (producer warpgroup),
-// min(tiles, SMs) CTAs.  The others store from the fragment, have nothing to overlap their epilogue with, and run one tile per
-// CTA with 288 threads (one producer warp)
-template <int EPI, bool SPLIT>
-constexpr bool kStagedStore = (EPI == EPI_QKV || EPI == EPI_RELU) && !SPLIT;
-template <int EPI, int MODE>
-constexpr int kGemmThreads = kStagedStore<EPI, kOpSplit<MODE>> ? 384 : 288;
+// gemm_tc_kernel stores from the fragment and has nothing to overlap its epilogue with: one tile per CTA, 288 threads (one
+// producer warp)
+constexpr int kGemmThreads = 288;
 
-template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false, bool STAGED = false>
+template <int BN_WG, int WG_M, int STAGES, bool SPLIT = false>
 struct GemmSmem {
   using R = Ring<gemm_kb(SPLIT), SPLIT ? 2 : 1, 64 * WG_M, BN_WG, 3 - WG_M, STAGES>;
-  // staging tile of a 16-bit output tile: [column block of 64][row][128 B] with the 128-byte swizzle, so warpgroup wm's rows of
-  // column block cb are one TMA store box (64 columns x 64 rows) at cb * kStoreCb + wm * 8 KB
-  static constexpr int kStoreCb = 64 * WG_M * 128;
-  static constexpr int kStoreBytes = STAGED ? (R::kWgN * BN_WG / 64) * kStoreCb : 0;
-  static_assert(!STAGED || BN_WG % 64 == 0, "staged stores go out in 64-column boxes");
-  static constexpr int kOffStore = R::kBytes;
-  static constexpr int kOffBars = kOffStore + kStoreBytes;
+  static constexpr int kOffBars = R::kBytes;
   static constexpr int kOffStat = kOffBars + 256;                // LN: per-row sum, then sum of squared deviations, of each warpgroup's columns
   static constexpr int kBytes = kOffStat + 2 * 64 * 16 + 1024 /*align slack*/;
   static_assert(2 * STAGES * 8 <= 256, "barrier block overflow");
@@ -213,15 +208,13 @@ LDM_DEVINL LnAffine ln_affine(const float* scale, const float* shift, int adaln,
   return a;
 }
 
-// grid: staged (persistent): up to tiles = n_tiles * M / (64 WG_M) CTAs, otherwise exactly one CTA per tile; map_out: the TMA
-// store map of a staged epilogue (box 64 x 64 rows)
+// grid: one CTA per tile, tiles = n_tiles * M / (64 WG_M)
 template <int BN_WG, int WG_M, int STAGES, int EPI, int MODE>
-__global__ void __launch_bounds__(kGemmThreads<EPI, MODE>, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M rows*/,
-               const __grid_constant__ OpMaps<MODE> map_b /*box KB x BN_WG rows*/,
-               const __grid_constant__ CUtensorMap map_out, const GemmParams p) {
-  constexpr bool SPLIT = kOpSplit<MODE>, STAGED = kStagedStore<EPI, SPLIT>;
-  using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT, STAGED>;
+               const __grid_constant__ OpMaps<MODE> map_b /*box KB x BN_WG rows*/, const GemmParams p) {
+  constexpr bool SPLIT = kOpSplit<MODE>;
+  using SM = GemmSmem<BN_WG, WG_M, STAGES, SPLIT>;
   using O = OpT<MODE>;
   constexpr int kBMt = 64 * WG_M, kAcc = BN_WG / 2;
   static_assert(EPI != EPI_LN || (WG_M == 1 && BN_WG == 232), "LN epilogue is laid out for 464 = 2 x 232 columns");
@@ -233,15 +226,211 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M row
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int num_kb = SM::R::num_kb(p.K);
-  const int n_mblk = p.M / kBMt, n_work = n_mblk * p.n_tiles;
-  // tile t: row block t / n_tiles (walked from the last one down when rev), column tile t % n_tiles
-  const auto tile_m0 = [&](int t) { const int mb = t / p.n_tiles; return (p.rev ? n_mblk - 1 - mb : mb) * kBMt; };
-  const auto tile_n0 = [&](int t) { return (t % p.n_tiles) * BN_WG * SM::R::kWgN; };
+  const int n_mblk = p.M / kBMt;
+  // tile blockIdx.x: row block blockIdx.x / n_tiles (walked from the last one down when rev), column tile blockIdx.x % n_tiles
+  const int mb = blockIdx.x / p.n_tiles;
+  const int m0 = (p.rev ? n_mblk - 1 - mb : mb) * kBMt, n0 = (blockIdx.x % p.n_tiles) * BN_WG * SM::R::kWgN;
 
   if (threadIdx.x == kGemmConsumers) {
     ring.prefetch(map_a, map_b);
-    if constexpr (STAGED) tma_prefetch_desc(&map_out);
     ring.init();
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();                                                // everything above overlapped the previous kernel's tail
+
+  int s = 0;
+  uint32_t phase = 0;
+  if (warp >= kGemmConsumers / 32) {
+    // ===================== TMA producer =====================
+    if (threadIdx.x == kGemmConsumers) ring.load_tile(s, phase, map_a, map_b, num_kb, m0, n0);
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int wm = WG_M == 2 ? wg : 0, wn = WG_M == 2 ? 0 : wg;
+  float acc[kAcc];
+#pragma unroll
+  for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
+  ring.template mma_tile<MODE>(s, phase, acc, wm, wn, num_kb, p.K);
+
+  const int rw = (warp & 3) * 16 + (lane >> 2);           // fragment rows rw and rw + 8 of the warpgroup's 64
+  const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
+  const int col0 = n0 + wn * BN_WG + 2 * (lane & 3);        // + 8 j: columns col, col + 1 of n8 block j
+
+  if constexpr (EPI != EPI_LN) {
+    float scale = 1.0f;
+    if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
+      float v[4];
+      bias_act<EPI>(acc, j, p.bias, c, scale, v);
+      if constexpr (EPI == EPI_F32) {
+        float* o = static_cast<float*>(p.out);
+        *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
+        *reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * p.ldo + c) = make_float2(v[2], v[3]);
+      } else {
+        uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
+        uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
+        if constexpr (SPLIT) {
+          uint32_t* l0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row0) * p.ldo + c);
+          uint32_t* l1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row1) * p.ldo + c);
+          O::pack_pair(v[0], v[1], *o0, *l0);
+          O::pack_pair(v[2], v[3], *o1, *l1);
+        } else {
+          *o0 = O::pack(v[0], v[1]);
+          *o1 = O::pack(v[2], v[3]);
+        }
+      }
+    }
+  } else {
+    // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
+    //   y = acc + bias + resid (-> y_out); two-pass row statistics: the row sum over the thread's columns, the quad of lanes
+    //   that shares a row, then the other warpgroup (other 232 columns) through shared memory gives the mean; the sum of
+    //   (y - mean)^2 is reduced the same way.  One pass, E[y^2] - mean^2, loses the variance to cancellation once
+    //   |mean| / std is large.  The sums run over y - pivot, pivot = bias[0] + resid[row][0] (y's column 0 without the GEMM
+    //   term, the same in all 8 threads of a row): their terms are of the row's spread, not of its mean, so the mean of a row
+    //   far from zero comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the
+    //   mean, which every output of the row inherits).  Normalise, 16-bit (+ fp32) outputs.
+    float* ssum = reinterpret_cast<float*>(smem + SM::kOffStat);   // [warpgroup][64 rows] row sums of y - pivot
+    float* ssq = ssum + 2 * 64;                                     // [warpgroup][64 rows] sums of squared deviations
+    const int N = p.N;
+    const float* r0p = p.resid + static_cast<size_t>(row0) * N;
+    const float* r1p = p.resid + static_cast<size_t>(row1) * N;
+    const float piv0 = __ldg(p.bias) + r0p[0], piv1 = __ldg(p.bias) + r1p[0];
+    float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+      const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
+      acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
+      acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
+      if (p.y_out != nullptr) {
+        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      acc[4 * j] -= piv0; acc[4 * j + 1] -= piv0; acc[4 * j + 2] -= piv1; acc[4 * j + 3] -= piv1;   // from here on: y - pivot
+      s0 += acc[4 * j] + acc[4 * j + 1];
+      s1 += acc[4 * j + 2] + acc[4 * j + 3];
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    }
+    if ((lane & 3) == 0) { ssum[wn * 64 + rw] = s0; ssum[wn * 64 + rw + 8] = s1; }
+    named_bar_sync(1, kGemmConsumers);
+    const float inv_n = 1.0f / static_cast<float>(N);
+    const float mean0 = (s0 + ssum[(wn ^ 1) * 64 + rw]) * inv_n, mean1 = (s1 + ssum[(wn ^ 1) * 64 + rw + 8]) * inv_n;   // mean - pivot, like acc
+    float q0 = 0.0f, q1 = 0.0f;
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const float d0 = acc[4 * j] - mean0, d1 = acc[4 * j + 1] - mean0, d2 = acc[4 * j + 2] - mean1, d3 = acc[4 * j + 3] - mean1;
+      q0 = fmaf(d0, d0, fmaf(d1, d1, q0));
+      q1 = fmaf(d2, d2, fmaf(d3, d3, q1));
+    }
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+      q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+    }
+    if ((lane & 3) == 0) { ssq[wn * 64 + rw] = q0; ssq[wn * 64 + rw + 8] = q1; }
+    named_bar_sync(1, kGemmConsumers);
+    const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
+    const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
+    const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
+    typename O::T* out16 = static_cast<typename O::T*>(p.out);
+#pragma unroll
+    for (int j = 0; j < BN_WG / 8; ++j) {
+      const int c = col0 + 8 * j;
+      const float2 g = __ldg(reinterpret_cast<const float2*>(a.gam + c)), h = __ldg(reinterpret_cast<const float2*>(a.bet + c));
+      const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + a.gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + a.gadd) + h.y;
+      const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + a.gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + a.gadd) + h.y;
+      if constexpr (SPLIT) {
+        typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
+        O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
+        O::pack_pair(v2, v3, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row1) * N + c));
+      } else {
+        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
+        *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
+      }
+      if (p.out32 != nullptr) {
+        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
+        *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);
+      }
+    }
+  }
+}
+
+// ============ row-block GEMM: QKV and FF1 in the one-plane modes ============
+// K = d = 464 is small enough for a layout's whole A row block (128 x 464, 119 KB) to stay in shared memory, so a CTA loads it
+// once per work item and streams only the weights.  Work item = one 128-row block and a contiguous range of its 128-column
+// tiles (n_ranges ranges per row block); min(items, SMs) CTAs of 384 threads, CTA b runs items b, b + gridDim.x, ...
+//   warpgroup 2 : producer, one lane issues the TMA loads.  An item's A k-block kb is loaded just before the k-block kb of the
+//                 item's first tile, as soon as both consumer warpgroups have released it (a_empty[kb]: their MMAs of the
+//                 previous item reading it have retired), so the next item's first tile waits k-block by k-block.
+//   warpgroups 0, 1 : consumers, ping-pong: the CTA's tiles are numbered in order across its items and warpgroup w takes the
+//                 tiles q with q % 2 == w, each a whole 128 x 128 tile (two m64n128k16 wgmmas per k16 step, 128 fp32
+//                 accumulators).  The weight ring serialises their mainloops; a named barrier hands the ring from one to the
+//                 other once it has seen its tile's last stage arrive, so a warpgroup's ring waits never run a pass ahead of
+//                 the slot's phase.  Each runs its epilogue (bias, q-scale | ReLU, 16-bit, through its own staging buffer, one
+//                 TMA store per 64 columns) under the other's MMAs.
+// Resident A: 8 k-blocks of 64 elements with the 128-byte swizzle, the 8th holding K's 16-column tail (the rest zero-filled by
+// TMA; one k16 step, Ring's K_TAIL rule).  Every output element is bias + the same k16 steps in the same order as in gemm_tc_kernel.
+constexpr int kRbThreads = 384;
+struct RbSmem {
+  static constexpr int kKB = 64, kCols = 128, kAKb = 8;            // k-block, tile columns, resident A k-blocks (K <= 512)
+  // weights only, one warpgroup consumes a stage: 4 stages of 16 KB.  64-element (128-byte) box rows: with 32-element ones the
+  // TMA loads ran well below the L2 rate
+  using R = Ring<kKB, 1, 0, kCols, 1, 4, true, 128>;
+  static constexpr int kAKbBytes = kBM * 2 * kKB;                  // 16 KB
+  static constexpr int kOffRing = kAKb * kAKbBytes;                // 128 KB of A
+  // staging buffer of a warpgroup: one 64-column block of its tile, [row][128 B] with the 128-byte swizzle = one TMA store box
+  // (64 columns x 128 rows); the tile's two blocks go through it in turn
+  static constexpr int kStoreBytes = kBM * 128;                    // 16 KB
+  static constexpr int kOffStore = kOffRing + R::kBytes;
+  static constexpr int kOffBars = kOffStore + 2 * kStoreBytes;     // ring full[4], empty[4]; a_full[8], a_empty[8]
+  static constexpr int kBytes = kOffBars + (2 * R::kStages + 2 * kAKb) * 8 + 1024 /*align slack*/;
+  static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
+};
+
+template <int EPI, int MODE>
+__global__ void __launch_bounds__(kRbThreads, 1)
+gemm_rowblock_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 128 rows*/,
+                     const __grid_constant__ CUtensorMap map_out /*box 64 x 128 rows*/, const GemmParams p) {
+  static_assert(EPI == EPI_QKV || EPI == EPI_RELU, "16-bit plain epilogues only");
+  static_assert(!kOpSplit<MODE>, "the split mode runs gemm_tc_kernel");
+  using SM = RbSmem;
+  using R = SM::R;
+  using O = OpT<MODE>;
+  constexpr int kKB = SM::kKB, kCols = SM::kCols;
+
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
+  R ring(smem + SM::kOffRing, bars);
+  uint64_t* a_full = bars + 2 * R::kStages;                      // A k-block kb of the current item has landed
+  uint64_t* a_empty = a_full + SM::kAKb;                          // both warpgroups are done reading A k-block kb
+
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+  const int num_kb = R::num_kb(p.K);                              // <= kAKb (checked at create)
+  const int n_mblk = p.M / kBM, n_items = n_mblk * p.n_ranges;
+  // item w: row block w / n_ranges (walked from the last one down when rev), tiles [j0, j1) of range w % n_ranges
+  const auto item = [&](int w, int& m0, int& j0, int& j1) {
+    const int mb = w / p.n_ranges, r = w - mb * p.n_ranges;
+    m0 = (p.rev ? n_mblk - 1 - mb : mb) * kBM;
+    j0 = r * p.n_tiles / p.n_ranges; j1 = (r + 1) * p.n_tiles / p.n_ranges;
+  };
+
+  if (threadIdx.x == kGemmConsumers) {
+    R::prefetch(map_a, map_b);
+    tma_prefetch_desc(&map_out);
+    ring.init();
+    for (int kb = 0; kb < SM::kAKb; ++kb) { mbar_init(&a_full[kb], 1); mbar_init(&a_empty[kb], kGemmConsumers); }
     fence_mbar_init();
   }
   __syncthreads();
@@ -249,175 +438,131 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M row
 
   if (warp >= kGemmConsumers / 32) {
     // ===================== TMA producer =====================
-    if constexpr (STAGED) setmaxnreg_dec<kProducerRegs>();
+    setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == kGemmConsumers) {
       int s = 0;
-      uint32_t phase = 0;                                    // ring slot and pass, carried from tile to tile
-      for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-        ring.load_tile(s, phase, map_a, map_b, num_kb, tile_m0(t), tile_n0(t));
-        if constexpr (!STAGED) break;                        // one tile per CTA
+      uint32_t phase = 0, ip = 0;                            // ring slot and pass; parity of the CTA's item count
+      for (int w = blockIdx.x; w < n_items; w += gridDim.x, ip ^= 1) {
+        int m0, j0, j1;
+        item(w, m0, j0, j1);
+        for (int j = j0; j < j1; ++j) {
+          const auto load_a = [&](int kb) {                  // the item's A k-block kb, ahead of its first tile's k-block kb
+            if (j != j0) return;
+            mbar_wait(&a_empty[kb], ip ^ 1);
+            mbar_arrive_expect_tx(&a_full[kb], SM::kAKbBytes);   // the tail k-block's zero-filled columns are counted too
+            tma_load_2d(smem + kb * SM::kAKbBytes, &map_a.hi, &a_full[kb], kb * kKB, m0);
+          };
+          ring.load_tile(s, phase, map_b, map_b, num_kb, 0, j * kCols, load_a);
+        }
       }
     }
     return;
   }
 
   // ===================== consumer warpgroups =====================
-  if constexpr (STAGED) setmaxnreg_inc<kConsumerRegs>();
+  setmaxnreg_inc<kConsumerRegs>();
   const int wg = warp >> 2;
-  const int wm = WG_M == 2 ? wg : 0, wn = WG_M == 2 ? 0 : wg;
-  float acc[kAcc];
-#pragma unroll
-  for (int i = 0; i < kAcc; ++i) acc[i] = 0.0f;
-  int s = 0;
-  uint32_t phase = 0;
-  for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-    const int m0 = tile_m0(t), n0 = tile_n0(t);
-    ring.template mma_tile<MODE>(s, phase, acc, wm, wn, num_kb, p.K);
+  const bool leader = (threadIdx.x & 127) == 0;
+  // ring hand-over: warpgroup wg waits on barrier 4 + wg before its tile's mainloop, the other arrives on it after its own
+  // (compile-time ids; 2, 3 are the warpgroups' epilogue barriers)
+  const auto wait_turn = [&]() { if (wg == 0) named_bar_sync(4, kGemmConsumers); else named_bar_sync(5, kGemmConsumers); };
+  const auto pass_turn = [&]() { if (wg == 0) named_bar_arrive(5, kGemmConsumers); else named_bar_arrive(4, kGemmConsumers); };
+  const auto wg_bar = [&]() { if (wg == 0) named_bar_sync(2, 128); else named_bar_sync(3, 128); };
+  int n_cta_tiles = 0;
+  for (int w = blockIdx.x; w < n_items; w += gridDim.x) { int m0, j0, j1; item(w, m0, j0, j1); n_cta_tiles += j1 - j0; }
 
-    const int rw = (warp & 3) * 16 + (lane >> 2);           // fragment rows rw and rw + 8 of the warpgroup's 64
-    const int row0 = m0 + wm * 64 + rw, row1 = row0 + 8;
-    const int col0 = n0 + wn * BN_WG + 2 * (lane & 3);        // + 8 j: columns col, col + 1 of n8 block j
+  float acc[2][kCols / 2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < kCols / 2; ++i) acc[h][i] = 0.0f;
+  const uint32_t a_base = smem_u32(smem);
+  uint8_t* stage = smem + SM::kOffStore + wg * SM::kStoreBytes;
+  const uint32_t stage_u32 = smem_u32(stage);                  // 32-bit shared addresses: 64-bit generic ones cost registers
+  const int rw = (warp & 3) * 16 + (lane >> 2);                 // fragment rows rw, rw + 8 of each 64-row half
+  const int sw = (rw & 7) << 4;                                 // 128-byte swizzle: 16-byte chunk ^= row % 8 (the same for all four rows)
+  int s = 0, q = 0;                                             // ring cursor; the CTA's tile count so far
+  uint32_t phase = 0, ip = 0;
+  for (int w = blockIdx.x; w < n_items; w += gridDim.x, ip ^= 1) {
+    int m0, j0, j1;
+    item(w, m0, j0, j1);
+    bool mine_any = false;
+    for (int j = j0; j < j1; ++j, ++q) {
+      if ((q & 1) != wg) {                                      // the other warpgroup's tile: its stages pass by
+        for (int kb = 0; kb < num_kb; ++kb) R::advance(s, phase);
+        continue;
+      }
+      mine_any = true;
+      const bool last_mine = j + 2 >= j1;                        // this warpgroup's last read of the item's A rows
+      const int n0 = j * kCols;
+      if (q > 0) wait_turn();
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&a_full[kb], ip);
+        mbar_wait(&ring.full[s], phase);
+        const uint64_t da = make_smem_desc<2 * kKB>(a_base + kb * SM::kAKbBytes);
+        const uint64_t db = make_smem_desc<2 * kKB>(smem_u32(ring.stages + s * R::kStageBytes));
+        wgmma_fence();
+        // k16 step k: +32 B (>>4 = 2); rows 64.. of A are 64 rows x 128 B = 8 KB (>>4 = 512) on
+        const auto step = [&](int k) {
+          wgmma_ss<kOpBf16<MODE>, kCols>(acc[0], da + 2 * k, db + 2 * k, (kb | k) != 0);
+          wgmma_ss<kOpBf16<MODE>, kCols>(acc[1], da + 512 + 2 * k, db + 2 * k, (kb | k) != 0);
+        };
+        const bool whole = kb * kKB + kKB <= p.K;
+        if (!whole) step(0);
+        if (whole) {
+#pragma unroll
+          for (int k = 0; k < kKB / kWgK; ++k) step(k);
+        }
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();
+          ring.release_prev(s);
+          if (last_mine) mbar_arrive(&a_empty[kb - 1]);
+        }
+        R::advance(s, phase);
+      }
+      if (q + 1 < n_cta_tiles) pass_turn();
+      wgmma_wait<0>();
+      fence_acc(acc[0]);
+      fence_acc(acc[1]);
+      ring.release_prev(s);
+      if (last_mine) mbar_arrive(&a_empty[num_kb - 1]);
 
-    if constexpr (STAGED) {
-      // bias (q-scale | ReLU), 16-bit, into the staging tile; then one thread of the warpgroup stores its 64 rows with TMA
+      // epilogue: bias (q-scale | ReLU), 16-bit, one 64-column block at a time into the staging buffer, which the leader then
+      // stores with TMA.  N is a multiple of 64 (checked at create): a block past N (FF1's last tile) is not computed
       float scale = 1.0f;
-      if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
-      const bool leader = (threadIdx.x & 127) == 0;
-      uint8_t* stage = smem + SM::kOffStore + wm * 64 * 128;
-      const uint32_t stage_u32 = smem_u32(stage);            // 32-bit shared addresses: 64-bit generic ones cost registers per column block
-      // one named barrier per warpgroup, with a compile-time id
-      const auto wg_bar = [&]() { if (wg == 0) named_bar_sync(2, 128); else named_bar_sync(3, 128); };
-      if (leader) bulk_wait_group_read<0>();                   // the previous tile's store has read the staging tile
-      wg_bar();
-      const int sw = (rw & 7) << 4;                            // 128-byte swizzle: 16-byte chunk ^= row % 8 (rw + 8: the same)
+      if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 128 == 0)
+      const int col0 = n0 + 2 * (lane & 3);                      // + 8 j: columns c, c + 1 of n8 block j
 #pragma unroll
-      for (int j = 0; j < BN_WG / 8; ++j) {
-        const int c = col0 + 8 * j;
-        if (c >= p.N) continue;                               // columns past N: the TMA store clips them
-        float v[4];
-        bias_act<EPI>(acc, j, p.bias, c, scale, v);
-        const uint32_t blk = stage_u32 + (j >> 3) * SM::kStoreCb + ((((j & 7) << 4) ^ sw) | (4 * (lane & 3)));
-        st_shared_u32(blk + rw * 128, O::pack(v[0], v[1]));
-        st_shared_u32(blk + (rw + 8) * 128, O::pack(v[2], v[3]));
-      }
-      fence_proxy_async_smem();
-      wg_bar();
-      if (leader) {
+      for (int cb = 0; cb < kCols / 64; ++cb) {
+        if (n0 + cb * 64 >= p.N) continue;
+        if (leader) bulk_wait_group_read<0>();                 // the previous store has read the staging buffer
+        wg_bar();
 #pragma unroll
-        for (int cb = 0; cb < BN_WG / 64; ++cb)
-          if (n0 + cb * 64 < p.N) tma_store_2d(&map_out, stage + cb * SM::kStoreCb, n0 + cb * 64, m0 + wm * 64);
-        bulk_commit_group();
-      }
-    } else if constexpr (EPI != EPI_LN) {
-      float scale = 1.0f;
-      if constexpr (EPI == EPI_QKV) scale = (n0 < p.qcols) ? p.qscale : 1.0f;   // Q tiles are whole tiles (512 % 256 == 0)
+        for (int j8 = 8 * cb; j8 < 8 * cb + 8; ++j8) {
+          const int c = col0 + 8 * j8;
+          const uint32_t blk = stage_u32 + ((((j8 & 7) << 4) ^ sw) | (4 * (lane & 3)));
 #pragma unroll
-      for (int j = 0; j < BN_WG / 8; ++j) {
-        const int c = col0 + 8 * j;
-        if (c >= p.N) continue;                               // N is even: the pair (c, c + 1) is in or out together
-        float v[4];
-        bias_act<EPI>(acc, j, p.bias, c, scale, v);
-        if constexpr (EPI == EPI_F32) {
-          float* o = static_cast<float*>(p.out);
-          *reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * p.ldo + c) = make_float2(v[0], v[1]);
-          *reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * p.ldo + c) = make_float2(v[2], v[3]);
-        } else {
-          uint32_t* o0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row0) * p.ldo + c);
-          uint32_t* o1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out) + static_cast<size_t>(row1) * p.ldo + c);
-          if constexpr (SPLIT) {
-            uint32_t* l0 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row0) * p.ldo + c);
-            uint32_t* l1 = reinterpret_cast<uint32_t*>(static_cast<typename O::T*>(p.out_lo) + static_cast<size_t>(row1) * p.ldo + c);
-            O::pack_pair(v[0], v[1], *o0, *l0);
-            O::pack_pair(v[2], v[3], *o1, *l1);
-          } else {
-            *o0 = O::pack(v[0], v[1]);
-            *o1 = O::pack(v[2], v[3]);
+          for (int h = 0; h < 2; ++h) {
+            float v[4];
+            bias_act<EPI>(acc[h], j8, p.bias, c, scale, v);
+            st_shared_u32(blk + (h * 64 + rw) * 128, O::pack(v[0], v[1]));
+            st_shared_u32(blk + (h * 64 + rw + 8) * 128, O::pack(v[2], v[3]));
           }
         }
-      }
-    } else {
-      // ============ fused residual + LayerNorm epilogue (out-projection / FF2) ============
-      //   y = acc + bias + resid (-> y_out); two-pass row statistics: the row sum over the thread's columns, the quad of lanes
-      //   that shares a row, then the other warpgroup (other 232 columns) through shared memory gives the mean; the sum of
-      //   (y - mean)^2 is reduced the same way.  One pass, E[y^2] - mean^2, loses the variance to cancellation once
-      //   |mean| / std is large.  The sums run over y - pivot, pivot = bias[0] + resid[row][0] (y's column 0 without the GEMM
-      //   term, the same in all 8 threads of a row): their terms are of the row's spread, not of its mean, so the mean of a row
-      //   far from zero comes out correctly rounded too (a plain fp32 sum of 464 values near 256 is off by several ulps of the
-      //   mean, which every output of the row inherits).  Normalise, 16-bit (+ fp32) outputs.
-      float* ssum = reinterpret_cast<float*>(smem + SM::kOffStat);   // [warpgroup][64 rows] row sums of y - pivot
-      float* ssq = ssum + 2 * 64;                                     // [warpgroup][64 rows] sums of squared deviations
-      const int N = p.N;
-      const float* r0p = p.resid + static_cast<size_t>(row0) * N;
-      const float* r1p = p.resid + static_cast<size_t>(row1) * N;
-      const float piv0 = __ldg(p.bias) + r0p[0], piv1 = __ldg(p.bias) + r1p[0];
-      float s0 = 0.0f, s1 = 0.0f;
-#pragma unroll
-      for (int j = 0; j < BN_WG / 8; ++j) {
-        const int c = col0 + 8 * j;
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c));
-        const float2 ra = *reinterpret_cast<const float2*>(r0p + c), rb = *reinterpret_cast<const float2*>(r1p + c);
-        acc[4 * j] += b.x + ra.x; acc[4 * j + 1] += b.y + ra.y;
-        acc[4 * j + 2] += b.x + rb.x; acc[4 * j + 3] += b.y + rb.y;
-        if (p.y_out != nullptr) {
-          *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row0) * N + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(p.y_out + static_cast<size_t>(row1) * N + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        acc[4 * j] -= piv0; acc[4 * j + 1] -= piv0; acc[4 * j + 2] -= piv1; acc[4 * j + 3] -= piv1;   // from here on: y - pivot
-        s0 += acc[4 * j] + acc[4 * j + 1];
-        s1 += acc[4 * j + 2] + acc[4 * j + 3];
-      }
-#pragma unroll
-      for (int o = 1; o <= 2; o <<= 1) {
-        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-      }
-      if ((lane & 3) == 0) { ssum[wn * 64 + rw] = s0; ssum[wn * 64 + rw + 8] = s1; }
-      named_bar_sync(1, kGemmConsumers);
-      const float inv_n = 1.0f / static_cast<float>(N);
-      const float mean0 = (s0 + ssum[(wn ^ 1) * 64 + rw]) * inv_n, mean1 = (s1 + ssum[(wn ^ 1) * 64 + rw + 8]) * inv_n;   // mean - pivot, like acc
-      float q0 = 0.0f, q1 = 0.0f;
-#pragma unroll
-      for (int j = 0; j < BN_WG / 8; ++j) {
-        const float d0 = acc[4 * j] - mean0, d1 = acc[4 * j + 1] - mean0, d2 = acc[4 * j + 2] - mean1, d3 = acc[4 * j + 3] - mean1;
-        q0 = fmaf(d0, d0, fmaf(d1, d1, q0));
-        q1 = fmaf(d2, d2, fmaf(d3, d3, q1));
-      }
-#pragma unroll
-      for (int o = 1; o <= 2; o <<= 1) {
-        q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-        q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-      }
-      if ((lane & 3) == 0) { ssq[wn * 64 + rw] = q0; ssq[wn * 64 + rw + 8] = q1; }
-      named_bar_sync(1, kGemmConsumers);
-      const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
-      const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
-      const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
-      typename O::T* out16 = static_cast<typename O::T*>(p.out);
-#pragma unroll
-      for (int j = 0; j < BN_WG / 8; ++j) {
-        const int c = col0 + 8 * j;
-        const float2 g = __ldg(reinterpret_cast<const float2*>(a.gam + c)), h = __ldg(reinterpret_cast<const float2*>(a.bet + c));
-        const float v0 = (acc[4 * j] - mean0) * rstd0 * (g.x + a.gadd) + h.x, v1 = (acc[4 * j + 1] - mean0) * rstd0 * (g.y + a.gadd) + h.y;
-        const float v2 = (acc[4 * j + 2] - mean1) * rstd1 * (g.x + a.gadd) + h.x, v3 = (acc[4 * j + 3] - mean1) * rstd1 * (g.y + a.gadd) + h.y;
-        if constexpr (SPLIT) {
-          typename O::T* lo16 = static_cast<typename O::T*>(p.out_lo);
-          O::pack_pair(v0, v1, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row0) * N + c));
-          O::pack_pair(v2, v3, *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c), *reinterpret_cast<uint32_t*>(lo16 + static_cast<size_t>(row1) * N + c));
-        } else {
-          *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row0) * N + c) = O::pack(v0, v1);
-          *reinterpret_cast<uint32_t*>(out16 + static_cast<size_t>(row1) * N + c) = O::pack(v2, v3);
-        }
-        if (p.out32 != nullptr) {
-          *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row0) * N + c) = make_float2(v0, v1);
-          *reinterpret_cast<float2*>(p.out32 + static_cast<size_t>(row1) * N + c) = make_float2(v2, v3);
+        fence_proxy_async_smem();
+        wg_bar();
+        if (leader) {
+          tma_store_2d(&map_out, stage, n0 + cb * 64, m0);
+          bulk_commit_group();
         }
       }
     }
-    if constexpr (!STAGED) break;                            // one tile per CTA
+    if (!mine_any) {                                             // no tile of this item: release its A rows unread
+      for (int kb = 0; kb < num_kb; ++kb) { mbar_wait(&a_full[kb], ip); mbar_arrive(&a_empty[kb]); }
+    }
   }
-  if constexpr (STAGED) {
-    if ((threadIdx.x & 127) == 0) bulk_wait_group_all();   // the last staged stores are complete before the CTA exits
-  }
+  if (leader) bulk_wait_group_all();                           // the last stores are complete before the CTA exits
 }
 
 // ============ persistent LN GEMM: out-projection / FF2 in the one-plane modes ============

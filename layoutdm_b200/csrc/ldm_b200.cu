@@ -44,10 +44,12 @@ constexpr int kMaxLayouts = 32767;  // layouts per call
 constexpr int kLogitLd = 160;       // padded logits row (C <= 160)
 constexpr int kDModel = 464;        // the kernels are laid out for the paper's backbone: d = 464 (LN tiles 224 + 240), ff = 4 d
 // GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, operand mode>
-// QKV / FF1: 128 x 256 tiles; 3 ring stages next to the 64 KB store staging tile (one-plane modes), 4 in the split mode,
-// which stores straight from the fragment
-constexpr int kPlainBN = 256;
-template <int MODE> constexpr int kPlainStages = kOpSplit<MODE> ? 4 : 3;
+// QKV / FF1: fp16 / bf16: gemm_rowblock_kernel (resident A rows, 128-column tiles); the split mode: 128 x 256 tiles of
+// gemm_tc_kernel, 4 ring stages
+constexpr int kPlainBN = 256, kPlainStages = 4;
+constexpr int kRbCols = RbSmem::kCols;
+static_assert(kDModel <= RbSmem::kAKb * RbSmem::kKB && kAttN % kRbCols == 0 && kQkvN % 64 == 0 && 4 * kDModel % 64 == 0,
+              "row-block GEMM shapes: K fits the resident A, Q tiles are whole tiles, N is whole 64-column store blocks");
 constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
 // out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue).  fp16 / bf16: gemm_ln_kernel (persistent, epilogue
 // warps, 32-element k-blocks: K = 512 and 1856 have no tail); the split mode: the fragment-epilogue kernel below
@@ -55,21 +57,16 @@ constexpr int kLnBN = 232, kLnStages = 3;
 // k-block of the LN GEMMs' operands (the TMA box columns) in every mode: the persistent kernel's, which is the split mode's
 constexpr int kLnKB = LnSmem::R::kKB;
 static_assert(LnSmem::kWgCols == kLnBN && kAttN % kLnKB == 0 && 4 * kDModel % kLnKB == 0 && gemm_kb(true) == kLnKB, "LN GEMM shapes");
-template <int MODE> constexpr auto kGemmQkv = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_QKV, MODE>;
-template <int MODE> constexpr auto kGemmFf1 = gemm_tc_kernel<kPlainBN, 2, kPlainStages<MODE>, EPI_RELU, MODE>;
+template <int EPI, int MODE> constexpr auto kGemmPlainSplit = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
 template <int MODE> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, MODE>;
-template <int MODE>
-constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages<MODE>, kOpSplit<MODE>, kStagedStore<EPI_QKV, kOpSplit<MODE>>>::kBytes;
+constexpr int kPlainSmem = GemmSmem<kPlainBN, 2, kPlainStages, true>::kBytes;
 constexpr int kHeadSmem = GemmSmem<kHeadBN, 2, kHeadStages>::kBytes;
 constexpr int kLnSmem = GemmSmem<kLnBN, 1, kLnStages>::kBytes;
 // the split mode's stage (two planes of a 32-element k-block) has the bytes of the one-plane 64-element stage, so the head and
-// LN GEMMs keep their stage counts in every mode (the plain GEMMs trade the staging tile for a fourth stage)
-static_assert(GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem && GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem &&
-              GemmSmem<kPlainBN, 2, 4, true>::R::kStageBytes == GemmSmem<kPlainBN, 2, 4>::R::kStageBytes,
+// LN GEMMs keep their stage counts in every mode
+static_assert(GemmSmem<kHeadBN, 2, kHeadStages, true>::kBytes == kHeadSmem && GemmSmem<kLnBN, 1, kLnStages, true>::kBytes == kLnSmem,
               "split-mode ring stages must keep the one-plane sizes");
-static_assert(kStagedStore<EPI_QKV, false> == kStagedStore<EPI_RELU, false> && kStagedStore<EPI_QKV, true> == kStagedStore<EPI_RELU, true>,
-              "QKV and FF1 share one shared-memory size");
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -153,7 +150,7 @@ struct LdmHandle {
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
   CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
-  CUtensorMap m_qkv16_st, m_hid16_st;                                        // 64-row boxes: the QKV / FF1 GEMMs' TMA stores (one-plane modes)
+  CUtensorMap m_qkv16_st, m_hid16_st;                                        // 128-row boxes: the row-block GEMMs' TMA stores (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
@@ -164,6 +161,7 @@ struct LdmHandle {
   int num_sms = 0;             // the persistent GEMMs run at most one CTA per SM
   int max_threads_sm = 0;      // with num_sms: the launch policy of torch's distribution kernels (LDM_NOISE_TORCH)
   int gemm_ctas = 0;           // env LDM_GEMM_CTAS=n (n >= 1): at most n CTAs in a persistent GEMM launch; 0: no cap
+  int gemm_split = 0;          // env LDM_GEMM_SPLIT=g (g >= 1): column ranges per row block of the row-block GEMMs; 0: automatic
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
                                // The split mode always launches it: the draw kernels write one 16-bit plane only
   cudaStream_t cap_stream = nullptr;
@@ -352,8 +350,13 @@ cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), dim3 grid,
 template <int MODE>
 int set_smem() {
   constexpr auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-  CK(cudaFuncSetAttribute(kGemmQkv<MODE>, attr, kPlainSmem<MODE>));
-  CK(cudaFuncSetAttribute(kGemmFf1<MODE>, attr, kPlainSmem<MODE>));
+  if constexpr (kOpSplit<MODE>) {
+    CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_QKV, MODE>, attr, kPlainSmem));
+    CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_RELU, MODE>, attr, kPlainSmem));
+  } else {
+    CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_QKV, MODE>, attr, RbSmem::kBytes));
+    CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_RELU, MODE>, attr, RbSmem::kBytes));
+  }
   CK(cudaFuncSetAttribute(kGemmHead<MODE>, attr, kHeadSmem));
   if constexpr (kOpSplit<MODE>) CK(cudaFuncSetAttribute(kGemmLn<MODE>, attr, kLnSmem));
   else CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE>, attr, LnSmem::kBytes));
@@ -417,6 +420,8 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   h->cap = n_layouts;
   h->ws_generation++;
   int rc;
+  // the row-block GEMM's resident A k-blocks are the one-plane ring's (64 elements): QKV, FF1 and the head share these maps
+  static_assert(gemm_kb(false) == RbSmem::kKB, "one A geometry for QKV / FF1 / head");
   const int kb = gemm_kb(h->split);
   if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM, kb))) return rc;
   if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM, kb))) return rc;
@@ -424,9 +429,9 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64, kLnKB))) return rc;
   // attention's Q / K / V head tiles: 128 rows x one padded head, in every mode
   if ((rc = make_op_maps(h, &h->m_qkv16, &h->m_qkv16_lo, h->qkv16, h->qkv16_lo, M, kQkvN, kBM, kHeadPad))) return rc;
-  // the staged stores: 64 x 64 boxes of the staging tile (128-byte swizzle)
-  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, 64, 64, h->bf16))) return rc;
-  if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16, M, ff, 64, 64, h->bf16))) return rc;
+  // the row-block GEMMs' stores: 64-column x 128-row boxes of the staging tile (128-byte swizzle)
+  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, kBM, 64, h->bf16))) return rc;
+  if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16, M, ff, kBM, 64, h->bf16))) return rc;
   return LDM_OK;
 }
 
@@ -435,21 +440,33 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   const auto maps = [](const CUtensorMap& hi, const CUtensorMap& lo) { return op_maps<MODE>(hi, lo); };
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
   const int M = n * kBM;
-  // Grids: the GEMMs with TMA-staged stores and the fp16 / bf16 LN GEMMs (epilogue warps) are persistent (one CTA per SM):
-  // their epilogues run under the next tile's MMAs.  The others store from the fragment, so a CTA has nothing to overlap its
+  // Grids: the fp16 / bf16 row-block GEMMs (QKV, FF1) and LN GEMMs (epilogue warps) are persistent (one CTA per SM): their
+  // epilogues run under the next tile's MMAs.  gemm_tc_kernel stores from the fragment, so a CTA has nothing to overlap its
   // epilogue with; one tile per CTA lets the hardware hand each SM its next tile the moment it is free, which measured faster
-  // for them than a static persistent split (the kernels of the latter run exactly one tile per CTA: LDM_GEMM_CTAS caps the
-  // persistent grids only)
+  // for it than a static persistent split (LDM_GEMM_CTAS caps the persistent grids only)
   const auto grid = [&](int tiles, bool persistent) {
     if (!persistent) return dim3(tiles);
     return dim3(std::min({tiles, h->num_sms, h->gemm_ctas > 0 ? h->gemm_ctas : tiles}));
   };
-  const CUtensorMap no_store{};            // map_out of the epilogues that store from the fragment
-  constexpr bool kStaged = kStagedStore<EPI_QKV, kOpSplit<MODE>>;
+  // QKV / FF1 (bias, q-scale | ReLU): the row-block kernel in fp16 / bf16, 128-row x 256-column tiles in the split mode.  The
+  // row-block kernel cuts each row block into n_ranges column ranges, each loading the row block's A once: one range when the
+  // row blocks alone fill the SMs, otherwise enough for the items to fill them (at most one per tile); LDM_GEMM_SPLIT=g forces g
+  const auto plain_gemm = [&](auto epi, const OpMaps<MODE>& a, const OpMaps<MODE>& w, const CUtensorMap& out, GemmParams p) {
+    constexpr int EPI = decltype(epi)::value;
+    if constexpr (kOpSplit<MODE>) {
+      p.n_tiles = (p.N + kPlainBN - 1) / kPlainBN;
+      return launch_step(h, kGemmPlainSplit<EPI, MODE>, grid(p.n_tiles * n, false), kGemmThreads, kPlainSmem, st, a, w, p);
+    } else {
+      p.n_tiles = (p.N + kRbCols - 1) / kRbCols;
+      const int g = h->gemm_split > 0 ? h->gemm_split : n >= h->num_sms ? 1 : (h->num_sms + n - 1) / n;
+      p.n_ranges = std::min(g, p.n_tiles);
+      return launch_step(h, gemm_rowblock_kernel<EPI, MODE>, grid(n * p.n_ranges, true), kRbThreads, RbSmem::kBytes, st, a, w, out, p);
+    }
+  };
   // the LN GEMMs (out-projection, FF2), 64 whole rows per tile: the fragment-epilogue kernel in the split mode, the persistent
   // LN kernel otherwise
   const auto ln_gemm = [&](const OpMaps<MODE>& a, const OpMaps<MODE>& w, const GemmParams& p) {
-    if constexpr (kOpSplit<MODE>) return launch_step(h, kGemmLn<MODE>, grid(M / 64, false), kGemmThreads<EPI_LN, MODE>, kLnSmem, st, a, w, no_store, p);
+    if constexpr (kOpSplit<MODE>) return launch_step(h, kGemmLn<MODE>, grid(M / 64, false), kGemmThreads, kLnSmem, st, a, w, p);
     else return launch_step(h, gemm_ln_kernel<MODE>, grid(M / 64, true), kLnThreads, LnSmem::kBytes, st, a, w, p);
   };
   int done = 0;
@@ -468,11 +485,10 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
     {  // QKV projection (+bias, q * 1/sqrt(head_dim))
-      GemmParams p{M, kQkvN, d, kQkvN / kPlainBN, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
+      GemmParams p{M, kQkvN, d, 0, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
       p.rev = next_rev(); p.out_lo = h->qkv16_lo;
       ProfScope ps(h, CAT_QKV, st);
-      CK(launch_step(h, kGemmQkv<MODE>, grid(p.n_tiles * n, kStaged), kGemmThreads<EPI_QKV, MODE>, kPlainSmem<MODE>, st, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]),
-                     kStaged ? h->m_qkv16_st : no_store, p));
+      CK(plain_gemm(std::integral_constant<int, EPI_QKV>{}, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]), h->m_qkv16_st, p));
     }
     LDM_STAGE_DONE();
     {
@@ -489,11 +505,10 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
-      GemmParams p{M, ff, d, (ff + kPlainBN - 1) / kPlainBN, h->b1[l], h->hid16, ff, 1.0f, 0};   // 7 tiles of 256 columns + one of 64
+      GemmParams p{M, ff, d, 0, h->b1[l], h->hid16, ff, 1.0f, 0};   // 14 tiles of 128 columns + one of 64 (split mode: 7 of 256 + one of 64)
       p.rev = next_rev(); p.out_lo = h->hid16_lo;
       ProfScope ps(h, CAT_FF1, st);
-      CK(launch_step(h, kGemmFf1<MODE>, grid(p.n_tiles * n, kStaged), kGemmThreads<EPI_RELU, MODE>, kPlainSmem<MODE>, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]),
-                     kStaged ? h->m_hid16_st : no_store, p));
+      CK(plain_gemm(std::integral_constant<int, EPI_RELU>{}, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]), h->m_hid16_st, p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
@@ -515,7 +530,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads<EPI_F32, MODE>, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), no_store, p));
+    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
@@ -712,6 +727,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   h->num_sms = prop.multiProcessorCount;
   h->max_threads_sm = prop.maxThreadsPerMultiProcessor;
   if (const char* e = getenv("LDM_GEMM_CTAS")) h->gemm_ctas = std::max(1, atoi(e));
+  if (const char* e = getenv("LDM_GEMM_SPLIT")) h->gemm_split = std::max(1, atoi(e));
 #define TRY(x) do { rc = (x); if (rc) { ldm_destroy(h); return rc; } } while (0)
 
   // parameter buffers and the TMA descriptors of the 16-bit weights
@@ -720,6 +736,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   TRY(dev_alloc(h, &h->hlnw, static_cast<size_t>(d)));
   TRY(dev_alloc(h, &h->hlnb, static_cast<size_t>(d)));
   TRY(dev_alloc(h, &h->adaln, static_cast<size_t>(L) * T * 2 * d));
+  const int plain_w_rows = h->split ? kPlainBN : kRbCols;
   for (int l = 0; l < L; ++l) {
     TRY(alloc16(h, &h->wqkv[l], &h->wqkv_lo[l], kQkvN, d));
     TRY(alloc16(h, &h->wo[l], &h->wo_lo[l], d, kAttN));
@@ -731,9 +748,10 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(dev_alloc(h, &h->b2[l], static_cast<size_t>(d)));
     TRY(dev_alloc(h, &h->ln2w[l], static_cast<size_t>(d)));
     TRY(dev_alloc(h, &h->ln2b[l], static_cast<size_t>(d)));
-    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, kPlainBN, gemm_kb(h->split)));   // one warpgroup's weight rows per box
+    // QKV / FF1 weights: one tile's weight rows per box (row-block kernel: 128, split mode: 256)
+    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, plain_w_rows, gemm_kb(h->split)));
     TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, kLnKB));
-    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, kPlainBN, gemm_kb(h->split)));
+    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, plain_w_rows, gemm_kb(h->split)));
     TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, kLnKB));
   }
   TRY(alloc16(h, &h->whead, &h->whead_lo, kLogitLd, d));
