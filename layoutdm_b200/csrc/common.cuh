@@ -107,6 +107,28 @@ LDM_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32
 template <int R>
 LDM_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
+// ------------------------------------------------------------------------------------------------------------
+// thread-block clusters (1-D): the CTA's rank, the cluster's index and count, the cluster barrier, stores into a peer's
+// shared memory
+// ------------------------------------------------------------------------------------------------------------
+LDM_DEVINL uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+LDM_DEVINL uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
+LDM_DEVINL uint32_t cluster_count_x() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return r; }
+// every thread of every CTA of the cluster arrives (release) and waits (acquire); also a barrier of the CTA's own threads
+LDM_DEVINL void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// the shared::cluster address of this CTA's shared-memory location p in cluster CTA `rank`
+LDM_DEVINL uint32_t map_peer(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+// 4-byte store into another CTA's shared memory (addresses from map_peer) that counts its bytes on that CTA's mbarrier bar
+LDM_DEVINL void st_async_f32(uint32_t addr, float v, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.f32 [%0], %1, [%2];" ::"r"(addr), "f"(v), "r"(bar) : "memory");
+}
+
 // named barrier among a subset of the CTA's warps (id 1..15; id 0 is __syncthreads)
 LDM_DEVINL void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 // counts the calling warp's threads toward the barrier without waiting for it

@@ -13,12 +13,14 @@
 //
 // gemm_tc_kernel adds the epilogue on the consumers' own accumulator fragment.  Tile shapes:
 //   WG_M = 2 : 128 rows x BN_WG columns, the warpgroups split the rows (split-mode QKV, FF1: 256 columns; vocabulary head: 160)
-//   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the LN epilogue: 2 x 232 = 464 =
-//              d_model, so a CTA holds whole rows and the LayerNorm row statistics are combined in shared memory.
+//   WG_M = 1 :  64 rows x 2 BN_WG columns, the warpgroups split the columns.  Used by the split mode's LN epilogue: 2 x 232 =
+//              464 = d_model, so a CTA holds whole rows and the LayerNorm row statistics are combined in shared memory.
 // Epilogues:  QKV (bias, q-scale, 16-bit) | RELU (FF1: bias, ReLU, 16-bit) | F32 (bias; vocabulary head) |
 //             LN  (out-projection / FF2: bias + residual + LayerNorm, affine or timestep-adaptive, fused).
 // It stores from the fragment.  gemm_rowblock_kernel (QKV, FF1 in fp16 / bf16) keeps each layout's A rows resident and stores
-// through staging buffers with TMA (see there).  gemm_ln_kernel (out-projection, FF2 in fp16 / bf16) adds a tile buffer and epilogue warps of its own (see there).
+// through staging buffers with TMA (see there).  gemm_ln_kernel (out-projection, FF2 in fp16 / bf16) runs on CTA pairs that
+// split a 128-row block's columns and exchange the LayerNorm row statistics through each other's shared memory, with a tile
+// buffer and epilogue warps of its own (see there).
 //
 // Reference ops replaced: nn.Linear / nn.MultiheadAttention projections / nn.LayerNorm / AdaLayerNorm in
 // T/models/transformer_utils.py:79-83,165-210 and T/models/common/nn_lib.py:187-189,235.
@@ -566,74 +568,107 @@ gemm_rowblock_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 r
 }
 
 // ============ persistent LN GEMM: out-projection / FF2 in the one-plane modes ============
-// 64 x 464 tiles (whole rows), min(tiles, SMs) CTAs of 384 threads; CTA b runs tiles b, b + gridDim.x, ...  The LayerNorm runs
-// in warps of its own and the fp32 traffic goes through bulk copies, so a tile's epilogue overlaps the next tile's MMAs:
-//   warps 0..7  : two MMA warpgroups, 64 rows x 232 columns each, m64n232k16 from the ring.  After a tile's last k-block they
-//                 wait for the tile's residual rows in the tile buffer, replace them by y = acc + (bias + resid) and go
-//                 straight on to the next tile.
+// A cluster of two CTAs takes one layout's 128-row block at a time and splits its 464 columns: CTA rank h computes columns
+// 232 h .. 232 h + 231 of all 128 rows, so every weight k-block it streams from L2 feeds 128 rows (FF2 reads 1.34 MB per CTA
+// tile against 1.96 MB for a 64 x 464 tile of the same floats).  Clusters: min(row blocks, active clusters); cluster c runs the
+// row blocks c, c + clusters, ...  384 threads per CTA.  The LayerNorm runs in warps of its own and the fp32 traffic goes
+// through bulk copies, so a tile's epilogue overlaps the next tile's MMAs:
+//   warps 0..7  : two MMA warpgroups, warpgroup w rows 64 w .. 64 w + 63 x the CTA's 232 columns, m64n232k16 from the ring.
+//                 After a tile's last k-block they wait for the tile's residual half rows in the tile buffer, replace them by
+//                 y = acc + (bias + resid), send the rows' sums of y - pivot (below) and go straight on to the next tile.
 //   warps 8..10 : epilogue: the row statistics, the LayerNorm / AdaLN and the 16-bit stores from the tile buffer.  Warp 8
-//                 also issues the bulk copies of whole rows between the buffer and global memory: y out (the next residual),
-//                 the normalised fp32 rows (written back into the buffer) out, and the next tile's residual rows in.
+//                 also issues the bulk copies of half rows (928 bytes at byte offset 928 h) between the buffer and global
+//                 memory: y out (the next residual), the normalised fp32 rows (written back into the buffer) out, and the next
+//                 tile's residual rows in.
 //   warp 11     : producer, one lane issues the TMA loads.
 // 168 registers for every warp, no setmaxnreg: ptxas compiles the whole kernel under the launch bound's register count, and a
 // 512-thread block (a whole producer warpgroup) would leave the m64n232 wgmma 128, fewer than it needs.  Three epilogue warps
-// cannot keep enough loads and stores in flight to move a tile's ~300 KB of fp32 rows at HBM rate themselves (~40 us per
-// tile); the bulk copies need no registers.  Ring: 3 stages of 32-element k-blocks with the 64-byte swizzle (the split mode's
-// geometry, one plane): a 64-element k-block leaves room for only 2 stages beside the 118 KB tile buffer.  The split mode keeps
-// the fragment-epilogue kernel above: its two-plane stages do not fit beside the buffer.
+// cannot keep enough loads and stores in flight to move a tile's fp32 rows at HBM rate themselves; the bulk copies need no
+// registers.  Ring: STAGES stages of 32-element k-blocks with the 64-byte swizzle (8 KB of A + 14.5 KB of W each) beside the
+// 116 KB tile buffer; 4 fit.  The split mode keeps the fragment-epilogue kernel above: its two-plane stages do not fit beside the buffer.
+//
 // The results are bit for bit those of the fragment epilogue: the same k16 MMA sequence, y = acc + (bias + resid), and the row
 // statistics keep its summation order (per row 8 chains (h, q), h = column half, q = quad lane, each summing
 // (y_c - piv) + (y_c+1 - piv) over c = 232 h + 8 j + 2 q, j ascending; (q0 + q1) + (q2 + q3), then half + half) and its FMA
-// contractions (y - mean is one fma(-sum, 1/N, y - piv), the output fma(d * rstd, gamma + gadd, beta)).
+// contractions (y - mean is one fma(-sum, 1/N, y - piv), the output fma(d * rstd, gamma + gadd, beta)).  The pivot is
+// bias[0] + resid[row][0] in both CTAs, read from global memory (rank 1 does not hold column 0).  Half h of a row lives in
+// CTA h: each CTA forms its half's quad-combined partial, stores it into the peer's slot with st.async (completion counted on
+// the peer's mbarrier) and adds the two, own + peer -- the same float in both CTAs, since addition commutes.  The row sums
+// are formed by the MMA warpgroups from y in registers (a fragment thread's columns 2 q + 8 j are exactly chain q) and sent
+// before the epilogue starts, so the epilogue reads the buffer once for the statistics, not twice, and rarely waits for
+// the peer's sums.  The epilogue warps form and exchange the sums of squared deviations the same way.
+// Exchange slots: two per statistic, by tile parity, each with an mbarrier that its own CTA arms (expect_tx) in the tile
+// that uses it; the peer's bytes may land before that, which the transaction count allows.  The peer writes slot b for tile
+// i + 2 only once it holds this CTA's variance partials of tile i + 1 (its MMA warpgroups send the sums of tile i + 2 after
+// its epilogue has finished tile i + 1 and loaded the residual rows of tile i + 2), and those partials are sent after every
+// epilogue thread of this CTA has passed the named barriers that end tile i, so after every read of slot b for tile i: two
+// slots cannot be overrun.
+// Cluster barriers: after the barrier init (no remote store before the peer's barriers exist) and before exit (no CTA leaves
+// while its peer may still store into its shared memory); every thread reaches both.
 constexpr int kLnThreads = 384, kLnEpiThreads = 96;
+template <int STAGES>
 struct LnSmem {
-  static constexpr int kRows = 64, kWgCols = 232, kCols = 2 * kWgCols;
-  using R = Ring<32, 1, kRows, kWgCols, 2, 3, false>;          // K = 512, 1856 (checked at create)
-  // tile buffer [64][kLd] fp32: the 8-float pad puts the 8 rows of a fragment access in distinct 32-byte bank groups and
-  // keeps every row 16-byte aligned for the bulk copies
-  static constexpr int kLd = kCols + 8;
+  static constexpr int kRows = kBM, kCols = 232, kPairCols = 2 * kCols;
+  using R = Ring<32, 1, kRows, kCols, 1, STAGES, false>;       // K = 512, 1856 (checked at create)
+  // tile buffer [128][kLd] fp32, unpadded: a row is 928 bytes = 32 mod 128, so the 4 rows of a half warp's fragment access fall in
+  // distinct 32-byte bank groups, and every row is 16-byte aligned for the bulk copies
+  static constexpr int kLd = kCols;
   static constexpr int kOffBuf = R::kBytes;
-  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // ring full[3], empty[3]; res_full, buf_full
-  static constexpr int kOffStat = kOffBars + 64;                 // per row: pivot, row sum of y - pivot, rstd
-  static constexpr int kBytes = kOffStat + 3 * kRows * 4 + 1024 /*align slack*/;
-  static_assert(kLd * 4 % 16 == 0, "bulk copies need 16-byte aligned rows");
-  static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory per CTA");
+  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // ring full[4], empty[4]; res_full, buf_full; xs_full[2], xv_full[2]
+  static constexpr int kOffStat = kOffBars + 128;
+  // per row: pivot, own half's sum of y - pivot, row sum, own half's sum of squared deviations, rstd; the peer's partials [2][kRows] x 2
+  static constexpr int kBytes = kOffStat + 9 * kRows * 4 + 1024 /*align slack*/;
+  static_assert(2 * R::kStages * 8 + 6 * 8 <= 128, "barrier block overflow");
+  static_assert(kLd * 4 % 16 == 0 && kLd * 4 % 128 == 32, "bulk copies need 16-byte aligned rows; fragment accesses need rows 32 mod 128 bytes");
+  static_assert(kRows * kCols * 4 < (1 << 20), "a tile's residual bytes exceed the mbarrier transaction count");
 };
 
-template <int MODE>
+template <int MODE, int STAGES>
 __global__ void __launch_bounds__(kLnThreads, 1)
-gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 64 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 232 rows*/,
+gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 232 rows*/,
                const GemmParams p) {
   static_assert(!kOpSplit<MODE>, "the split mode runs the fragment-epilogue LN GEMM");
-  using SM = LnSmem;
+  using SM = LnSmem<STAGES>;
   using O = OpT<MODE>;
-  constexpr int kRows = SM::kRows, kWgCols = SM::kWgCols, kLd = SM::kLd, kAcc = kWgCols / 2;
+  constexpr int kRows = SM::kRows, kCols = SM::kCols, kLd = SM::kLd, kAcc = kCols / 2;
   constexpr int kEpi = kGemmConsumers, kProducer = kEpi + kLnEpiThreads;   // first thread of the epilogue warps / producer warp
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
+  typename SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
   uint64_t* res_full = ring.empty + SM::R::kStages;             // the tile's residual rows have landed in the buffer
   uint64_t* buf_full = res_full + 1;                             // the MMA warpgroups wrote y into the buffer
+  uint64_t* xs_full = buf_full + 1;                              // [2] the peer's row sums of tile parity b have landed
+  uint64_t* xv_full = xs_full + 2;                               // [2] the peer's sums of squared deviations
   float* buf = reinterpret_cast<float*>(smem + SM::kOffBuf);
   float* s_piv = reinterpret_cast<float*>(smem + SM::kOffStat);
-  float* s_sum = s_piv + kRows;
-  float* s_rstd = s_sum + kRows;
+  float* s_own = s_piv + kRows;
+  float* s_sum = s_own + kRows;
+  float* v_own = s_sum + kRows;
+  float* s_rstd = v_own + kRows;
+  float* x_sum = s_rstd + kRows;                                 // [2][kRows] written by the peer
+  float* x_var = x_sum + 2 * kRows;                              // [2][kRows] written by the peer
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int N = p.N;
   const int num_kb = SM::R::num_kb(p.K);
   const int n_work = p.M / kRows;
+  const uint32_t rank = cluster_ctarank();
+  const int col0 = kCols * static_cast<int>(rank);               // the CTA's first column
+  const int cl = static_cast<int>(cluster_id_x()), n_cl = static_cast<int>(cluster_count_x());
   const auto tile_m0 = [&](int t) { return (p.rev ? n_work - 1 - t : t) * kRows; };
+  const uint32_t peer = rank ^ 1;
+  const uint32_t px_sum = map_peer(x_sum, peer), pxs_full = map_peer(xs_full, peer);
 
   if (threadIdx.x == kProducer) {
     ring.prefetch(map_a, map_b);
     ring.init();
     mbar_init(res_full, 1);
     mbar_init(buf_full, kGemmConsumers);
+    for (int b = 0; b < 2; ++b) { mbar_init(&xs_full[b], 1); mbar_init(&xv_full[b], 1); }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync();                                            // both CTAs' barriers are initialised before any remote store
   pdl_sync();                                                // everything above overlapped the previous kernel's tail
 
   if (threadIdx.x >= kProducer) {
@@ -641,72 +676,72 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 64 rows*/, 
     if (threadIdx.x == kProducer) {
       uint32_t phase = 0;
       int s = 0;
-      for (int t = blockIdx.x; t < n_work; t += gridDim.x) ring.load_tile(s, phase, map_a, map_b, num_kb, tile_m0(t), 0);
+      for (int t = cl; t < n_work; t += n_cl) ring.load_tile(s, phase, map_a, map_b, num_kb, tile_m0(t), col0);
     }
-    return;
-  }
-
-  if (threadIdx.x >= kEpi) {
+  } else if (threadIdx.x >= kEpi) {
     // ===================== epilogue warps =====================
     const int et = threadIdx.x - kEpi;
-    const bool copier = et < 32;                             // warp 8: the bulk copies, one row per lane at a time
-    const uint32_t row_bytes = static_cast<uint32_t>(N) * sizeof(float);
+    const bool copier = et < 32;                             // warp 8: the bulk copies, one half row per lane at a time
+    constexpr uint32_t kRowBytes = kCols * sizeof(float);
     const float inv_n = 1.0f / static_cast<float>(N);
-    constexpr int kVec = kWgCols / 2;                        // float4 columns of a row (116)
+    constexpr int kVec = kCols / 4;                          // float4 columns of a half row (58)
     constexpr int kTotal = kRows * kVec;                     // float4 of a tile; element i = k * 96 + et
     constexpr int kPerThread = (kTotal + kLnEpiThreads - 1) / kLnEpiThreads;
-    // the residual rows of tile t into the buffer (the buffer is free: every read of it and every bulk store from it is done)
+    const uint32_t px_var = map_peer(x_var, peer), pxv_full = map_peer(xv_full, peer);
+    // the residual half rows of tile t into the buffer (the buffer is free: every read of it and every bulk store from it is done)
     const auto load_resid = [&](int t) {
-      if (lane == 0) mbar_arrive_expect_tx(res_full, kRows * row_bytes);
+      if (lane == 0) mbar_arrive_expect_tx(res_full, kRows * kRowBytes);
       __syncwarp();
-      const float* src = p.resid + static_cast<size_t>(tile_m0(t)) * N;
-      for (int r = lane; r < kRows; r += 32) bulk_copy_g2s(buf + r * kLd, src + static_cast<size_t>(r) * N, row_bytes, res_full);
+      const float* src = p.resid + static_cast<size_t>(tile_m0(t)) * N + col0;
+      for (int r = lane; r < kRows; r += 32) bulk_copy_g2s(buf + r * kLd, src + static_cast<size_t>(r) * N, kRowBytes, res_full);
     };
-    const auto store_rows = [&](float* dst) {                // the buffer's rows to dst, one bulk group per lane
-      for (int r = lane; r < kRows; r += 32) bulk_copy_s2g(dst + static_cast<size_t>(r) * N, buf + r * kLd, row_bytes);
+    const auto store_rows = [&](float* dst) {                // the buffer's half rows to dst, one bulk group per lane
+      for (int r = lane; r < kRows; r += 32) bulk_copy_s2g(dst + static_cast<size_t>(r) * N, buf + r * kLd, kRowBytes);
       bulk_commit_group();
     };
-    if (copier) load_resid(blockIdx.x);
+    if (copier) load_resid(cl);
     uint32_t bphase = 0;
-    for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-      const int m0 = tile_m0(t);
+    int it = 0;                                              // the CTA's tile count: exchange slot it & 1, its pass (it >> 1) & 1
+    for (int t = cl; t < n_work; t += n_cl, ++it) {
+      const int m0 = tile_m0(t), b = it & 1;
+      const uint32_t xph = (it >> 1) & 1;
+      if (et == 0) { mbar_arrive_expect_tx(&xs_full[b], kRows * 4); mbar_arrive_expect_tx(&xv_full[b], kRows * 4); }
       mbar_wait(buf_full, bphase);
-      if (copier && p.y_out != nullptr) store_rows(p.y_out + static_cast<size_t>(m0) * N);
-      // row statistics, a group of 4 rows per warp at a time; lane = 8 row + 4 h + q owns chain (h, q) of its row
-      {
-        const int h = (lane >> 2) & 1, q = lane & 3;
+      if (copier && p.y_out != nullptr) store_rows(p.y_out + static_cast<size_t>(m0) * N + col0);
+      // the sums of squared deviations, a group of 8 rows per warp at a time; lane = 4 row + q owns chain q of its row's half.
+      // The row sums came with y: this half's from the MMA warpgroups (s_own), the other's from the peer's
+      const int q = lane & 3;
+      mbar_wait(&xs_full[b], xph);
 #pragma unroll 1
-        for (int g = et >> 5; g < kRows / 4; g += kLnEpiThreads / 32) {
-          const int r = 4 * g + (lane >> 3);
-          const float piv = s_piv[r];
-          const float* yr = buf + r * kLd + h * kWgCols + 2 * q;
-          float s = 0.0f;
+      for (int g = et >> 5; g < kRows / 8; g += kLnEpiThreads / 32) {
+        const int r = 8 * g + (lane >> 2);
+        const float piv = s_piv[r], s = s_own[r] + x_sum[b * kRows + r];   // the row sum of y - pivot; mean - pivot = s / N
+        const float* yr = buf + r * kLd + 2 * q;
+        float v = 0.0f;
 #pragma unroll
-          for (int j = 0; j < kWgCols / 8; ++j) {
-            const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
-            s += (y.x - piv) + (y.y - piv);
-          }
-          s += __shfl_xor_sync(0xffffffffu, s, 1);
-          s += __shfl_xor_sync(0xffffffffu, s, 2);
-          s += __shfl_xor_sync(0xffffffffu, s, 4);           // the row sum of y - pivot; mean - pivot = s / N
-          float v = 0.0f;
-#pragma unroll
-          for (int j = 0; j < kWgCols / 8; ++j) {
-            const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
-            const float d0 = fmaf(-s, inv_n, y.x - piv), d1 = fmaf(-s, inv_n, y.y - piv);
-            v = fmaf(d0, d0, fmaf(d1, d1, v));
-          }
-          v += __shfl_xor_sync(0xffffffffu, v, 1);
-          v += __shfl_xor_sync(0xffffffffu, v, 2);
-          v += __shfl_xor_sync(0xffffffffu, v, 4);
-          if ((lane & 7) == 0) { s_sum[r] = s; s_rstd[r] = 1.0f / sqrtf(fmaxf(v * inv_n, 0.0f) + 1e-5f); }
+        for (int j = 0; j < kCols / 8; ++j) {
+          const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
+          const float d0 = fmaf(-s, inv_n, y.x - piv), d1 = fmaf(-s, inv_n, y.y - piv);
+          v = fmaf(d0, d0, fmaf(d1, d1, v));
+        }
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        if (q == 0) { s_sum[r] = s; v_own[r] = v; st_async_f32(px_var + (b * kRows + r) * 4, v, pxv_full + b * 8); }
+      }
+      mbar_wait(&xv_full[b], xph);
+      if (q == 0) {                                          // the rows whose partials this lane sent
+#pragma unroll 1
+        for (int g = et >> 5; g < kRows / 8; g += kLnEpiThreads / 32) {
+          const int r = 8 * g + (lane >> 2);
+          s_rstd[r] = 1.0f / sqrtf(fmaxf((v_own[r] + x_var[b * kRows + r]) * inv_n, 0.0f) + 1e-5f);
         }
       }
       if (copier) bulk_wait_group_read<0>();                 // the y rows are out of the buffer before it is overwritten
       named_bar_sync(1, kLnEpiThreads);
       // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a bulk store
       const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
-      typename O::T* out16 = static_cast<typename O::T*>(p.out);
+      const float *gam = a.gam + col0, *bet = a.bet + col0;
+      typename O::T* out16 = static_cast<typename O::T*>(p.out) + col0;
       const bool keep32 = p.out32 != nullptr;
 #pragma unroll 6
       for (int k = 0; k < kPerThread; ++k) {
@@ -714,52 +749,80 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 64 rows*/, 
         if (i >= kTotal) continue;
         float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
         const float4 y = *bp;
-        const float4 g = __ldg(reinterpret_cast<const float4*>(a.gam + c)), b = __ldg(reinterpret_cast<const float4*>(a.bet + c));
+        const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), h = __ldg(reinterpret_cast<const float4*>(bet + c));
         const float piv = s_piv[r], s = s_sum[r], rstd = s_rstd[r];
-        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, b.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, b.y),
-                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, b.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, b.w));
+        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, h.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, h.y),
+                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, h.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, h.w));
         *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
         if (keep32) *bp = v;
       }
       if (keep32) fence_proxy_async_smem();                  // the fp32 rows are visible to the bulk store
       named_bar_sync(1, kLnEpiThreads);
       if (copier) {
-        if (keep32) store_rows(p.out32 + static_cast<size_t>(m0) * N);
+        if (keep32) store_rows(p.out32 + static_cast<size_t>(m0) * N + col0);
         bulk_wait_group_read<0>();
-        if (t + static_cast<int>(gridDim.x) < n_work) load_resid(t + gridDim.x);
+        if (t + n_cl < n_work) load_resid(t + n_cl);
       }
       bphase ^= 1;
     }
     if (copier) bulk_wait_group_all();                       // the last bulk stores are complete before the CTA exits
-    return;
-  }
-
-  // ===================== MMA warpgroups =====================
-  const int wn = warp >> 2;                                  // column half
-  float acc[kAcc];
-  int s = 0;
-  uint32_t phase = 0, bphase = 0;
-  const int rw = (warp & 3) * 16 + (lane >> 2);              // fragment rows rw and rw + 8 of the tile
-  const int cw = wn * kWgCols + 2 * (lane & 3);              // + 8 j: columns c, c + 1 of n8 block j
-  float* bw = buf + rw * kLd + cw;
-  for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
-    ring.mma_tile<MODE>(s, phase, acc, 0, wn, num_kb, p.K);
-    // y = acc + (bias + resid) over the residual rows in the buffer; the pivot bias[0] + resid[row][0] of rows rw, rw + 8
-    mbar_wait(res_full, bphase);
-    if (cw == 0) { const float b0 = __ldg(p.bias); s_piv[rw] = b0 + bw[0]; s_piv[rw + 8] = b0 + bw[8 * kLd]; }
+  } else {
+    // ===================== MMA warpgroups =====================
+    const int wg = warp >> 2;                                // row half
+    float acc[kAcc];
+    int s = 0;
+    uint32_t phase = 0, bphase = 0;
+    const int rw = 64 * wg + (warp & 3) * 16 + (lane >> 2);  // fragment rows rw and rw + 8 of the tile
+    const int cw = 2 * (lane & 3);                           // + 8 j: columns c, c + 1 of n8 block j (of the CTA's)
+    const float* bias = p.bias + col0;
+    float* bw = buf + rw * kLd + cw;
+    int it = 0;                                              // the CTA's tile count: exchange slot it & 1
+    for (int t = cl; t < n_work; t += n_cl, ++it) {
+      const int m0 = tile_m0(t);
+      ring.template mma_tile<MODE>(s, phase, acc, wg, 0, num_kb, p.K);
+      // the pivot bias[0] + resid[row][0] of rows rw, rw + 8 (column 0 of y without the GEMM term)
+      float piv0 = 0.0f, piv1 = 0.0f;
+      if (cw == 0) {
+        const float b0 = __ldg(p.bias);
+        piv0 = b0 + p.resid[static_cast<size_t>(m0 + rw) * N];
+        piv1 = b0 + p.resid[static_cast<size_t>(m0 + rw + 8) * N];
+      }
+      piv0 = __shfl_sync(0xffffffffu, piv0, lane & ~3);
+      piv1 = __shfl_sync(0xffffffffu, piv1, lane & ~3);
+      // y = acc + (bias + resid) over the residual rows in the buffer.  The thread's columns 2 q + 8 j (q = lane % 4) are chain q
+      // of rows rw and rw + 8: it sums (y_c - piv) + (y_c+1 - piv), j ascending, as the statistics require
+      mbar_wait(res_full, bphase);
+      if (cw == 0) { s_piv[rw] = piv0; s_piv[rw + 8] = piv1; }
+      float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
-    for (int j = 0; j < kAcc / 4; ++j) {
-      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + cw + 8 * j));
-      float2* y0 = reinterpret_cast<float2*>(bw + 8 * j);
-      float2* y1 = reinterpret_cast<float2*>(bw + 8 * kLd + 8 * j);
-      const float2 r0 = *y0, r1 = *y1;
-      *y0 = make_float2(acc[4 * j] + (b.x + r0.x), acc[4 * j + 1] + (b.y + r0.y));
-      *y1 = make_float2(acc[4 * j + 2] + (b.x + r1.x), acc[4 * j + 3] + (b.y + r1.y));
+      for (int j = 0; j < kAcc / 4; ++j) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + cw + 8 * j));
+        float2* y0 = reinterpret_cast<float2*>(bw + 8 * j);
+        float2* y1 = reinterpret_cast<float2*>(bw + 8 * kLd + 8 * j);
+        const float2 r0 = *y0, r1 = *y1;
+        const float2 v0 = make_float2(acc[4 * j] + (b.x + r0.x), acc[4 * j + 1] + (b.y + r0.y));
+        const float2 v1 = make_float2(acc[4 * j + 2] + (b.x + r1.x), acc[4 * j + 3] + (b.y + r1.y));
+        *y0 = v0;
+        *y1 = v1;
+        s0 += (v0.x - piv0) + (v0.y - piv0);
+        s1 += (v1.x - piv1) + (v1.y - piv1);
+      }
+      s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+      s0 += __shfl_xor_sync(0xffffffffu, s0, 2);             // this half's sums of y - pivot of rows rw, rw + 8
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+      if (cw == 0) {
+        const int b = it & 1;
+        s_own[rw] = s0; s_own[rw + 8] = s1;
+        st_async_f32(px_sum + (b * kRows + rw) * 4, s0, pxs_full + b * 8);
+        st_async_f32(px_sum + (b * kRows + rw + 8) * 4, s1, pxs_full + b * 8);
+      }
+      fence_proxy_async_smem();                              // y is visible to the bulk store of y_out
+      mbar_arrive(buf_full);
+      bphase ^= 1;
     }
-    fence_proxy_async_smem();                                // y is visible to the bulk store of y_out
-    mbar_arrive(buf_full);
-    bphase ^= 1;
   }
+  cluster_sync();                                            // the peer stores nothing into this CTA's shared memory any more
 }
 
 }  // namespace ldm

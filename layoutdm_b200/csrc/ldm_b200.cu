@@ -51,12 +51,20 @@ constexpr int kRbCols = RbSmem::kCols;
 static_assert(kDModel <= RbSmem::kAKb * RbSmem::kKB && kAttN % kRbCols == 0 && kQkvN % 64 == 0 && 4 * kDModel % 64 == 0,
               "row-block GEMM shapes: K fits the resident A, Q tiles are whole tiles, N is whole 64-column store blocks");
 constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 (the padded logits row)
-// out-projection / FF2: 64 x 464 (whole rows, LayerNorm in the epilogue).  fp16 / bf16: gemm_ln_kernel (persistent, epilogue
-// warps, 32-element k-blocks: K = 512 and 1856 have no tail); the split mode: the fragment-epilogue kernel below
+// out-projection / FF2 (LayerNorm in the epilogue).  fp16 / bf16: gemm_ln_kernel (persistent CTA pairs, each pair one 128-row
+// block, each CTA 232 of its 464 columns; epilogue warps, 32-element k-blocks: K = 512 and 1856 have no tail); the split mode:
+// the fragment-epilogue kernel below, 64 x 464 tiles
 constexpr int kLnBN = 232, kLnStages = 3;
+constexpr int kLnSplitRows = 64;   // A box rows of the split mode's LN GEMMs (the one-plane kernel's: LnSmem<>::kRows)
+// ring stages of gemm_ln_kernel: FF2 (K = 1856) waits on its operand feed and takes the most that fit; the out-projection
+// (K = 512) waits on its epilogue, which measured faster beside the smaller shared-memory footprint of 3 stages (DESIGN §4)
+constexpr int kLnOutStages = 3, kLnFf2Stages = 4;
+using LnOut = LnSmem<kLnOutStages>;
+using LnFf2 = LnSmem<kLnFf2Stages>;
 // k-block of the LN GEMMs' operands (the TMA box columns) in every mode: the persistent kernel's, which is the split mode's
-constexpr int kLnKB = LnSmem::R::kKB;
-static_assert(LnSmem::kWgCols == kLnBN && kAttN % kLnKB == 0 && 4 * kDModel % kLnKB == 0 && gemm_kb(true) == kLnKB, "LN GEMM shapes");
+constexpr int kLnKB = LnFf2::R::kKB;
+static_assert(LnOut::R::kKB == kLnKB && LnFf2::kCols == kLnBN && LnFf2::kPairCols == kDModel && kAttN % kLnKB == 0 &&
+              4 * kDModel % kLnKB == 0 && gemm_kb(true) == kLnKB, "LN GEMM shapes");
 template <int EPI, int MODE> constexpr auto kGemmPlainSplit = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
 template <int MODE> constexpr auto kGemmLn = gemm_tc_kernel<kLnBN, 1, kLnStages, EPI_LN, MODE>;
@@ -149,7 +157,7 @@ struct LdmHandle {
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
-  CUtensorMap m_att16, m_hid16;                                              // 64-row boxes: A operands of the LN GEMMs
+  CUtensorMap m_att16, m_hid16;                                              // A operands of the LN GEMMs: 128-row boxes (split mode: 64)
   CUtensorMap m_qkv16_st, m_hid16_st;                                        // 128-row boxes: the row-block GEMMs' TMA stores (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
@@ -160,7 +168,9 @@ struct LdmHandle {
   int sweep = 1;               // env LDM_SWEEP=0: every kernel walks its row blocks in ascending order (no alternating directions)
   int num_sms = 0;             // the persistent GEMMs run at most one CTA per SM
   int max_threads_sm = 0;      // with num_sms: the launch policy of torch's distribution kernels (LDM_NOISE_TORCH)
-  int gemm_ctas = 0;           // env LDM_GEMM_CTAS=n (n >= 1): at most n CTAs in a persistent GEMM launch; 0: no cap
+  int gemm_ctas = 0;           // env LDM_GEMM_CTAS=n (n >= 1): at most n CTAs in a persistent GEMM launch (the LN GEMMs: max(1, n / 2)
+                               // CTA pairs); 0: no cap
+  int ln_clusters = 0;         // one-plane modes: the CTA pairs of gemm_ln_kernel that can be resident at once
   int gemm_split = 0;          // env LDM_GEMM_SPLIT=g (g >= 1): column ranges per row block of the row-block GEMMs; 0: automatic
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
                                // The split mode always launches it: the draw kernels write one 16-bit plane only
@@ -336,19 +346,26 @@ struct ProfScope {   // counts the launch; when profiling is on, brackets it wit
 // the kernel's CTAs may start while the previous kernel of the stream drains; every kernel calls pdl_sync() (griddepcontrol.wait
 // + launch_dependents) after its prologue and before its first dependent global access, so barrier init / descriptor prefetch /
 // parameter loads overlap the predecessor's tail and the launch latency disappears.
+// cluster > 1: clusters of that many consecutive CTAs along x (cudaLaunchAttributeClusterDimension).
 template <typename... KArgs, typename... Args>
-cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), dim3 grid, int block, int smem, cudaStream_t st, Args&&... args) {
+cudaError_t launch_cluster(const LdmHandle* h, int cluster, void (*kernel)(KArgs...), dim3 grid, int block, int smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
+  cudaLaunchAttribute at[2];
   cfg.attrs = at; cfg.numAttrs = 0;
-  if (h->pdl) { at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1; cfg.numAttrs = 1; }
+  if (h->pdl) { at[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[cfg.numAttrs++].val.programmaticStreamSerializationAllowed = 1; }
+  if (cluster > 1) { at[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension; at[cfg.numAttrs++].val.clusterDim = {static_cast<unsigned>(cluster), 1, 1}; }
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+template <typename... KArgs, typename... Args>
+cudaError_t launch_step(const LdmHandle* h, void (*kernel)(KArgs...), dim3 grid, int block, int smem, cudaStream_t st, Args&&... args) {
+  return launch_cluster(h, 1, kernel, grid, block, smem, st, std::forward<Args>(args)...);
+}
 
-// the dynamic shared memory of the kernels of MODE that use more than the default 48 KB
+// the dynamic shared memory of the kernels of MODE that use more than the default 48 KB; one-plane modes: how many CTA pairs of
+// gemm_ln_kernel can be resident at once (h->ln_clusters)
 template <int MODE>
-int set_smem() {
+int set_smem(LdmHandle* h) {
   constexpr auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
   if constexpr (kOpSplit<MODE>) {
     CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_QKV, MODE>, attr, kPlainSmem));
@@ -359,8 +376,21 @@ int set_smem() {
   }
   CK(cudaFuncSetAttribute(kGemmHead<MODE>, attr, kHeadSmem));
   if constexpr (kOpSplit<MODE>) CK(cudaFuncSetAttribute(kGemmLn<MODE>, attr, kLnSmem));
-  else CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE>, attr, LnSmem::kBytes));
+  else {
+    CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnOutStages>, attr, LnOut::kBytes));
+    CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnFf2Stages>, attr, LnFf2::kBytes));
+  }
   CK(cudaFuncSetAttribute(attention_kernel<MODE>, attr, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes));
+  if constexpr (!kOpSplit<MODE>) {
+    // the larger of the two: the out-projection's pairs fit wherever FF2's do (the same threads and registers, less shared memory)
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2); cfg.blockDim = dim3(kLnThreads); cfg.dynamicSmemBytes = LnFf2::kBytes;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {2, 1, 1};
+    cfg.attrs = at; cfg.numAttrs = 1;
+    CK(cudaOccupancyMaxActiveClusters(&h->ln_clusters, gemm_ln_kernel<MODE, kLnFf2Stages>, &cfg));
+    if (h->ln_clusters < 1) return fail(LDM_ERR_UNSUPPORTED, "gemm_ln_kernel: no CTA pair of %d bytes of shared memory fits the device", LnFf2::kBytes);
+  }
   return LDM_OK;
 }
 
@@ -425,8 +455,9 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   const int kb = gemm_kb(h->split);
   if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM, kb))) return rc;
   if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM, kb))) return rc;
-  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, 64, kLnKB))) return rc;
-  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, 64, kLnKB))) return rc;
+  const int ln_rows = h->split ? kLnSplitRows : LnFf2::kRows;
+  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, ln_rows, kLnKB))) return rc;
+  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, ln_rows, kLnKB))) return rc;
   // attention's Q / K / V head tiles: 128 rows x one padded head, in every mode
   if ((rc = make_op_maps(h, &h->m_qkv16, &h->m_qkv16_lo, h->qkv16, h->qkv16_lo, M, kQkvN, kBM, kHeadPad))) return rc;
   // the row-block GEMMs' stores: 64-column x 128-row boxes of the staging tile (128-byte swizzle)
@@ -463,11 +494,16 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       return launch_step(h, gemm_rowblock_kernel<EPI, MODE>, grid(n * p.n_ranges, true), kRbThreads, RbSmem::kBytes, st, a, w, out, p);
     }
   };
-  // the LN GEMMs (out-projection, FF2), 64 whole rows per tile: the fragment-epilogue kernel in the split mode, the persistent
-  // LN kernel otherwise
+  // the LN GEMMs (out-projection, FF2): the fragment-epilogue kernel in the split mode, 64 whole rows per tile; otherwise the
+  // persistent LN kernel, min(row blocks, resident pairs, LDM_GEMM_CTAS / 2) CTA pairs, each pair one row block at a time
   const auto ln_gemm = [&](const OpMaps<MODE>& a, const OpMaps<MODE>& w, const GemmParams& p) {
-    if constexpr (kOpSplit<MODE>) return launch_step(h, kGemmLn<MODE>, grid(M / 64, false), kGemmThreads, kLnSmem, st, a, w, p);
-    else return launch_step(h, gemm_ln_kernel<MODE>, grid(M / 64, true), kLnThreads, LnSmem::kBytes, st, a, w, p);
+    if constexpr (kOpSplit<MODE>) {
+      return launch_step(h, kGemmLn<MODE>, grid(M / kLnSplitRows, false), kGemmThreads, kLnSmem, st, a, w, p);
+    } else {
+      const int pairs = std::min({n, h->ln_clusters, h->gemm_ctas > 0 ? std::max(1, h->gemm_ctas / 2) : n});
+      if (p.K == kAttN) return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnOutStages>, dim3(2 * pairs), kLnThreads, LnOut::kBytes, st, a, w, p);
+      return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, p);
+    }
   };
   int done = 0;
   // alternating sweep direction: every kernel walks the row blocks opposite to its predecessor (GemmParams::rev); the embedding /
@@ -795,7 +831,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (cudaDeviceSynchronize() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(cudaGetLastError())); }
   free_staging(h);
 
-  TRY(h->mode == OP_BF16X3 ? set_smem<OP_BF16X3>() : h->mode == OP_BF16 ? set_smem<OP_BF16>() : set_smem<OP_F16>());
+  TRY(h->mode == OP_BF16X3 ? set_smem<OP_BF16X3>(h) : h->mode == OP_BF16 ? set_smem<OP_BF16>(h) : set_smem<OP_F16>(h));
 #undef TRY
   *out = h;
   return LDM_OK;
