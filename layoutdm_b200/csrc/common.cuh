@@ -80,18 +80,6 @@ LDM_DEVINL void tma_store_2d(const CUtensorMap* map, const void* smem_src, int32
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
 }
-// 1-D bulk copies of a contiguous range (bytes a multiple of 16, both addresses 16-byte aligned): global -> shared with
-// completion on an mbarrier, shared -> global tracked in this thread's bulk groups
-LDM_DEVINL void bulk_copy_g2s(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-LDM_DEVINL void bulk_copy_s2g(void* dst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-               ::"l"(reinterpret_cast<uint64_t>(dst)), "r"(smem_u32(smem_src)), "r"(bytes)
-               : "memory");
-}
 LDM_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's bulk groups still reading their shared-memory source
 template <int N>

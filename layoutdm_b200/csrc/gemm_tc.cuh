@@ -572,81 +572,116 @@ gemm_rowblock_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 r
 // 232 h .. 232 h + 231 of all 128 rows, so every weight k-block it streams from L2 feeds 128 rows (FF2 reads 1.34 MB per CTA
 // tile against 1.96 MB for a 64 x 464 tile of the same floats).  Clusters: min(row blocks, active clusters); cluster c runs the
 // row blocks c, c + clusters, ...  384 threads per CTA.  The LayerNorm runs in warps of its own and the fp32 traffic goes
-// through bulk copies, so a tile's epilogue overlaps the next tile's MMAs:
+// through TMA, so a tile's epilogue overlaps the next tile's MMAs:
 //   warps 0..7  : two MMA warpgroups, warpgroup w rows 64 w .. 64 w + 63 x the CTA's 232 columns, m64n232k16 from the ring.
-//                 After a tile's last k-block they wait for the tile's residual half rows in the tile buffer, replace them by
-//                 y = acc + (bias + resid), send the rows' sums of y - pivot (below) and go straight on to the next tile.
-//   warps 8..10 : epilogue: the row statistics, the LayerNorm / AdaLN and the 16-bit stores from the tile buffer.  Warp 8
-//                 also issues the bulk copies of half rows (928 bytes at byte offset 928 h) between the buffer and global
-//                 memory: y out (the next residual), the normalised fp32 rows (written back into the buffer) out, and the next
-//                 tile's residual rows in.
+//                 After a tile's last k-block warpgroup w waits for the residual rows of its row half w in the tile buffer,
+//                 replaces them by y = acc + (bias + resid), sends the rows' sums of y - pivot (below) and goes straight on
+//                 to the next tile.
+//   warps 8..10 : epilogue: the row statistics, the LayerNorm / AdaLN and the 16-bit stores from the tile buffer, one row half
+//                 at a time: (tile t, half 0), (t, 1), (t + 1, 0), ...  Thread 0 of warp 8 also moves the fp32 row halves
+//                 between the buffer and global memory, one 2-D TMA box of 64 rows x the CTA's 232 columns each (map_res,
+//                 map_st; no swizzle, so a box is the half's dense [64][232] rows): the half's y out (the next residual) or
+//                 its normalised fp32 rows (written back into the buffer) out -- the host sets at most one of the two, so
+//                 the normalise pass never overwrites rows a store still reads -- and, as soon as that store has read the
+//                 half, the next tile's residual rows of the same half in.  So the load of half w and warpgroup w's y pass
+//                 run while the epilogue works on the other half.
 //   warp 11     : producer, one lane issues the TMA loads.
+// The tile buffer is two row halves, [2][64][232] fp32, each with its own barriers: res_full[w] (its residual rows have
+// landed; armed by the copying thread), buf_full[w] (warpgroup w wrote y; 128 arrivals).  A half is free again once the copying
+// thread's wait_group.read of its store returns after the named barrier that ends the epilogue's pass over it; that thread
+// loads the half's next residual rows only then, so the hand-off is program order in one thread.  Both warpgroups consume every ring
+// stage, so one can run at most the ring's depth ahead of the other.
 // 168 registers for every warp, no setmaxnreg: ptxas compiles the whole kernel under the launch bound's register count, and a
 // 512-thread block (a whole producer warpgroup) would leave the m64n232 wgmma 128, fewer than it needs.  Three epilogue warps
-// cannot keep enough loads and stores in flight to move a tile's fp32 rows at HBM rate themselves; the bulk copies need no
+// cannot keep enough loads and stores in flight to move a tile's fp32 rows at HBM rate themselves; the TMA copies need no
 // registers.  Ring: STAGES stages of 32-element k-blocks with the 64-byte swizzle (8 KB of A + 14.5 KB of W each) beside the
-// 116 KB tile buffer; 4 fit.  The split mode keeps the fragment-epilogue kernel above: its two-plane stages do not fit beside the buffer.
+// 116 KB tile buffer; 4 fit.  (With one 1-D bulk copy per 928-byte row, issuing a half's 64 loads took warp 8 about 2 us per
+// row half (H100 SXM), on the epilogue's critical path.)  The split mode keeps the fragment-epilogue kernel above: its two-plane stages do not fit beside the buffer.
 //
 // The results are bit for bit those of the fragment epilogue: the same k16 MMA sequence, y = acc + (bias + resid), and the row
 // statistics keep its summation order (per row 8 chains (h, q), h = column half, q = quad lane, each summing
 // (y_c - piv) + (y_c+1 - piv) over c = 232 h + 8 j + 2 q, j ascending; (q0 + q1) + (q2 + q3), then half + half) and its FMA
 // contractions (y - mean is one fma(-sum, 1/N, y - piv), the output fma(d * rstd, gamma + gadd, beta)).  The pivot is
-// bias[0] + resid[row][0] in both CTAs, read from global memory (rank 1 does not hold column 0).  Half h of a row lives in
-// CTA h: each CTA forms its half's quad-combined partial, stores it into the peer's slot with st.async (completion counted on
-// the peer's mbarrier) and adds the two, own + peer -- the same float in both CTAs, since addition commutes.  The row sums
+// bias[0] + resid[row][0] in both CTAs, read from global memory (rank 1 does not hold column 0).  Column half h of a row lives
+// in CTA h: each CTA forms its half's quad-combined partial, stores it into the peer's slot with st.async (completion counted
+// on the peer's mbarrier) and adds the two, own + peer -- the same float in both CTAs, since addition commutes.  The row sums
 // are formed by the MMA warpgroups from y in registers (a fragment thread's columns 2 q + 8 j are exactly chain q) and sent
 // before the epilogue starts, so the epilogue reads the buffer once for the statistics, not twice, and rarely waits for
 // the peer's sums.  The epilogue warps form and exchange the sums of squared deviations the same way.
-// Exchange slots: two per statistic, by tile parity, each with an mbarrier that its own CTA arms (expect_tx) in the tile
-// that uses it; the peer's bytes may land before that, which the transaction count allows.  The peer writes slot b for tile
-// i + 2 only once it holds this CTA's variance partials of tile i + 1 (its MMA warpgroups send the sums of tile i + 2 after
-// its epilogue has finished tile i + 1 and loaded the residual rows of tile i + 2), and those partials are sent after every
-// epilogue thread of this CTA has passed the named barriers that end tile i, so after every read of slot b for tile i: two
-// slots cannot be overrun.
+// Exchange slots: two per statistic, by tile parity b, indexed by row; each (b, row half w) has an mbarrier that its own CTA
+// arms (expect_tx) when its epilogue starts on half w of a tile of parity b; the peer's bytes may land before that, which the
+// transaction count allows.  Overrun: the peer writes the row-sum slots (b, w) for tile i + 2 from its warpgroup w after that
+// half's residual rows of tile i + 2 have landed, which its warp 8 loads only after its epilogue has finished (i + 1, w), and
+// that needed this CTA's variance partials of (i + 1, w).  It writes the variance slots (b, w) for tile i + 2 in its
+// epilogue's pass over (i + 2, w), which comes after (i + 1, w) as well.  This CTA sends its partials of (i + 1, w) only after
+// every epilogue thread has passed the named barriers that end (i, w) (and (i, 1 - w)), so after every read of the slots
+// (b, w) for tile i: two slots cannot be overrun.
 // Cluster barriers: after the barrier init (no remote store before the peer's barriers exist) and before exit (no CTA leaves
 // while its peer may still store into its shared memory); every thread reaches both.
 constexpr int kLnThreads = 384, kLnEpiThreads = 96;
+
+// Phase probe (tools/ln_phase_probe.py), compiled in only with -DLDM_LN_PROBE: rank 0 of the first kLnProbePairs pairs records
+// %globaltimer stamps per tile and row half; each launch overwrites its GEMM's entries, so after a step they hold the
+// step's last out-projection (K = 512) and last FF2 launch.
+enum : int { LNP_MAIN = 0, LNP_RES, LNP_Y, LNP_BUF, LNP_XS, LNP_XV, LNP_NORM, LNP_WAIT, LNP_NEXT, LNP_N };
+constexpr int kLnProbePairs = 8, kLnProbeTiles = 32;
+#ifdef LDM_LN_PROBE
+__device__ unsigned long long g_ln_probe[2][kLnProbePairs][kLnProbeTiles][2][LNP_N];
+#endif
+LDM_DEVINL void ln_probe(int K, uint32_t rank, int cl, int it, int half, int stamp) {
+#ifdef LDM_LN_PROBE
+  if (rank == 0 && cl < kLnProbePairs && it < kLnProbeTiles) {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    g_ln_probe[K == 512 ? 0 : 1][cl][it][half][stamp] = t;
+  }
+#endif
+}
+
 template <int STAGES>
 struct LnSmem {
-  static constexpr int kRows = kBM, kCols = 232, kPairCols = 2 * kCols;
+  static constexpr int kRows = kBM, kHalf = kRows / 2, kCols = 232, kPairCols = 2 * kCols;
   using R = Ring<32, 1, kRows, kCols, 1, STAGES, false>;       // K = 512, 1856 (checked at create)
-  // tile buffer [128][kLd] fp32, unpadded: a row is 928 bytes = 32 mod 128, so the 4 rows of a half warp's fragment access fall in
-  // distinct 32-byte bank groups, and every row is 16-byte aligned for the bulk copies
+  // tile buffer [2 row halves][64][kLd] fp32, unpadded: a row is 928 bytes = 32 mod 128, so the 4 rows of a half warp's fragment
+  // access fall in distinct 32-byte bank groups; a half is one TMA box (rows of 16-byte multiples, 128-byte aligned start)
   static constexpr int kLd = kCols;
   static constexpr int kOffBuf = R::kBytes;
-  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;      // ring full[4], empty[4]; res_full, buf_full; xs_full[2], xv_full[2]
-  static constexpr int kOffStat = kOffBars + 128;
-  // per row: pivot, own half's sum of y - pivot, row sum, own half's sum of squared deviations, rstd; the peer's partials [2][kRows] x 2
-  static constexpr int kBytes = kOffStat + 9 * kRows * 4 + 1024 /*align slack*/;
-  static_assert(2 * R::kStages * 8 + 6 * 8 <= 128, "barrier block overflow");
-  static_assert(kLd * 4 % 16 == 0 && kLd * 4 % 128 == 32, "bulk copies need 16-byte aligned rows; fragment accesses need rows 32 mod 128 bytes");
-  static_assert(kRows * kCols * 4 < (1 << 20), "a tile's residual bytes exceed the mbarrier transaction count");
+  // ring full[4], empty[4]; res_full[2], buf_full[2]; xs_full[2][2], xv_full[2][2]
+  static constexpr int kOffBars = kOffBuf + kRows * kLd * 4;
+  static constexpr int kOffStat = kOffBars + 256;
+  // per row: pivot, own half's sum of y - pivot, row sum, own half's sum of squared deviations (then rstd); the peer's partials
+  // [2][kRows] x 2
+  static constexpr int kBytes = kOffStat + 8 * kRows * 4 + 1024 /*align slack*/;
+  static_assert(2 * R::kStages * 8 + 12 * 8 <= 256, "barrier block overflow");
+  static_assert(kLd * 4 % 16 == 0 && kHalf * kLd * 4 % 128 == 0 && kLd * 4 % 128 == 32,
+                "TMA boxes need 16-byte multiple rows and 128-byte aligned halves; fragment accesses need rows 32 mod 128 bytes");
+  static_assert(kHalf * kCols * 4 < (1 << 20), "a row half's residual bytes exceed the mbarrier transaction count");
 };
 
 template <int MODE, int STAGES>
 __global__ void __launch_bounds__(kLnThreads, 1)
 gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 232 rows*/,
-               const GemmParams p) {
+               const __grid_constant__ CUtensorMap map_res /*p.resid, fp32, box 232 x 64 rows*/,
+               const __grid_constant__ CUtensorMap map_st /*p.y_out or p.out32, whichever is set*/, const GemmParams p) {
   static_assert(!kOpSplit<MODE>, "the split mode runs the fragment-epilogue LN GEMM");
   using SM = LnSmem<STAGES>;
   using O = OpT<MODE>;
-  constexpr int kRows = SM::kRows, kCols = SM::kCols, kLd = SM::kLd, kAcc = kCols / 2;
+  constexpr int kRows = SM::kRows, kHalf = SM::kHalf, kCols = SM::kCols, kLd = SM::kLd, kAcc = kCols / 2;
   constexpr int kEpi = kGemmConsumers, kProducer = kEpi + kLnEpiThreads;   // first thread of the epilogue warps / producer warp
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   typename SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
-  uint64_t* res_full = ring.empty + SM::R::kStages;             // the tile's residual rows have landed in the buffer
-  uint64_t* buf_full = res_full + 1;                             // the MMA warpgroups wrote y into the buffer
-  uint64_t* xs_full = buf_full + 1;                              // [2] the peer's row sums of tile parity b have landed
-  uint64_t* xv_full = xs_full + 2;                               // [2] the peer's sums of squared deviations
+  uint64_t* res_full = ring.empty + SM::R::kStages;             // [2] row half w's residual rows have landed in the buffer
+  uint64_t* buf_full = res_full + 2;                             // [2] MMA warpgroup w wrote y into row half w
+  uint64_t* xs_full = buf_full + 2;                              // [2 b][2 w] the peer's row sums of tile parity b, row half w have landed
+  uint64_t* xv_full = xs_full + 4;                               // [2][2] the peer's sums of squared deviations
   float* buf = reinterpret_cast<float*>(smem + SM::kOffBuf);
   float* s_piv = reinterpret_cast<float*>(smem + SM::kOffStat);
   float* s_own = s_piv + kRows;
   float* s_sum = s_own + kRows;
-  float* v_own = s_sum + kRows;
-  float* s_rstd = v_own + kRows;
-  float* x_sum = s_rstd + kRows;                                 // [2][kRows] written by the peer
+  float* s_var = s_sum + kRows;                                  // own half's sum of squared deviations, then the row's rstd
+  float* x_sum = s_var + kRows;                                  // [2][kRows] written by the peer
   float* x_var = x_sum + 2 * kRows;                              // [2][kRows] written by the peer
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -662,10 +697,11 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
 
   if (threadIdx.x == kProducer) {
     ring.prefetch(map_a, map_b);
+    tma_prefetch_desc(&map_res);
+    tma_prefetch_desc(&map_st);
     ring.init();
-    mbar_init(res_full, 1);
-    mbar_init(buf_full, kGemmConsumers);
-    for (int b = 0; b < 2; ++b) { mbar_init(&xs_full[b], 1); mbar_init(&xv_full[b], 1); }
+    for (int w = 0; w < 2; ++w) { mbar_init(&res_full[w], 1); mbar_init(&buf_full[w], kGemmConsumers / 2); }
+    for (int x = 0; x < 4; ++x) { mbar_init(&xs_full[x], 1); mbar_init(&xv_full[x], 1); }
     fence_mbar_init();
   }
   cluster_sync();                                            // both CTAs' barriers are initialised before any remote store
@@ -681,98 +717,106 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
   } else if (threadIdx.x >= kEpi) {
     // ===================== epilogue warps =====================
     const int et = threadIdx.x - kEpi;
-    const bool copier = et < 32;                             // warp 8: the bulk copies, one half row per lane at a time
-    constexpr uint32_t kRowBytes = kCols * sizeof(float);
+    const bool copier = et == 0;                             // the row halves' TMA loads and stores
+    constexpr uint32_t kHalfBytes = kHalf * kCols * sizeof(float);
     const float inv_n = 1.0f / static_cast<float>(N);
-    constexpr int kVec = kCols / 4;                          // float4 columns of a half row (58)
-    constexpr int kTotal = kRows * kVec;                     // float4 of a tile; element i = k * 96 + et
+    constexpr int kVec = kCols / 4;                          // float4 columns of the CTA's part of a row (58)
+    constexpr int kTotal = kHalf * kVec;                     // float4 of a row half; element i = k * 96 + et
     constexpr int kPerThread = (kTotal + kLnEpiThreads - 1) / kLnEpiThreads;
     const uint32_t px_var = map_peer(x_var, peer), pxv_full = map_peer(xv_full, peer);
-    // the residual half rows of tile t into the buffer (the buffer is free: every read of it and every bulk store from it is done)
-    const auto load_resid = [&](int t) {
-      if (lane == 0) mbar_arrive_expect_tx(res_full, kRows * kRowBytes);
-      __syncwarp();
-      const float* src = p.resid + static_cast<size_t>(tile_m0(t)) * N + col0;
-      for (int r = lane; r < kRows; r += 32) bulk_copy_g2s(buf + r * kLd, src + static_cast<size_t>(r) * N, kRowBytes, res_full);
+    // the residual rows of row half w of tile t into the buffer (the half is free: every read of it and every store from it is
+    // done)
+    const auto load_resid = [&](int t, int w) {
+      mbar_arrive_expect_tx(&res_full[w], kHalfBytes);
+      tma_load_2d(buf + kHalf * w * kLd, &map_res, &res_full[w], col0, tile_m0(t) + kHalf * w);
     };
-    const auto store_rows = [&](float* dst) {                // the buffer's half rows to dst, one bulk group per lane
-      for (int r = lane; r < kRows; r += 32) bulk_copy_s2g(dst + static_cast<size_t>(r) * N, buf + r * kLd, kRowBytes);
+    const auto store_rows = [&](int m0, int w) {             // row half w of the buffer to map_st's rows of tile m0, one bulk group
+      tma_store_2d(&map_st, buf + kHalf * w * kLd, col0, m0 + kHalf * w);
       bulk_commit_group();
     };
-    if (copier) load_resid(cl);
+    if (copier) { load_resid(cl, 0); load_resid(cl, 1); }
     uint32_t bphase = 0;
     int it = 0;                                              // the CTA's tile count: exchange slot it & 1, its pass (it >> 1) & 1
     for (int t = cl; t < n_work; t += n_cl, ++it) {
       const int m0 = tile_m0(t), b = it & 1;
       const uint32_t xph = (it >> 1) & 1;
-      if (et == 0) { mbar_arrive_expect_tx(&xs_full[b], kRows * 4); mbar_arrive_expect_tx(&xv_full[b], kRows * 4); }
-      mbar_wait(buf_full, bphase);
-      if (copier && p.y_out != nullptr) store_rows(p.y_out + static_cast<size_t>(m0) * N + col0);
-      // the sums of squared deviations, a group of 8 rows per warp at a time; lane = 4 row + q owns chain q of its row's half.
-      // The row sums came with y: this half's from the MMA warpgroups (s_own), the other's from the peer's
-      const int q = lane & 3;
-      mbar_wait(&xs_full[b], xph);
-#pragma unroll 1
-      for (int g = et >> 5; g < kRows / 8; g += kLnEpiThreads / 32) {
-        const int r = 8 * g + (lane >> 2);
-        const float piv = s_piv[r], s = s_own[r] + x_sum[b * kRows + r];   // the row sum of y - pivot; mean - pivot = s / N
-        const float* yr = buf + r * kLd + 2 * q;
-        float v = 0.0f;
-#pragma unroll
-        for (int j = 0; j < kCols / 8; ++j) {
-          const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
-          const float d0 = fmaf(-s, inv_n, y.x - piv), d1 = fmaf(-s, inv_n, y.y - piv);
-          v = fmaf(d0, d0, fmaf(d1, d1, v));
-        }
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        if (q == 0) { s_sum[r] = s; v_own[r] = v; st_async_f32(px_var + (b * kRows + r) * 4, v, pxv_full + b * 8); }
-      }
-      mbar_wait(&xv_full[b], xph);
-      if (q == 0) {                                          // the rows whose partials this lane sent
-#pragma unroll 1
-        for (int g = et >> 5; g < kRows / 8; g += kLnEpiThreads / 32) {
-          const int r = 8 * g + (lane >> 2);
-          s_rstd[r] = 1.0f / sqrtf(fmaxf((v_own[r] + x_var[b * kRows + r]) * inv_n, 0.0f) + 1e-5f);
-        }
-      }
-      if (copier) bulk_wait_group_read<0>();                 // the y rows are out of the buffer before it is overwritten
-      named_bar_sync(1, kLnEpiThreads);
-      // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a bulk store
       const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
       const float *gam = a.gam + col0, *bet = a.bet + col0;
       typename O::T* out16 = static_cast<typename O::T*>(p.out) + col0;
       const bool keep32 = p.out32 != nullptr;
+#pragma unroll 1
+      for (int w = 0; w < 2; ++w) {
+        const int h0 = kHalf * w, x = 2 * b + w;             // the half's first row; its exchange barriers
+        if (et == 0) { mbar_arrive_expect_tx(&xs_full[x], kHalf * 4); mbar_arrive_expect_tx(&xv_full[x], kHalf * 4); }
+        mbar_wait(&buf_full[w], bphase);
+        if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_BUF);
+        if (copier && p.y_out != nullptr) store_rows(m0, w);
+        // the sums of squared deviations, a group of 8 rows per warp at a time; lane = 4 row + q owns chain q of its row's half.
+        // The row sums came with y: this half's from the MMA warpgroups (s_own), the other's from the peer's
+        const int q = lane & 3;
+        mbar_wait(&xs_full[x], xph);
+        if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_XS);
+#pragma unroll 1
+        for (int g = et >> 5; g < kHalf / 8; g += kLnEpiThreads / 32) {
+          const int r = h0 + 8 * g + (lane >> 2);
+          const float piv = s_piv[r], s = s_own[r] + x_sum[b * kRows + r];   // the row sum of y - pivot; mean - pivot = s / N
+          const float* yr = buf + r * kLd + 2 * q;
+          float v = 0.0f;
+#pragma unroll
+          for (int j = 0; j < kCols / 8; ++j) {
+            const float2 y = *reinterpret_cast<const float2*>(yr + 8 * j);
+            const float d0 = fmaf(-s, inv_n, y.x - piv), d1 = fmaf(-s, inv_n, y.y - piv);
+            v = fmaf(d0, d0, fmaf(d1, d1, v));
+          }
+          v += __shfl_xor_sync(0xffffffffu, v, 1);
+          v += __shfl_xor_sync(0xffffffffu, v, 2);
+          if (q == 0) { s_sum[r] = s; s_var[r] = v; st_async_f32(px_var + (b * kRows + r) * 4, v, pxv_full + x * 8); }
+        }
+        mbar_wait(&xv_full[x], xph);
+        if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_XV);
+        if (q == 0) {                                        // the rows whose partials this lane sent
+#pragma unroll 1
+          for (int g = et >> 5; g < kHalf / 8; g += kLnEpiThreads / 32) {
+            const int r = h0 + 8 * g + (lane >> 2);
+            s_var[r] = 1.0f / sqrtf(fmaxf((s_var[r] + x_var[b * kRows + r]) * inv_n, 0.0f) + 1e-5f);
+          }
+        }
+        named_bar_sync(1, kLnEpiThreads);
+        // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a TMA store
 #pragma unroll 6
-      for (int k = 0; k < kPerThread; ++k) {
-        const int i = k * kLnEpiThreads + et, r = i / kVec, c = (i - r * kVec) * 4;
-        if (i >= kTotal) continue;
-        float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
-        const float4 y = *bp;
-        const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), h = __ldg(reinterpret_cast<const float4*>(bet + c));
-        const float piv = s_piv[r], s = s_sum[r], rstd = s_rstd[r];
-        const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, h.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, h.y),
-                                     fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, h.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, h.w));
-        *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
-        if (keep32) *bp = v;
-      }
-      if (keep32) fence_proxy_async_smem();                  // the fp32 rows are visible to the bulk store
-      named_bar_sync(1, kLnEpiThreads);
-      if (copier) {
-        if (keep32) store_rows(p.out32 + static_cast<size_t>(m0) * N + col0);
-        bulk_wait_group_read<0>();
-        if (t + n_cl < n_work) load_resid(t + n_cl);
+        for (int k = 0; k < kPerThread; ++k) {
+          const int i = k * kLnEpiThreads + et, r = h0 + i / kVec, c = (i - (r - h0) * kVec) * 4;
+          if (i >= kTotal) continue;
+          float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
+          const float4 y = *bp;
+          const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), h = __ldg(reinterpret_cast<const float4*>(bet + c));
+          const float piv = s_piv[r], s = s_sum[r], rstd = s_var[r];
+          const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, h.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, h.y),
+                                       fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, h.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, h.w));
+          *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
+          if (keep32) *bp = v;
+        }
+        if (keep32) fence_proxy_async_smem();                // the fp32 rows are visible to the TMA store
+        named_bar_sync(1, kLnEpiThreads);
+        if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_NORM);
+        if (copier) {
+          if (keep32) store_rows(m0, w);
+          bulk_wait_group_read<0>();
+          if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_WAIT);
+          if (t + n_cl < n_work) load_resid(t + n_cl, w);
+          if (et == 0) ln_probe(p.K, rank, cl, it, w, LNP_NEXT);
+        }
       }
       bphase ^= 1;
     }
-    if (copier) bulk_wait_group_all();                       // the last bulk stores are complete before the CTA exits
+    if (copier) bulk_wait_group_all();                       // the last TMA stores are complete before the CTA exits
   } else {
     // ===================== MMA warpgroups =====================
     const int wg = warp >> 2;                                // row half
     float acc[kAcc];
     int s = 0;
     uint32_t phase = 0, bphase = 0;
-    const int rw = 64 * wg + (warp & 3) * 16 + (lane >> 2);  // fragment rows rw and rw + 8 of the tile
+    const int rw = kHalf * wg + (warp & 3) * 16 + (lane >> 2);   // fragment rows rw and rw + 8 of the tile
     const int cw = 2 * (lane & 3);                           // + 8 j: columns c, c + 1 of n8 block j (of the CTA's)
     const float* bias = p.bias + col0;
     float* bw = buf + rw * kLd + cw;
@@ -780,6 +824,7 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
     for (int t = cl; t < n_work; t += n_cl, ++it) {
       const int m0 = tile_m0(t);
       ring.template mma_tile<MODE>(s, phase, acc, wg, 0, num_kb, p.K);
+      if (threadIdx.x % 128 == 0) ln_probe(p.K, rank, cl, it, wg, LNP_MAIN);
       // the pivot bias[0] + resid[row][0] of rows rw, rw + 8 (column 0 of y without the GEMM term)
       float piv0 = 0.0f, piv1 = 0.0f;
       if (cw == 0) {
@@ -789,9 +834,10 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
       }
       piv0 = __shfl_sync(0xffffffffu, piv0, lane & ~3);
       piv1 = __shfl_sync(0xffffffffu, piv1, lane & ~3);
-      // y = acc + (bias + resid) over the residual rows in the buffer.  The thread's columns 2 q + 8 j (q = lane % 4) are chain q
-      // of rows rw and rw + 8: it sums (y_c - piv) + (y_c+1 - piv), j ascending, as the statistics require
-      mbar_wait(res_full, bphase);
+      // y = acc + (bias + resid) over the half's residual rows in the buffer.  The thread's columns 2 q + 8 j (q = lane % 4)
+      // are chain q of rows rw and rw + 8: it sums (y_c - piv) + (y_c+1 - piv), j ascending, as the statistics require
+      mbar_wait(&res_full[wg], bphase);
+      if (threadIdx.x % 128 == 0) ln_probe(p.K, rank, cl, it, wg, LNP_RES);
       if (cw == 0) { s_piv[rw] = piv0; s_piv[rw + 8] = piv1; }
       float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
@@ -812,13 +858,14 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
       s0 += __shfl_xor_sync(0xffffffffu, s0, 2);             // this half's sums of y - pivot of rows rw, rw + 8
       s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
       if (cw == 0) {
-        const int b = it & 1;
+        const int b = it & 1, x = 2 * b + wg;
         s_own[rw] = s0; s_own[rw + 8] = s1;
-        st_async_f32(px_sum + (b * kRows + rw) * 4, s0, pxs_full + b * 8);
-        st_async_f32(px_sum + (b * kRows + rw + 8) * 4, s1, pxs_full + b * 8);
+        st_async_f32(px_sum + (b * kRows + rw) * 4, s0, pxs_full + x * 8);
+        st_async_f32(px_sum + (b * kRows + rw + 8) * 4, s1, pxs_full + x * 8);
       }
-      fence_proxy_async_smem();                              // y is visible to the bulk store of y_out
-      mbar_arrive(buf_full);
+      fence_proxy_async_smem();                              // y is visible to the TMA store of y_out
+      mbar_arrive(&buf_full[wg]);
+      if (threadIdx.x % 128 == 0) ln_probe(p.K, rank, cl, it, wg, LNP_Y);
       bphase ^= 1;
     }
   }

@@ -106,6 +106,19 @@ int make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uin
   return LDM_OK;
 }
 
+// 2-D row-major [rows][cols] fp32 tensor, box = box_rows x box_cols, no swizzle: a box lands as dense [box_rows][box_cols] rows
+int make_map_f32(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols) {
+  const cuuint64_t dims[2] = {cols, rows};
+  const cuuint64_t strides[1] = {cols * 4};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(LDM_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) fp32 rows=%llu cols=%llu box %u x %u", (int)r,
+                                     (unsigned long long)rows, (unsigned long long)cols, box_rows, box_cols);
+  return LDM_OK;
+}
+
 // (B,S,C) contiguous <-> padded internal logits [B*128][160]
 __global__ void logits_scatter_kernel(const float* __restrict__ src, float* __restrict__ dst, int n_layouts, int S, int C) {
   const size_t n = static_cast<size_t>(n_layouts) * S * C;
@@ -159,6 +172,7 @@ struct LdmHandle {
   CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
   CUtensorMap m_att16, m_hid16;                                              // A operands of the LN GEMMs: 128-row boxes (split mode: 64)
   CUtensorMap m_qkv16_st, m_hid16_st;                                        // 128-row boxes: the row-block GEMMs' TMA stores (one-plane modes)
+  CUtensorMap m_x32, m_y32;                                                  // 64 x 232 fp32 boxes: the LN GEMMs' row halves (one-plane modes)
   void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
   CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
@@ -463,6 +477,9 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   // the row-block GEMMs' stores: 64-column x 128-row boxes of the staging tile (128-byte swizzle)
   if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, kBM, 64, h->bf16))) return rc;
   if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16, M, ff, kBM, 64, h->bf16))) return rc;
+  // the persistent LN GEMMs' residual loads and fp32 stores: one row half of the CTA's columns per box
+  if (!h->split && (rc = make_map_f32(&h->m_x32, h->x32, M, d, LnFf2::kHalf, kLnBN))) return rc;
+  if (!h->split && (rc = make_map_f32(&h->m_y32, h->y32, M, d, LnFf2::kHalf, kLnBN))) return rc;
   return LDM_OK;
 }
 
@@ -496,13 +513,14 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   };
   // the LN GEMMs (out-projection, FF2): the fragment-epilogue kernel in the split mode, 64 whole rows per tile; otherwise the
   // persistent LN kernel, min(row blocks, resident pairs, LDM_GEMM_CTAS / 2) CTA pairs, each pair one row block at a time
-  const auto ln_gemm = [&](const OpMaps<MODE>& a, const OpMaps<MODE>& w, const GemmParams& p) {
+  // res / st: the fp32 maps of p.resid and of p.y_out or p.out32 (the one that is set; at most one is)
+  const auto ln_gemm = [&](const OpMaps<MODE>& a, const OpMaps<MODE>& w, const CUtensorMap& res, const CUtensorMap& st32, const GemmParams& p) {
     if constexpr (kOpSplit<MODE>) {
       return launch_step(h, kGemmLn<MODE>, grid(M / kLnSplitRows, false), kGemmThreads, kLnSmem, st, a, w, p);
     } else {
       const int pairs = std::min({n, h->ln_clusters, h->gemm_ctas > 0 ? std::max(1, h->gemm_ctas / 2) : n});
-      if (p.K == kAttN) return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnOutStages>, dim3(2 * pairs), kLnThreads, LnOut::kBytes, st, a, w, p);
-      return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, p);
+      if (p.K == kAttN) return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnOutStages>, dim3(2 * pairs), kLnThreads, LnOut::kBytes, st, a, w, res, st32, p);
+      return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, res, st32, p);
     }
   };
   int done = 0;
@@ -537,7 +555,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
       p.rev = next_rev(); p.out_lo = h->z16_lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(ln_gemm(maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), p));
+      CK(ln_gemm(maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), h->m_x32, h->m_y32, p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
@@ -558,7 +576,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(ln_gemm(maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), p));
+      CK(ln_gemm(maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), h->m_y32, h->m_x32, p));
     }
     LDM_STAGE_DONE();
   }
@@ -1252,6 +1270,17 @@ int ldm_profile_end(LdmHandle* h, float* ms_per_category, int64_t* launches_per_
   h->prof_recs.clear();
   return LDM_OK;
 }
+
+#ifdef LDM_LN_PROBE
+// the LN GEMMs' phase stamps (gemm_tc.cuh, ln_probe) since the last call, then cleared; returns the bytes copied, or -1
+int64_t ldm_probe_ln_read(void* dst, int64_t capacity_bytes) {
+  const int64_t bytes = sizeof(g_ln_probe);
+  if (!dst || capacity_bytes < bytes) return -1;
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(dst, g_ln_probe, bytes) != cudaSuccess) return -1;
+  static const unsigned char zeros[sizeof(g_ln_probe)] = {};
+  return cudaMemcpyToSymbol(g_ln_probe, zeros, bytes) == cudaSuccess ? bytes : -1;
+}
+#endif
 
 int ldm_debug_set_stop_after(LdmHandle* h, int32_t n_launches) {
   if (!h) return fail(LDM_ERR_INVALID, "null handle");
