@@ -140,12 +140,26 @@ __global__ void fill_ids_kernel(long long* dst, long long v, size_t n) {
 
 }  // namespace
 
+// one 16-bit operand: its hi plane, its lo plane in the split mode (nullptr otherwise), and their tensor maps
+struct Op16 {
+  void* hi = nullptr;
+  void* lo = nullptr;
+  CUtensorMap map, map_lo;
+  template <int MODE>
+  OpMaps<MODE> maps() const {
+    OpMaps<MODE> m;
+    m.hi = map;
+    if constexpr (kOpSplit<MODE>) m.lo = map_lo;
+    return m;
+  }
+};
+
 struct LdmHandle {
   LdmModelDesc desc;
   int C = 0, S = 0, L = 0, T = 0, G = 0;
   int mode = OP_F16;          // operand mode (LdmModelDesc::operand_dtype)
   bool bf16 = false;          // bf16 operand data (OP_BF16, OP_BF16X3)
-  bool split = false;         // OP_BF16X3: every 16-bit weight and activation buffer has a lo plane (the *_lo members)
+  bool split = false;         // OP_BF16X3: every 16-bit weight and activation buffer has a lo plane (Op16::lo)
   int64_t launches = 0;
   int pdl = 1;                // env LDM_PDL=0: no programmatic dependent launch
   int debug_stop_after = 0;   // test tap: stop the denoiser after this many launches (0 = run everything)
@@ -154,27 +168,21 @@ struct LdmHandle {
   std::vector<ProfRec> prof_recs;
   // parameters (device)
   float *cat_emb = nullptr, *pos = nullptr, *adaln = nullptr, *sched = nullptr, *lae = nullptr;
-  void *wqkv[kMaxLayers] = {}, *wo[kMaxLayers] = {}, *w1[kMaxLayers] = {}, *w2[kMaxLayers] = {}, *whead = nullptr;
+  Op16 wqkv[kMaxLayers], wo[kMaxLayers], w1[kMaxLayers], w2[kMaxLayers], whead;
   float *bqkv[kMaxLayers] = {}, *bo[kMaxLayers] = {}, *b1[kMaxLayers] = {}, *b2[kMaxLayers] = {}, *ln2w[kMaxLayers] = {}, *ln2b[kMaxLayers] = {};
   float *hlnw = nullptr, *hlnb = nullptr;
-  CUtensorMap m_wqkv[kMaxLayers], m_wo[kMaxLayers], m_w1[kMaxLayers], m_w2[kMaxLayers], m_whead;
-  void *wqkv_lo[kMaxLayers] = {}, *wo_lo[kMaxLayers] = {}, *w1_lo[kMaxLayers] = {}, *w2_lo[kMaxLayers] = {}, *whead_lo = nullptr;
-  CUtensorMap m_wqkv_lo[kMaxLayers], m_wo_lo[kMaxLayers], m_w1_lo[kMaxLayers], m_w2_lo[kMaxLayers], m_whead_lo;
   int *qmap = nullptr, *amap = nullptr, *hmap = nullptr;   // source row / column maps of the padded QKV, out-projection and head weights
-  // workspace (device), sized for cap layouts
+  // workspace (device), sized for cap layouts (workspace_bufs)
   int cap = 0;
-  void *x16 = nullptr, *qkv16 = nullptr, *att16 = nullptr, *z16 = nullptr, *hid16 = nullptr;
+  Op16 x16, z16, qkv16;                // maps: 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
+  Op16 att16, hid16;                   // maps: A operands of the LN GEMMs: 128-row boxes (split mode: 64)
   float *x32 = nullptr, *y32 = nullptr, *logits = nullptr;
   float* rel_lp = nullptr;      // [cap][S][C] log-probabilities between the posterior and the draw (cond = relation)
   long long* ids[2] = {nullptr, nullptr};
   long long* ids_final = nullptr;
   long long *c_seq = nullptr, *c_seq_orig = nullptr; unsigned char* c_mask = nullptr; float* c_tbl = nullptr;  // staging for ldm_sample_host
-  CUtensorMap m_x16, m_z16, m_qkv16;                                         // 128-row boxes: QKV / FF1 / head A operands, attention's head tiles
-  CUtensorMap m_att16, m_hid16;                                              // A operands of the LN GEMMs: 128-row boxes (split mode: 64)
   CUtensorMap m_qkv16_st, m_hid16_st;                                        // 128-row boxes: the row-block GEMMs' TMA stores (one-plane modes)
   CUtensorMap m_x32, m_y32;                                                  // 64 x 232 fp32 boxes: the LN GEMMs' row halves (one-plane modes)
-  void *x16_lo = nullptr, *qkv16_lo = nullptr, *att16_lo = nullptr, *z16_lo = nullptr, *hid16_lo = nullptr;   // split mode only
-  CUtensorMap m_x16_lo, m_z16_lo, m_qkv16_lo, m_att16_lo, m_hid16_lo;
   std::vector<void*> owned;
   // CUDA graph of the whole T-step loop (ldm_sample_loop): captured once per (batch, plan, sampling, conditioning kind) and
   // replayed; everything that changes from call to call lives in device memory (noise key block, staged cond / start ids)
@@ -226,22 +234,30 @@ void free_staging(LdmHandle* h) {
   h->staging.clear();
 }
 
-// 16-bit weight buffer of rows x cols (split mode: the hi plane in dst, the lo plane in dst_lo)
-int alloc16(LdmHandle* h, void** dst, void** dst_lo, int rows, int cols) {
+// f(std::integral_constant<int, MODE>{}) for the handle's operand mode: the one place a run-time mode becomes a template argument
+template <typename F>
+auto with_mode(const LdmHandle* h, F&& f) {
+  if (h->mode == OP_BF16X3) return f(std::integral_constant<int, OP_BF16X3>{});
+  if (h->mode == OP_BF16) return f(std::integral_constant<int, OP_BF16>{});
+  return f(std::integral_constant<int, OP_F16>{});
+}
+
+// 16-bit weight buffer of rows x cols (split mode: both planes)
+int alloc16(LdmHandle* h, Op16& dst, int rows, int cols) {
   const size_t bytes = static_cast<size_t>(rows) * cols * 2;
-  CK(cudaMalloc(dst, bytes));
-  h->owned.push_back(*dst);
-  if (h->split) { CK(cudaMalloc(dst_lo, bytes)); h->owned.push_back(*dst_lo); }
+  CK(cudaMalloc(&dst.hi, bytes));
+  h->owned.push_back(dst.hi);
+  if (h->split) { CK(cudaMalloc(&dst.lo, bytes)); h->owned.push_back(dst.lo); }
   return LDM_OK;
 }
 
-// fp32 weight -> the 16-bit operand in dst (split mode: both planes), on stream st
-int pack16(const LdmHandle* h, void* dst, void* dst_lo, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
+// fp32 weight -> the 16-bit operand dst (split mode: both planes), on stream st
+int pack16(const LdmHandle* h, const Op16& dst, const float* src_dev, const int* row_map_dev, int dst_rows, int dst_cols, int src_cols,
            cudaStream_t st, const int* col_map_dev = nullptr) {
-  const int blocks = 512;
-  if (h->mode == OP_BF16X3) pack_weight_kernel<OP_BF16X3><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, dst_lo);
-  else if (h->mode == OP_BF16) pack_weight_kernel<OP_BF16><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
-  else pack_weight_kernel<OP_F16><<<blocks, 256, 0, st>>>(src_dev, dst, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, nullptr);
+  with_mode(h, [&](auto mode) {
+    pack_weight_kernel<decltype(mode)::value><<<512, 256, 0, st>>>(src_dev, dst.hi, row_map_dev, col_map_dev, dst_rows, dst_cols, src_cols, dst.lo);
+    return LDM_OK;
+  });
   CK(cudaGetLastError());
   return LDM_OK;
 }
@@ -278,37 +294,27 @@ int pack_weights(LdmHandle* h, const LdmWeights& w, cudaStream_t st) {
   int rc;
   for (int l = 0; l < L; ++l) {
     const size_t dd = static_cast<size_t>(d) * d;
-    if ((rc = pack16(h, h->wqkv[l], h->wqkv_lo[l], w.in_proj_w + l * 3 * dd, h->qmap, kQkvN, d, d, st))) return rc;
+    if ((rc = pack16(h, h->wqkv[l], w.in_proj_w + l * 3 * dd, h->qmap, kQkvN, d, d, st))) return rc;
     qkv_bias_kernel<<<(kQkvN + 255) / 256, 256, 0, st>>>(w.in_proj_b + static_cast<size_t>(l) * 3 * d, h->qmap, h->bqkv[l], kQkvN,
                                                         2 * 8 * kHeadPad, kHeadPad, d / h->desc.n_heads);
     CK(cudaGetLastError());
-    if ((rc = pack16(h, h->wo[l], h->wo_lo[l], w.out_proj_w + l * dd, nullptr, d, kAttN, d, st, h->amap))) return rc;   // K = 512: head h occupies columns h*64 .. h*64+57
+    if ((rc = pack16(h, h->wo[l], w.out_proj_w + l * dd, nullptr, d, kAttN, d, st, h->amap))) return rc;   // K = 512: head h occupies columns h*64 .. h*64+57
     CK(copy(h->bo[l], w.out_proj_b + static_cast<size_t>(l) * d, d));
-    if ((rc = pack16(h, h->w1[l], h->w1_lo[l], w.linear1_w + l * ff * static_cast<size_t>(d), nullptr, ff, d, d, st))) return rc;
+    if ((rc = pack16(h, h->w1[l], w.linear1_w + l * ff * static_cast<size_t>(d), nullptr, ff, d, d, st))) return rc;
     CK(copy(h->b1[l], w.linear1_b + static_cast<size_t>(l) * ff, ff));
-    if ((rc = pack16(h, h->w2[l], h->w2_lo[l], w.linear2_w + l * ff * static_cast<size_t>(d), nullptr, d, ff, ff, st))) return rc;
+    if ((rc = pack16(h, h->w2[l], w.linear2_w + l * ff * static_cast<size_t>(d), nullptr, d, ff, ff, st))) return rc;
     CK(copy(h->b2[l], w.linear2_b + static_cast<size_t>(l) * d, d));
     CK(copy(h->ln2w[l], w.norm2_w + static_cast<size_t>(l) * d, d));
     CK(copy(h->ln2b[l], w.norm2_b + static_cast<size_t>(l) * d, d));
   }
-  return pack16(h, h->whead, h->whead_lo, w.head_w, h->hmap, kLogitLd, d, d, st);
+  return pack16(h, h->whead, w.head_w, h->hmap, kLogitLd, d, d, st);
 }
 
 // TMA descriptor(s) of one 16-bit operand (split mode: both planes), boxes of box_rows x kb elements
-int make_op_maps(const LdmHandle* h, CUtensorMap* m, CUtensorMap* m_lo, const void* base, const void* base_lo, uint64_t rows, uint64_t cols,
-                 uint32_t box_rows, int kb) {
-  int rc = make_map(m, base, rows, cols, box_rows, kb, h->bf16);
+int make_op_maps(const LdmHandle* h, Op16& op, uint64_t rows, uint64_t cols, uint32_t box_rows, int kb) {
+  int rc = make_map(&op.map, op.hi, rows, cols, box_rows, kb, h->bf16);
   if (rc || !h->split) return rc;
-  return make_map(m_lo, base_lo, rows, cols, box_rows, kb, h->bf16);
-}
-
-template <int MODE>
-OpMaps<MODE> op_maps(const CUtensorMap& hi, const CUtensorMap& lo) {
-  OpMaps<MODE> m;
-  m.hi = hi;
-  if constexpr (kOpSplit<MODE>) m.lo = lo;
-  else (void)lo;
-  return m;
+  return make_map(&op.map_lo, op.lo, rows, cols, box_rows, kb, h->bf16);
 }
 
 // util.py:47-70 + constrained.py:64-90: float64 schedule, fp32 log tables, 8 rows of length T+1 per group
@@ -408,13 +414,25 @@ int set_smem(LdmHandle* h) {
   return LDM_OK;
 }
 
+// The per-batch workspace: each buffer holds per_layout bytes per layout.  ldm_debug_read reads a buffer by its name (nullptr: not
+// readable); a 16-bit operand (lo != nullptr) also has a lo plane in the split mode, read as "<name>_lo".
+struct WsBuf { const char* name; void** hi; void** lo; size_t per_layout; };
+std::vector<WsBuf> workspace_bufs(LdmHandle* h) {
+  const size_t d = h->desc.d_model, ff = h->desc.d_ff, S = h->S;
+  const auto op = [](const char* name, Op16& o, size_t cols) { return WsBuf{name, &o.hi, &o.lo, kBM * cols * 2}; };
+  const auto buf = [](const char* name, auto** p, size_t per_layout) { return WsBuf{name, reinterpret_cast<void**>(p), nullptr, per_layout}; };
+  return {op("x16", h->x16, d), op("qkv16", h->qkv16, kQkvN), op("att16", h->att16, kAttN), op("z16", h->z16, d), op("hid16", h->hid16, ff),
+          buf("x32", &h->x32, kBM * d * 4), buf("y32", &h->y32, kBM * d * 4), buf("logits", &h->logits, kBM * kLogitLd * 4),
+          buf(nullptr, &h->ids[0], S * 8), buf(nullptr, &h->ids[1], S * 8), buf(nullptr, &h->ids_final, S * 8),
+          buf(nullptr, &h->c_seq, S * 8), buf(nullptr, &h->c_seq_orig, S * 8), buf(nullptr, &h->c_mask, S)};
+}
+
 void free_workspace(LdmHandle* h) {
-  void** ws[] = {&h->x16, &h->qkv16, &h->att16, &h->z16, &h->hid16, &h->x16_lo, &h->qkv16_lo, &h->att16_lo, &h->z16_lo, &h->hid16_lo,
-                 reinterpret_cast<void**>(&h->x32), reinterpret_cast<void**>(&h->y32),
-                 reinterpret_cast<void**>(&h->logits), reinterpret_cast<void**>(&h->ids[0]), reinterpret_cast<void**>(&h->ids[1]),
-                 reinterpret_cast<void**>(&h->ids_final), reinterpret_cast<void**>(&h->c_seq), reinterpret_cast<void**>(&h->c_seq_orig),
-                 reinterpret_cast<void**>(&h->c_mask), reinterpret_cast<void**>(&h->rel_lp)};
-  for (void** p : ws) { if (*p) cudaFree(*p); *p = nullptr; }
+  for (const WsBuf& b : workspace_bufs(h))
+    for (void** p : {b.hi, b.lo})
+      if (p && *p) { cudaFree(*p); *p = nullptr; }
+  // sized for cap layouts too, but allocated by the first relation step (step_impl)
+  if (h->rel_lp) { cudaFree(h->rel_lp); h->rel_lp = nullptr; }
   h->cap = 0;
 }
 
@@ -424,59 +442,39 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   // free the old workspace: nothing may still be running on it, and a failed reallocation must not leave stale pointers behind
   CK(cudaDeviceSynchronize());
   free_workspace(h);
-  const size_t M = static_cast<size_t>(n_layouts) * kBM;
-  const int d = h->desc.d_model, ff = h->desc.d_ff;
-  if (h->split) {
-    // the lo planes: ~1.24 MB per layout.  An allocation that does not fit is reported (not left as the runtime's last error)
-    // and releases what this call allocated
-    void** lo[] = {&h->x16_lo, &h->qkv16_lo, &h->att16_lo, &h->z16_lo, &h->hid16_lo};
-    const size_t cols[] = {static_cast<size_t>(d), static_cast<size_t>(kQkvN), static_cast<size_t>(kAttN), static_cast<size_t>(d), static_cast<size_t>(ff)};
-    for (int i = 0; i < 5; ++i) {
-      const cudaError_t e = cudaMalloc(lo[i], M * cols[i] * 2);
+  // every buffer is zeroed once: the 3 padding rows of every layout tile must stay finite.  An allocation that does not fit is
+  // reported (not left as the runtime's last error) and releases what this call allocated
+  for (const WsBuf& b : workspace_bufs(h)) {
+    for (void** p : {b.hi, h->split ? b.lo : nullptr}) {
+      if (!p) continue;
+      const size_t bytes = static_cast<size_t>(n_layouts) * b.per_layout;
+      cudaError_t e = cudaMalloc(p, bytes);
+      if (e == cudaSuccess) e = cudaMemset(*p, 0, bytes);
       if (e != cudaSuccess) {
         cudaGetLastError();
         free_workspace(h);
-        return fail(LDM_ERR_CUDA, "split-operand workspace for %d layouts does not fit: %s", n_layouts, cudaGetErrorString(e));
+        return fail(LDM_ERR_CUDA, "workspace for %d layouts does not fit: %s", n_layouts, cudaGetErrorString(e));
       }
-      CK(cudaMemset(*lo[i], 0, M * cols[i] * 2));
     }
   }
-  CK(cudaMalloc(&h->x16, M * d * 2));
-  CK(cudaMalloc(&h->qkv16, M * kQkvN * 2));
-  CK(cudaMalloc(&h->att16, M * kAttN * 2));
-  CK(cudaMalloc(&h->z16, M * d * 2));
-  CK(cudaMalloc(&h->hid16, M * ff * 2));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->x32), M * d * 4));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->y32), M * d * 4));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->logits), M * kLogitLd * 4));
-  const size_t nid = static_cast<size_t>(n_layouts) * h->S;
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->ids[0]), nid * 8));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->ids[1]), nid * 8));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->ids_final), nid * 8));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->c_seq), nid * 8));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->c_seq_orig), nid * 8));
-  CK(cudaMalloc(reinterpret_cast<void**>(&h->c_mask), nid));
-  // zero once: the 3 padding rows of every layout tile must stay finite
-  CK(cudaMemset(h->x16, 0, M * d * 2)); CK(cudaMemset(h->qkv16, 0, M * kQkvN * 2)); CK(cudaMemset(h->att16, 0, M * kAttN * 2));
-  CK(cudaMemset(h->z16, 0, M * d * 2)); CK(cudaMemset(h->hid16, 0, M * ff * 2)); CK(cudaMemset(h->x32, 0, M * d * 4));
-  CK(cudaMemset(h->y32, 0, M * d * 4));
-  CK(cudaMemset(h->logits, 0, M * kLogitLd * 4));
   h->cap = n_layouts;
   h->ws_generation++;
+  const size_t M = static_cast<size_t>(n_layouts) * kBM;
+  const int d = h->desc.d_model, ff = h->desc.d_ff;
   int rc;
   // the row-block GEMM's resident A k-blocks are the one-plane ring's (64 elements): QKV, FF1 and the head share these maps
   static_assert(gemm_kb(false) == RbSmem::kKB, "one A geometry for QKV / FF1 / head");
   const int kb = gemm_kb(h->split);
-  if ((rc = make_op_maps(h, &h->m_x16, &h->m_x16_lo, h->x16, h->x16_lo, M, d, kBM, kb))) return rc;
-  if ((rc = make_op_maps(h, &h->m_z16, &h->m_z16_lo, h->z16, h->z16_lo, M, d, kBM, kb))) return rc;
+  if ((rc = make_op_maps(h, h->x16, M, d, kBM, kb))) return rc;
+  if ((rc = make_op_maps(h, h->z16, M, d, kBM, kb))) return rc;
   const int ln_rows = h->split ? kLnSplitRows : LnFf2::kRows;
-  if ((rc = make_op_maps(h, &h->m_att16, &h->m_att16_lo, h->att16, h->att16_lo, M, kAttN, ln_rows, kLnKB))) return rc;
-  if ((rc = make_op_maps(h, &h->m_hid16, &h->m_hid16_lo, h->hid16, h->hid16_lo, M, ff, ln_rows, kLnKB))) return rc;
+  if ((rc = make_op_maps(h, h->att16, M, kAttN, ln_rows, kLnKB))) return rc;
+  if ((rc = make_op_maps(h, h->hid16, M, ff, ln_rows, kLnKB))) return rc;
   // attention's Q / K / V head tiles: 128 rows x one padded head, in every mode
-  if ((rc = make_op_maps(h, &h->m_qkv16, &h->m_qkv16_lo, h->qkv16, h->qkv16_lo, M, kQkvN, kBM, kHeadPad))) return rc;
+  if ((rc = make_op_maps(h, h->qkv16, M, kQkvN, kBM, kHeadPad))) return rc;
   // the row-block GEMMs' stores: 64-column x 128-row boxes of the staging tile (128-byte swizzle)
-  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16, M, kQkvN, kBM, 64, h->bf16))) return rc;
-  if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16, M, ff, kBM, 64, h->bf16))) return rc;
+  if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16.hi, M, kQkvN, kBM, 64, h->bf16))) return rc;
+  if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16.hi, M, ff, kBM, 64, h->bf16))) return rc;
   // the persistent LN GEMMs' residual loads and fp32 stores: one row half of the CTA's columns per box
   if (!h->split && (rc = make_map_f32(&h->m_x32, h->x32, M, d, LnFf2::kHalf, kLnBN))) return rc;
   if (!h->split && (rc = make_map_f32(&h->m_y32, h->y32, M, d, LnFf2::kHalf, kLnBN))) return rc;
@@ -485,7 +483,6 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
 
 template <int MODE>
 int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
-  const auto maps = [](const CUtensorMap& hi, const CUtensorMap& lo) { return op_maps<MODE>(hi, lo); };
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
   const int M = n * kBM;
   // Grids: the fp16 / bf16 row-block GEMMs (QKV, FF1) and LN GEMMs (epilogue warps) are persistent (one CTA per SM): their
@@ -534,49 +531,49 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     const int warps = n * 128, blocks = (warps * 32 + 255) / 256;
     ProfScope ps(h, CAT_EMBED, st);
     CK(launch_step(h, embed_adaln_kernel<MODE>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
-                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16, n, n, h->S, d, h->x16_lo));
+                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16.hi, n, n, h->S, d, h->x16.lo));
   }
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
     {  // QKV projection (+bias, q * 1/sqrt(head_dim))
-      GemmParams p{M, kQkvN, d, 0, h->bqkv[l], h->qkv16, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
-      p.rev = next_rev(); p.out_lo = h->qkv16_lo;
+      GemmParams p{M, kQkvN, d, 0, h->bqkv[l], h->qkv16.hi, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
+      p.rev = next_rev(); p.out_lo = h->qkv16.lo;
       ProfScope ps(h, CAT_QKV, st);
-      CK(plain_gemm(std::integral_constant<int, EPI_QKV>{}, maps(h->m_x16, h->m_x16_lo), maps(h->m_wqkv[l], h->m_wqkv_lo[l]), h->m_qkv16_st, p));
+      CK(plain_gemm(std::integral_constant<int, EPI_QKV>{}, h->x16.maps<MODE>(), h->wqkv[l].maps<MODE>(), h->m_qkv16_st, p));
     }
     LDM_STAGE_DONE();
     {
       ProfScope ps(h, CAT_ATTN, st);
       CK(launch_step(h, attention_kernel<MODE>, dim3(n * h->desc.n_heads), kAttThreads, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes, st,
-                     maps(h->m_qkv16, h->m_qkv16_lo), h->att16, h->S, h->desc.n_heads, n, next_rev(), h->att16_lo));
+                     h->qkv16.maps<MODE>(), h->att16.hi, h->S, h->desc.n_heads, n, next_rev(), h->att16.lo));
     }
     LDM_STAGE_DONE();
     {  // out-projection + bias + residual (from the NORMALISED x) -> y32 ; z16 = LayerNorm2(y)   [fused epilogue]
-      GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
-      p.rev = next_rev(); p.out_lo = h->z16_lo;
+      GemmParams p{M, d, kAttN, 1, h->bo[l], h->z16.hi, d, 1.0f, 0, h->x32, h->y32, h->ln2w[l], h->ln2b[l], 0, nullptr};
+      p.rev = next_rev(); p.out_lo = h->z16.lo;
       ProfScope ps(h, CAT_OUTPROJ, st);
-      CK(ln_gemm(maps(h->m_att16, h->m_att16_lo), maps(h->m_wo[l], h->m_wo_lo[l]), h->m_x32, h->m_y32, p));
+      CK(ln_gemm(h->att16.maps<MODE>(), h->wo[l].maps<MODE>(), h->m_x32, h->m_y32, p));
     }
     LDM_STAGE_DONE();
     {  // FF1 + ReLU
-      GemmParams p{M, ff, d, 0, h->b1[l], h->hid16, ff, 1.0f, 0};   // 14 tiles of 128 columns + one of 64 (split mode: 7 of 256 + one of 64)
-      p.rev = next_rev(); p.out_lo = h->hid16_lo;
+      GemmParams p{M, ff, d, 0, h->b1[l], h->hid16.hi, ff, 1.0f, 0};   // 14 tiles of 128 columns + one of 64 (split mode: 7 of 256 + one of 64)
+      p.rev = next_rev(); p.out_lo = h->hid16.lo;
       ProfScope ps(h, CAT_FF1, st);
-      CK(plain_gemm(std::integral_constant<int, EPI_RELU>{}, maps(h->m_z16, h->m_z16_lo), maps(h->m_w1[l], h->m_w1_lo[l]), h->m_hid16_st, p));
+      CK(plain_gemm(std::integral_constant<int, EPI_RELU>{}, h->z16.maps<MODE>(), h->w1[l].maps<MODE>(), h->m_hid16_st, p));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
       GemmParams p{M, d, ff, 1, h->b2[l], nullptr, d, 1.0f, 0, h->y32, nullptr, nullptr, nullptr, 0, nullptr};
       if (l + 1 < L) {
         const float* tab = h->adaln + (static_cast<size_t>(l + 1) * T + t_model) * 2 * d;
-        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16; p.out_lo = h->x16_lo;
+        p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16.hi; p.out_lo = h->x16.lo;
         if (t_layout) { p.ln_scale = h->adaln + static_cast<size_t>(l + 1) * T * 2 * d; p.t_layout = t_layout; p.n_layouts = n; }   // per-layout rows
       } else {
-        p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16; p.out_lo = h->z16_lo;
+        p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16.hi; p.out_lo = h->z16.lo;
       }
       p.rev = next_rev();
       ProfScope ps(h, CAT_FF2, st);
-      CK(ln_gemm(maps(h->m_hid16, h->m_hid16_lo), maps(h->m_w2[l], h->m_w2_lo[l]), h->m_y32, h->m_x32, p));
+      CK(ln_gemm(h->hid16.maps<MODE>(), h->w2[l].maps<MODE>(), h->m_y32, h->m_x32, p));
     }
     LDM_STAGE_DONE();
   }
@@ -584,7 +581,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads, kHeadSmem, st, maps(h->m_z16, h->m_z16_lo), maps(h->m_whead, h->m_whead_lo), p));
+    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads, kHeadSmem, st, h->z16.maps<MODE>(), h->whead.maps<MODE>(), p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
@@ -593,11 +590,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
 
 // the denoiser in the handle's operand mode
 int run_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
-  switch (h->mode) {
-    case OP_BF16X3: return launch_denoiser<OP_BF16X3>(h, n, ids_in, t_model, st, t_layout, skip_embed);
-    case OP_BF16: return launch_denoiser<OP_BF16>(h, n, ids_in, t_model, st, t_layout, skip_embed);
-    default: return launch_denoiser<OP_F16>(h, n, ids_in, t_model, st, t_layout, skip_embed);
-  }
+  return with_mode(h, [&](auto mode) { return launch_denoiser<decltype(mode)::value>(h, n, ids_in, t_model, st, t_layout, skip_embed); });
 }
 
 int validate_common(LdmHandle* h, int B, const LdmSampling* s) {
@@ -696,7 +689,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
   p.ids_out = ids_out; p.logprob_out = logprob_out;
   if (t_next >= 0) {     // the loop: this draw also writes the next step's embedding + AdaLN_0(t_next) rows
     p.emb_cat = h->cat_emb; p.emb_pos = h->pos; p.emb_adaln = h->adaln + static_cast<size_t>(t_next) * 2 * h->desc.d_model;
-    p.emb_x32 = h->x32; p.emb_x16 = h->x16; p.emb_d = h->desc.d_model; p.emb_bf16 = h->bf16 ? 1 : 0;
+    p.emb_x32 = h->x32; p.emb_x16 = h->x16.hi; p.emb_d = h->desc.d_model; p.emb_bf16 = h->bf16 ? 1 : 0;
   }
   const int warps = B * h->S, blocks = (warps * 32 + 255) / 256;
   // cond = relation on the device (base.py:243-284 order: strong mask [+ refinement prior] -> update() -> PAD-disable -> draw):
@@ -792,10 +785,10 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   TRY(dev_alloc(h, &h->adaln, static_cast<size_t>(L) * T * 2 * d));
   const int plain_w_rows = h->split ? kPlainBN : kRbCols;
   for (int l = 0; l < L; ++l) {
-    TRY(alloc16(h, &h->wqkv[l], &h->wqkv_lo[l], kQkvN, d));
-    TRY(alloc16(h, &h->wo[l], &h->wo_lo[l], d, kAttN));
-    TRY(alloc16(h, &h->w1[l], &h->w1_lo[l], ff, d));
-    TRY(alloc16(h, &h->w2[l], &h->w2_lo[l], d, ff));
+    TRY(alloc16(h, h->wqkv[l], kQkvN, d));
+    TRY(alloc16(h, h->wo[l], d, kAttN));
+    TRY(alloc16(h, h->w1[l], ff, d));
+    TRY(alloc16(h, h->w2[l], d, ff));
     TRY(dev_alloc(h, &h->bqkv[l], static_cast<size_t>(kQkvN)));
     TRY(dev_alloc(h, &h->bo[l], static_cast<size_t>(d)));
     TRY(dev_alloc(h, &h->b1[l], static_cast<size_t>(ff)));
@@ -803,13 +796,13 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
     TRY(dev_alloc(h, &h->ln2w[l], static_cast<size_t>(d)));
     TRY(dev_alloc(h, &h->ln2b[l], static_cast<size_t>(d)));
     // QKV / FF1 weights: one tile's weight rows per box (row-block kernel: 128, split mode: 256)
-    TRY(make_op_maps(h, &h->m_wqkv[l], &h->m_wqkv_lo[l], h->wqkv[l], h->wqkv_lo[l], kQkvN, d, plain_w_rows, gemm_kb(h->split)));
-    TRY(make_op_maps(h, &h->m_wo[l], &h->m_wo_lo[l], h->wo[l], h->wo_lo[l], d, kAttN, kLnBN, kLnKB));
-    TRY(make_op_maps(h, &h->m_w1[l], &h->m_w1_lo[l], h->w1[l], h->w1_lo[l], ff, d, plain_w_rows, gemm_kb(h->split)));
-    TRY(make_op_maps(h, &h->m_w2[l], &h->m_w2_lo[l], h->w2[l], h->w2_lo[l], d, ff, kLnBN, kLnKB));
+    TRY(make_op_maps(h, h->wqkv[l], kQkvN, d, plain_w_rows, gemm_kb(h->split)));
+    TRY(make_op_maps(h, h->wo[l], d, kAttN, kLnBN, kLnKB));
+    TRY(make_op_maps(h, h->w1[l], ff, d, plain_w_rows, gemm_kb(h->split)));
+    TRY(make_op_maps(h, h->w2[l], d, ff, kLnBN, kLnKB));
   }
-  TRY(alloc16(h, &h->whead, &h->whead_lo, kLogitLd, d));
-  TRY(make_op_maps(h, &h->m_whead, &h->m_whead_lo, h->whead, h->whead_lo, kLogitLd, d, kHeadBN, gemm_kb(h->split)));
+  TRY(alloc16(h, h->whead, kLogitLd, d));
+  TRY(make_op_maps(h, h->whead, kLogitLd, d, kHeadBN, gemm_kb(h->split)));
 
   // per-head padded QKV row map: dst row = which*512 + head*64 + j  <-  src row which*d + head*58 + j (j < 58)
   const int dh = d / desc->n_heads;
@@ -849,7 +842,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (cudaDeviceSynchronize() != cudaSuccess) { ldm_destroy(h); return fail(LDM_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(cudaGetLastError())); }
   free_staging(h);
 
-  TRY(h->mode == OP_BF16X3 ? set_smem<OP_BF16X3>(h) : h->mode == OP_BF16 ? set_smem<OP_BF16>(h) : set_smem<OP_F16>(h));
+  TRY(with_mode(h, [&](auto mode) { return set_smem<decltype(mode)::value>(h); }));
 #undef TRY
   *out = h;
   return LDM_OK;
@@ -1290,29 +1283,21 @@ int ldm_debug_set_stop_after(LdmHandle* h, int32_t n_launches) {
 
 int64_t ldm_debug_read(const LdmHandle* h, const char* name, void* dst, int64_t capacity_bytes, int32_t n_layouts) {
   if (!h || !name || n_layouts > h->cap) return -1;
-  const size_t M = static_cast<size_t>(n_layouts) * kBM;
-  const int d = h->desc.d_model, ff = h->desc.d_ff;
-  const void* src = nullptr; size_t bytes = 0;
-  if (!strcmp(name, "x32")) { src = h->x32; bytes = M * d * 4; }
-  else if (!strcmp(name, "y32")) { src = h->y32; bytes = M * d * 4; }
-  else if (!strcmp(name, "x16")) { src = h->x16; bytes = M * d * 2; }
-  else if (!strcmp(name, "z16")) { src = h->z16; bytes = M * d * 2; }
-  else if (!strcmp(name, "att16")) { src = h->att16; bytes = M * kAttN * 2; }
-  else if (!strcmp(name, "qkv16")) { src = h->qkv16; bytes = M * kQkvN * 2; }
-  else if (!strcmp(name, "hid16")) { src = h->hid16; bytes = M * ff * 2; }
-  else if (!strcmp(name, "logits")) { src = h->logits; bytes = M * kLogitLd * 4; }
-  else if (!strcmp(name, "x16_lo")) { src = h->x16_lo; bytes = M * d * 2; }
-  else if (!strcmp(name, "z16_lo")) { src = h->z16_lo; bytes = M * d * 2; }
-  else if (!strcmp(name, "att16_lo")) { src = h->att16_lo; bytes = M * kAttN * 2; }
-  else if (!strcmp(name, "qkv16_lo")) { src = h->qkv16_lo; bytes = M * kQkvN * 2; }
-  else if (!strcmp(name, "hid16_lo")) { src = h->hid16_lo; bytes = M * ff * 2; }
-  else return -1;
-  if (!h->split && strstr(name, "_lo") != nullptr) return -1;   // lo planes exist in the split mode only
-  if (dst && capacity_bytes >= static_cast<int64_t>(bytes)) {
-    if (cudaDeviceSynchronize() != cudaSuccess) return -2;
-    if (cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -2;
+  const size_t len = strlen(name), base_len = len > 3 && !strcmp(name + len - 3, "_lo") ? len - 3 : len;
+  // the table takes a mutable handle to allocate through; here it is only read
+  for (const WsBuf& b : workspace_bufs(const_cast<LdmHandle*>(h))) {
+    if (!b.name || strlen(b.name) != base_len || strncmp(name, b.name, base_len)) continue;
+    const bool lo = base_len < len;
+    if (lo && (!b.lo || !h->split)) return -1;   // lo planes: 16-bit operands in the split mode only
+    const void* src = lo ? *b.lo : *b.hi;
+    const size_t bytes = static_cast<size_t>(n_layouts) * b.per_layout;
+    if (dst && capacity_bytes >= static_cast<int64_t>(bytes)) {
+      if (cudaDeviceSynchronize() != cudaSuccess) return -2;
+      if (cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -2;
+    }
+    return static_cast<int64_t>(bytes);
   }
-  return static_cast<int64_t>(bytes);
+  return -1;
 }
 int32_t ldm_num_classes(const LdmHandle* h) { return h ? h->C : 0; }
 int32_t ldm_seq_len(const LdmHandle* h) { return h ? h->S : 0; }
