@@ -38,7 +38,7 @@ typedef struct LdmHandle LdmHandle;
 typedef struct {
   int32_t n_cat;          /* 25 rico25, 5 publaynet */
   int32_t n_bins;         /* 32 */
-  int32_t n_elem;         /* 25 (max_seq_length) */
+  int32_t n_elem;         /* max_seq_length: 25 by default; S = n_elem * n_attr <= 256 (51 elements of c-x-y-w-h) */
   int32_t n_attr;         /* 5  (c,x,y,w,h) */
   int32_t d_model;        /* 464 */
   int32_t n_heads;        /* 8 */
@@ -254,7 +254,9 @@ int ldm_profile_end(LdmHandle* h, float* ms_per_category, int64_t* launches_per_
 
 /* test taps (tests/ and tools/ only): stop the denoiser after n launches (0 = off); read a workspace buffer
  * ("x32","y32","x16","z16","att16","qkv16","hid16","logits"; operand_dtype 2 also the lo planes "x16_lo","z16_lo","att16_lo",
- * "qkv16_lo","hid16_lo") of the first n_layouts layouts to host; returns bytes (< 0: unknown name). */
+ * "qkv16_lo","hid16_lo") of the first n_layouts layouts to host; returns bytes (< 0: unknown name).  A layout takes 128 R rows
+ * of every row buffer, R = ceil(S / 128) (1 for S <= 128, 2 for S <= 256): [n_layouts][128 R][cols], token s in row s,
+ * rows S .. 128 R - 1 pad rows. */
 int ldm_debug_set_stop_after(LdmHandle* h, int32_t n_launches);
 /* test tap of LDM_NOISE_TORCH: out_dev[numel] = the float32 values torch's CUDA generator (this seed / offset, the handle's
  * device) gives exponential_ (which = 1) or rand (which = 0) of a contiguous tensor of numel < 2^31 elements, computed by

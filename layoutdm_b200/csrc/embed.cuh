@@ -2,7 +2,7 @@
 // plus the weight packing (AdaLN (scale, shift) table, 16-bit operands, padded QKV bias) of ldm_create / ldm_load_weights.
 //   h  = cat_emb[id] + pos[s]                                   T/models/common/nn_lib.py:204,220 (+ :112-127)
 //   x  = LN(h) * (1 + scale_t) + shift_t                        T/models/transformer_utils.py:79-83
-// One warp per token row; pad rows (s >= 125 of each 128-row layout tile) are written as zeros so that every
+// One warp per token row; pad rows (s >= S of each layout's 128 R rows) are written as zeros so that every
 // later tile stays finite.
 #pragma once
 #include "common.cuh"
@@ -128,16 +128,16 @@ __global__ void __launch_bounds__(256)
 embed_adaln_kernel(const long long* __restrict__ ids /*[B][S]*/, const float* __restrict__ cat_emb /*[C][d]*/,
                    const float* __restrict__ pos /*[S][d]*/, const float* __restrict__ adaln_tab /*[T][2d] of layer 0*/, int t_model,
                    const int* __restrict__ t_layout /*[n_layouts] per-layout timesteps (training-side calls) or nullptr*/,
-                   float* __restrict__ x32 /*[B*128][d]*/, void* __restrict__ x16_, int n_layouts, int n_layouts_padded, int S, int d,
+                   float* __restrict__ x32 /*[B*128R][d]*/, void* __restrict__ x16_, int n_layouts, int rows_log2 /*log2(128 R)*/, int S, int d,
                    void* __restrict__ x16_lo /*split mode: lo plane of x16*/) {
   using O = OpT<MODE>;
   typename O::T* x16 = static_cast<typename O::T*>(x16_);
   const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp_global >= n_layouts_padded * 128) return;
+  if (warp_global >= (n_layouts << rows_log2)) return;
   pdl_sync();                                // ids come from the previous step's draw; x32 / x16 may still be read by it
-  const int b = warp_global >> 7, s = warp_global & 127;
+  const int b = warp_global >> rows_log2, s = warp_global & ((1 << rows_log2) - 1);
   const size_t row = static_cast<size_t>(warp_global);
-  if (s >= S || b >= n_layouts) {      // padding rows / padding layout of an odd batch
+  if (s >= S) {                        // padding rows
     const int nv = d / 4;
     float4* o32 = reinterpret_cast<float4*>(x32 + row * d);
     uint2* o16 = reinterpret_cast<uint2*>(x16 + row * d);

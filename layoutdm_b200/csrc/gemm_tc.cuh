@@ -1,6 +1,6 @@
 // wgmma (Hopper warpgroup MMA) GEMMs of the LayoutDM denoiser, C[M,N] = A[M,K] * W[N,K]^T (+ fused epilogue).
 //
-//   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 * n_layouts (one 128-row block = one layout)
+//   A : activations, row-major [M][K] 16-bit (fp16 or bf16), M = 128 R * n_layouts (a layout is R = 1 or 2 128-row blocks)
 //   W : nn.Linear weight, row-major [N][K] 16-bit  (both operands are "K-major" for the MMA)
 //   split mode (OP_BF16X3): A and W are bf16 (hi, lo) plane pairs; 16-bit outputs are written as (hi, lo) pairs (out, out_lo)
 //
@@ -29,7 +29,7 @@
 
 namespace ldm {
 
-constexpr int kBM = 128;       // rows of one layout tile (125 tokens + 3 pad rows)
+constexpr int kBM = 128;       // rows of one row block; a layout of S tokens takes ceil(S / 128) of them (pad rows S ..)
 constexpr int kWgK = 16;       // K per wgmma (16-bit operands)
 constexpr int kGemmConsumers = 256;
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // persistent block: 128 x 40 + 256 x 232 <= the SM's 64 K registers
@@ -60,6 +60,7 @@ struct GemmParams {
                           // with the rows its producer wrote last -- the part of the intermediate that is still in L2
   void* out_lo;           // split mode: lo plane of the 16-bit output (same layout as out)
   int n_ranges;           // gemm_rowblock_kernel: column ranges each row block is cut into (work items = row blocks x n_ranges)
+  int layout_rows;        // EPI_LN + t_layout: rows per layout (128 R), which maps a tile's first row to its layout
 };
 
 template <bool BF16, int N>
@@ -200,10 +201,10 @@ LDM_DEVINL void bias_act(const float (&acc)[N], int j, const float* bias, int c,
 
 // the LayerNorm's (gamma, beta) rows of the tile at row m0 and the offset added to gamma (AdaLN: gamma = 1 + scale)
 struct LnAffine { const float* gam; const float* bet; float gadd; };
-LDM_DEVINL LnAffine ln_affine(const float* scale, const float* shift, int adaln, const int* t_layout, int n_layouts, int m0, int N) {
+LDM_DEVINL LnAffine ln_affine(const float* scale, const float* shift, int adaln, const int* t_layout, int n_layouts, int layout_rows, int m0, int N) {
   LnAffine a{scale, shift, adaln ? 1.0f : 0.0f};
   if (t_layout != nullptr) {                                 // per-layout timesteps: this layout's AdaLN (scale, shift) row
-    const int layout = m0 / kBM;
+    const int layout = m0 / layout_rows;
     const int tl = layout < n_layouts ? __ldg(t_layout + layout) : 0;
     a.gam = scale + static_cast<size_t>(tl) * 2 * N; a.bet = a.gam + N; a.gadd = 1.0f;
   }
@@ -344,7 +345,7 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M row
     named_bar_sync(1, kGemmConsumers);
     const float rstd0 = 1.0f / sqrtf(fmaxf((q0 + ssq[(wn ^ 1) * 64 + rw]) * inv_n, 0.0f) + 1e-5f);
     const float rstd1 = 1.0f / sqrtf(fmaxf((q1 + ssq[(wn ^ 1) * 64 + rw + 8]) * inv_n, 0.0f) + 1e-5f);
-    const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
+    const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, p.layout_rows, m0, N);
     typename O::T* out16 = static_cast<typename O::T*>(p.out);
 #pragma unroll
     for (int j = 0; j < BN_WG / 8; ++j) {
@@ -740,7 +741,7 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
     for (int t = cl; t < n_work; t += n_cl, ++it) {
       const int m0 = tile_m0(t), b = it & 1;
       const uint32_t xph = (it >> 1) & 1;
-      const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, m0, N);
+      const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, p.layout_rows, m0, N);
       const float *gam = a.gam + col0, *bet = a.bet + col0;
       typename O::T* out16 = static_cast<typename O::T*>(p.out) + col0;
       const bool keep32 = p.out32 != nullptr;

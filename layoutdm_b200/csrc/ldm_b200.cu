@@ -119,19 +119,19 @@ int make_map_f32(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols,
   return LDM_OK;
 }
 
-// (B,S,C) contiguous <-> padded internal logits [B*128][160]
-__global__ void logits_scatter_kernel(const float* __restrict__ src, float* __restrict__ dst, int n_layouts, int S, int C) {
+// (B,S,C) contiguous <-> padded internal logits [B*rows][160], rows = 128 R per layout
+__global__ void logits_scatter_kernel(const float* __restrict__ src, float* __restrict__ dst, int n_layouts, int S, int C, int rows) {
   const size_t n = static_cast<size_t>(n_layouts) * S * C;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % C); const size_t tok = i / C; const int s = static_cast<int>(tok % S); const size_t b = tok / S;
-    dst[(b * 128 + s) * kLogitLd + c] = src[i];
+    dst[(b * rows + s) * kLogitLd + c] = src[i];
   }
 }
-__global__ void logits_gather_kernel(const float* __restrict__ src, float* __restrict__ dst, int n_layouts, int S, int C) {
+__global__ void logits_gather_kernel(const float* __restrict__ src, float* __restrict__ dst, int n_layouts, int S, int C, int rows) {
   const size_t n = static_cast<size_t>(n_layouts) * S * C;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % C); const size_t tok = i / C; const int s = static_cast<int>(tok % S); const size_t b = tok / S;
-    dst[i] = src[(b * 128 + s) * kLogitLd + c];
+    dst[i] = src[(b * rows + s) * kLogitLd + c];
   }
 }
 __global__ void fill_ids_kernel(long long* dst, long long v, size_t n) {
@@ -157,6 +157,8 @@ struct Op16 {
 struct LdmHandle {
   LdmModelDesc desc;
   int C = 0, S = 0, L = 0, T = 0, G = 0;
+  int R = 1;                  // row tiles of kBM rows per layout: ceil(S / 128), 1 or 2.  Every row map and grid reads it
+  int layout_rows() const { return kBM * R; }
   int mode = OP_F16;          // operand mode (LdmModelDesc::operand_dtype)
   bool bf16 = false;          // bf16 operand data (OP_BF16, OP_BF16X3)
   bool split = false;         // OP_BF16X3: every 16-bit weight and activation buffer has a lo plane (Op16::lo)
@@ -400,7 +402,8 @@ int set_smem(LdmHandle* h) {
     CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnOutStages>, attr, LnOut::kBytes));
     CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnFf2Stages>, attr, LnFf2::kBytes));
   }
-  CK(cudaFuncSetAttribute(attention_kernel<MODE>, attr, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes));
+  CK(cudaFuncSetAttribute(attention_kernel<MODE, 1>, attr, AttSmem<1, kOpSplit<MODE>>::kBytes));
+  CK(cudaFuncSetAttribute(attention_kernel<MODE, 2>, attr, AttSmem<2, kOpSplit<MODE>>::kBytes));
   if constexpr (!kOpSplit<MODE>) {
     // the larger of the two: the out-projection's pairs fit wherever FF2's do (the same threads and registers, less shared memory)
     cudaLaunchConfig_t cfg = {};
@@ -414,15 +417,15 @@ int set_smem(LdmHandle* h) {
   return LDM_OK;
 }
 
-// The per-batch workspace: each buffer holds per_layout bytes per layout.  ldm_debug_read reads a buffer by its name (nullptr: not
+// The per-batch workspace: each buffer holds per_layout bytes per layout (the row buffers: 128 R rows per layout).  ldm_debug_read reads a buffer by its name (nullptr: not
 // readable); a 16-bit operand (lo != nullptr) also has a lo plane in the split mode, read as "<name>_lo".
 struct WsBuf { const char* name; void** hi; void** lo; size_t per_layout; };
 std::vector<WsBuf> workspace_bufs(LdmHandle* h) {
-  const size_t d = h->desc.d_model, ff = h->desc.d_ff, S = h->S;
-  const auto op = [](const char* name, Op16& o, size_t cols) { return WsBuf{name, &o.hi, &o.lo, kBM * cols * 2}; };
+  const size_t d = h->desc.d_model, ff = h->desc.d_ff, S = h->S, rows = h->layout_rows();
+  const auto op = [rows](const char* name, Op16& o, size_t cols) { return WsBuf{name, &o.hi, &o.lo, rows * cols * 2}; };
   const auto buf = [](const char* name, auto** p, size_t per_layout) { return WsBuf{name, reinterpret_cast<void**>(p), nullptr, per_layout}; };
   return {op("x16", h->x16, d), op("qkv16", h->qkv16, kQkvN), op("att16", h->att16, kAttN), op("z16", h->z16, d), op("hid16", h->hid16, ff),
-          buf("x32", &h->x32, kBM * d * 4), buf("y32", &h->y32, kBM * d * 4), buf("logits", &h->logits, kBM * kLogitLd * 4),
+          buf("x32", &h->x32, rows * d * 4), buf("y32", &h->y32, rows * d * 4), buf("logits", &h->logits, rows * kLogitLd * 4),
           buf(nullptr, &h->ids[0], S * 8), buf(nullptr, &h->ids[1], S * 8), buf(nullptr, &h->ids_final, S * 8),
           buf(nullptr, &h->c_seq, S * 8), buf(nullptr, &h->c_seq_orig, S * 8), buf(nullptr, &h->c_mask, S)};
 }
@@ -442,7 +445,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   // free the old workspace: nothing may still be running on it, and a failed reallocation must not leave stale pointers behind
   CK(cudaDeviceSynchronize());
   free_workspace(h);
-  // every buffer is zeroed once: the 3 padding rows of every layout tile must stay finite.  An allocation that does not fit is
+  // every buffer is zeroed once: the padding rows S .. 128 R - 1 of every layout must stay finite.  An allocation that does not fit is
   // reported (not left as the runtime's last error) and releases what this call allocated
   for (const WsBuf& b : workspace_bufs(h)) {
     for (void** p : {b.hi, h->split ? b.lo : nullptr}) {
@@ -459,7 +462,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   }
   h->cap = n_layouts;
   h->ws_generation++;
-  const size_t M = static_cast<size_t>(n_layouts) * kBM;
+  const size_t M = static_cast<size_t>(n_layouts) * h->layout_rows();
   const int d = h->desc.d_model, ff = h->desc.d_ff;
   int rc;
   // the row-block GEMM's resident A k-blocks are the one-plane ring's (64 elements): QKV, FF1 and the head share these maps
@@ -484,7 +487,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
 template <int MODE>
 int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, cudaStream_t st, const int* t_layout = nullptr, bool skip_embed = false) {
   const int d = h->desc.d_model, ff = h->desc.d_ff, L = h->L, T = h->T;
-  const int M = n * kBM;
+  const int R = h->R, nb = n * R, M = nb * kBM;   // nb: 128-row blocks
   // Grids: the fp16 / bf16 row-block GEMMs (QKV, FF1) and LN GEMMs (epilogue warps) are persistent (one CTA per SM): their
   // epilogues run under the next tile's MMAs.  gemm_tc_kernel stores from the fragment, so a CTA has nothing to overlap its
   // epilogue with; one tile per CTA lets the hardware hand each SM its next tile the moment it is free, which measured faster
@@ -495,17 +498,18 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   };
   // QKV / FF1 (bias, q-scale | ReLU): the row-block kernel in fp16 / bf16, 128-row x 256-column tiles in the split mode.  The
   // row-block kernel cuts each row block into n_ranges column ranges, each loading the row block's A once: one range when the
-  // row blocks alone fill the SMs, otherwise enough for the items to fill them (at most one per tile); LDM_GEMM_SPLIT=g forces g
+  // row blocks alone fill the SMs, otherwise enough for the items to fill them (at most one per tile); LDM_GEMM_SPLIT=g forces g.
+  // Row blocks, not layouts, are counted: a layout of R tiles is R row blocks
   const auto plain_gemm = [&](auto epi, const OpMaps<MODE>& a, const OpMaps<MODE>& w, const CUtensorMap& out, GemmParams p) {
     constexpr int EPI = decltype(epi)::value;
     if constexpr (kOpSplit<MODE>) {
       p.n_tiles = (p.N + kPlainBN - 1) / kPlainBN;
-      return launch_step(h, kGemmPlainSplit<EPI, MODE>, grid(p.n_tiles * n, false), kGemmThreads, kPlainSmem, st, a, w, p);
+      return launch_step(h, kGemmPlainSplit<EPI, MODE>, grid(p.n_tiles * nb, false), kGemmThreads, kPlainSmem, st, a, w, p);
     } else {
       p.n_tiles = (p.N + kRbCols - 1) / kRbCols;
-      const int g = h->gemm_split > 0 ? h->gemm_split : n >= h->num_sms ? 1 : (h->num_sms + n - 1) / n;
+      const int g = h->gemm_split > 0 ? h->gemm_split : nb >= h->num_sms ? 1 : (h->num_sms + nb - 1) / nb;
       p.n_ranges = std::min(g, p.n_tiles);
-      return launch_step(h, gemm_rowblock_kernel<EPI, MODE>, grid(n * p.n_ranges, true), kRbThreads, RbSmem::kBytes, st, a, w, out, p);
+      return launch_step(h, gemm_rowblock_kernel<EPI, MODE>, grid(nb * p.n_ranges, true), kRbThreads, RbSmem::kBytes, st, a, w, out, p);
     }
   };
   // the LN GEMMs (out-projection, FF2): the fragment-epilogue kernel in the split mode, 64 whole rows per tile; otherwise the
@@ -515,7 +519,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     if constexpr (kOpSplit<MODE>) {
       return launch_step(h, kGemmLn<MODE>, grid(M / kLnSplitRows, false), kGemmThreads, kLnSmem, st, a, w, p);
     } else {
-      const int pairs = std::min({n, h->ln_clusters, h->gemm_ctas > 0 ? std::max(1, h->gemm_ctas / 2) : n});
+      const int pairs = std::min({nb, h->ln_clusters, h->gemm_ctas > 0 ? std::max(1, h->gemm_ctas / 2) : nb});
       if (p.K == kAttN) return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnOutStages>, dim3(2 * pairs), kLnThreads, LnOut::kBytes, st, a, w, res, st32, p);
       return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, res, st32, p);
     }
@@ -528,10 +532,10 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   // test tap: stop after `debug_stop_after` launches
 #define LDM_STAGE_DONE() do { if (h->debug_stop_after && ++done >= h->debug_stop_after) { CK(cudaGetLastError()); return LDM_OK; } } while (0)
   if (!skip_embed) {     // skipped inside the loop: the previous step's draw kernel has already written this step's x32 / x16 rows
-    const int warps = n * 128, blocks = (warps * 32 + 255) / 256;
+    const int warps = M, blocks = (warps * 32 + 255) / 256;    // one warp per row, pad rows included
     ProfScope ps(h, CAT_EMBED, st);
     CK(launch_step(h, embed_adaln_kernel<MODE>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
-                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16.hi, n, n, h->S, d, h->x16.lo));
+                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16.hi, n, R == 1 ? 7 : 8, h->S, d, h->x16.lo));
   }
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
@@ -544,8 +548,13 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     LDM_STAGE_DONE();
     {
       ProfScope ps(h, CAT_ATTN, st);
-      CK(launch_step(h, attention_kernel<MODE>, dim3(n * h->desc.n_heads), kAttThreads, kOpSplit<MODE> ? kAttSmemBytesSplit : kAttSmemBytes, st,
-                     h->qkv16.maps<MODE>(), h->att16.hi, h->S, h->desc.n_heads, n, next_rev(), h->att16.lo));
+      const dim3 items(nb * h->desc.n_heads);                // (layout, query tile, head)
+      if (R == 1)
+        CK(launch_step(h, attention_kernel<MODE, 1>, items, kAttThreads, AttSmem<1, kOpSplit<MODE>>::kBytes, st, h->qkv16.maps<MODE>(), h->att16.hi,
+                       h->S, h->desc.n_heads, n, next_rev(), h->att16.lo));
+      else
+        CK(launch_step(h, attention_kernel<MODE, 2>, items, kAttThreads, AttSmem<2, kOpSplit<MODE>>::kBytes, st, h->qkv16.maps<MODE>(), h->att16.hi,
+                       h->S, h->desc.n_heads, n, next_rev(), h->att16.lo));
     }
     LDM_STAGE_DONE();
     {  // out-projection + bias + residual (from the NORMALISED x) -> y32 ; z16 = LayerNorm2(y)   [fused epilogue]
@@ -567,7 +576,9 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       if (l + 1 < L) {
         const float* tab = h->adaln + (static_cast<size_t>(l + 1) * T + t_model) * 2 * d;
         p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16.hi; p.out_lo = h->x16.lo;
-        if (t_layout) { p.ln_scale = h->adaln + static_cast<size_t>(l + 1) * T * 2 * d; p.t_layout = t_layout; p.n_layouts = n; }   // per-layout rows
+        if (t_layout) {   // per-layout rows
+          p.ln_scale = h->adaln + static_cast<size_t>(l + 1) * T * 2 * d; p.t_layout = t_layout; p.n_layouts = n; p.layout_rows = h->layout_rows();
+        }
       } else {
         p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out32 = nullptr; p.out = h->z16.hi; p.out_lo = h->z16.lo;
       }
@@ -581,7 +592,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
     GemmParams p{M, kLogitLd, d, 1, nullptr, h->logits, kLogitLd, 1.0f, 0};
     p.rev = next_rev();
     ProfScope ps(h, CAT_HEAD, st);
-    CK(launch_step(h, kGemmHead<MODE>, grid(n, false), kGemmThreads, kHeadSmem, st, h->z16.maps<MODE>(), h->whead.maps<MODE>(), p));
+    CK(launch_step(h, kGemmHead<MODE>, grid(nb, false), kGemmThreads, kHeadSmem, st, h->z16.maps<MODE>(), h->whead.maps<MODE>(), p));
   }
 #undef LDM_STAGE_DONE
   CK(cudaGetLastError());
@@ -642,7 +653,7 @@ StepParams base_step_params(const LdmHandle* h, int B) {
     p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
   }
   p.T = h->T; p.sched = h->sched; p.lae = h->lae;
-  p.logits = h->logits; p.ld_logits = kLogitLd;
+  p.logits = h->logits; p.ld_logits = kLogitLd; p.layout_rows = h->layout_rows();
   p.mode = SAMP_DETERMINISTIC; p.temperature = 1.0f;
   return p;
 }
@@ -659,14 +670,14 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
   if (logprob_in == nullptr) {
     if (logits_in != nullptr) {
       ProfScope ps(h, CAT_MISC, st);
-      logits_scatter_kernel<<<1024, 256, 0, st>>>(logits_in, h->logits, B, h->S, h->C);
+      logits_scatter_kernel<<<1024, 256, 0, st>>>(logits_in, h->logits, B, h->S, h->C, h->layout_rows());
     } else {
       rc = run_denoiser(h, B, ids_in, t_model, st, nullptr, skip_embed);
       if (rc) return rc;
     }
     if (logits_out != nullptr) {
       ProfScope ps(h, CAT_MISC, st);
-      logits_gather_kernel<<<1024, 256, 0, st>>>(h->logits, logits_out, B, h->S, h->C);
+      logits_gather_kernel<<<1024, 256, 0, st>>>(h->logits, logits_out, B, h->S, h->C, h->layout_rows());
     }
   }
   StepParams p = base_step_params(h, B);
@@ -749,8 +760,10 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (d != kDModel || desc->n_heads != 8 || ff != 4 * kDModel)
     return fail(LDM_ERR_UNSUPPORTED, "kernels are built for d_model=464, 8 heads, d_ff=1856 (got %d, %d, %d)", d, desc->n_heads, ff);
   if (L < 1 || L > kMaxLayers || T < 2) return fail(LDM_ERR_UNSUPPORTED, "n_layers must be in [1,%d], T >= 2", kMaxLayers);
-  if (C < 129 || C > kLogitLd || S > 125 || S < 1 || desc->n_attr > kMaxAttr || desc->n_attr < 1)
-    return fail(LDM_ERR_UNSUPPORTED, "vocabulary C=%d must be in [129,160] and S=%d <= 125", C, S);
+  if (C < 129 || C > kLogitLd || S > kAttMaxR * kBM || S < 1 || desc->n_attr > kMaxAttr || desc->n_attr < 1)
+    return fail(LDM_ERR_UNSUPPORTED, "vocabulary C=%d must be in [129,160] and S=%d <= %d (a layout spans at most %d row tiles of %d tokens: "
+                "max_seq_length <= %d with %d attributes)", C, S, kAttMaxR * kBM, kAttMaxR, kBM, desc->n_attr > 0 ? kAttMaxR * kBM / desc->n_attr : 0,
+                desc->n_attr);
   if (desc->q_type != 0 && desc->q_type != 1) return fail(LDM_ERR_INVALID, "q_type must be 0 (constrained) or 1 (vanilla)");
   if (desc->q_type == 0 && desc->n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "constrained q_type needs the c-x-y-w-h layout (5 attributes)");
   if (desc->operand_dtype < OP_F16 || desc->operand_dtype > OP_BF16X3)
@@ -764,6 +777,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
 
   LdmHandle* h = new LdmHandle();
   h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T;
+  h->R = (S + kBM - 1) / kBM;
   h->mode = desc->operand_dtype; h->bf16 = h->mode != OP_F16; h->split = h->mode == OP_BF16X3;
   h->G = desc->q_type == 0 ? desc->n_attr : 1;
   if (const char* e = getenv("LDM_PDL")) h->pdl = atoi(e);
@@ -1164,7 +1178,7 @@ int ldm_predict_start(LdmHandle* h, int32_t B, const int64_t* xt_ids, const int3
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = run_denoiser_per_layout_t(h, B, reinterpret_cast<const long long*>(xt_ids), t_dev, st);
   if (rc) return rc;
-  if (logits_out) { ProfScope ps(h, CAT_MISC, st); logits_gather_kernel<<<1024, 256, 0, st>>>(h->logits, logits_out, B, h->S, h->C); }
+  if (logits_out) { ProfScope ps(h, CAT_MISC, st); logits_gather_kernel<<<1024, 256, 0, st>>>(h->logits, logits_out, B, h->S, h->C, h->layout_rows()); }
   StepParams p = base_step_params(h, B);
   p.ids_in = reinterpret_cast<const long long*>(xt_ids); p.t_layout = t_dev; p.lx0_out = log_x0_out;   // ids_out == nullptr: no draw
   const int blocks = (B * h->S * 32 + 255) / 256;

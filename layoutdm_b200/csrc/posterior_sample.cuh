@@ -29,7 +29,8 @@ struct StepParams {
   int T, t_post;
   const float* sched;                    // [G][8][T+1]
   const float* lae;                      // [G][T+1][4] log_add_exp terms that depend on (group, t) only (lae_table_kernel)
-  const float* logits; int ld_logits;    // [n_layouts*128][ld]; row = b*128 + s      (nullptr if logprob_in)
+  const float* logits; int ld_logits;    // [n_layouts*layout_rows][ld]; row = b*layout_rows + s      (nullptr if logprob_in)
+  int layout_rows;                       // rows per layout of the logits and of the fused embedding's x32 / x16: 128 R
   const float* logprob_in;               // [n_layouts][S][C] or nullptr: draw from given log-probs (relation hook)
   const float* lx0_in;                   // [n_layouts][S][C] or nullptr: log p(x0) given by the caller instead of predict_start(logits)
                                          // (q_posterior as a callable API, constrained.py:135-206; the MASK column is ignored like :191)
@@ -77,7 +78,7 @@ __global__ void lae_table_kernel(const float* __restrict__ sched, float* __restr
 // the drawn token's row of the next step's denoiser input (see StepParams::emb_*); best_c is warp-uniform
 LDM_DEVINL void embed_next(const StepParams& p, const int b, const int s, const int best_c, const int lane) {
   if (p.emb_adaln == nullptr) return;
-  const size_t row = static_cast<size_t>(b) * 128 + s;
+  const size_t row = static_cast<size_t>(b) * p.layout_rows + s;
   if (p.emb_bf16) embed_token_row<true>(best_c, s, row, p.emb_cat, p.emb_pos, p.emb_adaln, p.emb_x32, p.emb_x16, p.emb_d, lane);
   else embed_token_row<false>(best_c, s, row, p.emb_cat, p.emb_pos, p.emb_adaln, p.emb_x32, p.emb_x16, p.emb_d, lane);
 }
@@ -276,7 +277,7 @@ LDM_DEVINL void posterior_token_generic(const StepParams& p, const int token, co
 #pragma unroll
       for (int j = 0; j < 5; ++j) lx0[j] = valid[j] ? p.lx0_in[static_cast<size_t>(token) * C + cls[j]] : -70.0f;
     } else {
-      predict_start_token(p, p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits, lane, cls, valid, lx0);
+      predict_start_token(p, p.logits + (static_cast<size_t>(b) * p.layout_rows + s) * p.ld_logits, lane, cls, valid, lx0);
     }
     if (p.lx0_out != nullptr) {
 #pragma unroll
@@ -401,7 +402,7 @@ LDM_DEVINL bool posterior_token_group(const StepParams& p, const int token, cons
   }
 
   // ---- predict_start: the log-sum-exp over all classes, log p(x0) of the group's ----
-  const float* lrow = p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits;
+  const float* lrow = p.logits + (static_cast<size_t>(b) * p.layout_rows + s) * p.ld_logits;
   int lcls[5]; bool lvalid[5];
   lane_classes(C, lane, lcls, lvalid);
   float l[5];
@@ -591,7 +592,7 @@ __global__ void __launch_bounds__(256) vb_terms_kernel(const VbParams v) {
 #pragma unroll
   for (int j = 0; j < 5; ++j) lxs[j] = (cls[j] == x0) ? 0.0f : kLogEps;            // index_to_log_onehot (util.py:34-40)
   posterior_token_logprob(p, s, x_t, t, lxs, cls, valid, ltp);
-  predict_start_token(p, p.logits + (static_cast<size_t>(b) * 128 + s) * p.ld_logits, lane, cls, valid, lx0);
+  predict_start_token(p, p.logits + (static_cast<size_t>(b) * p.layout_rows + s) * p.ld_logits, lane, cls, valid, lx0);
   posterior_token_logprob(p, s, x_t, t, lx0, cls, valid, lmp);
   float kl = 0.0f, nll = 0.0f, aux = 0.0f;
 #pragma unroll

@@ -20,8 +20,12 @@ import torch.nn.functional as F
 from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import _lib
-from .engine import Engine, sampling_struct
+from .engine import Engine, layout_length, sampling_struct
 from .vocab import Vocab, decode_ids, group_full_ids, linear_centers, refinement_table, relation_edge_table, timestep_plan
+
+
+# nodes of one layout's graph the on-device relation update holds: the canvas plus 31 elements (kRelMaxNodes, relation.cuh)
+RELATION_MAX_NODES = 32
 
 
 def _cfg_get(cfg, key, default=None):
@@ -169,9 +173,12 @@ class FusedMaskAndReplaceDiffusion:
                                                     _cfg_get(sampling_cfg, "refine_offset_ratio", 0.1),
                                                     _cfg_get(sampling_cfg, "refine_lambda", 3.0))
         if self.relation_on_device and cond.get("type") == "relation" and "batch_w_canvas" in cond and "rel_adj" not in cond \
+                and self.vocab.n_elem + 1 <= RELATION_MAX_NODES \
                 and _cfg_get(sampling_cfg, "relation_mode", "average") == "average" and float(_cfg_get(sampling_cfg, "relation_lambda", 0.0)) > 0.0:
             # logit_adjustment.update (:88-126) on the device: dense edge table + bin centres + SGD hyper-parameters.
-            # relation_mode "gumbel" draws torch noise inside the update and stays on the reference's autograd path (logit_adjust_fn).
+            # relation_mode "gumbel" draws torch noise inside the update and stays on the reference's autograd path (logit_adjust_fn),
+            # and so does a layout of more elements than the update kernel holds (the canvas + 31): without rel_adj the step
+            # takes the log-prob hook path.
             cond["rel_adj"] = relation_edge_table(cond["batch_w_canvas"], cond["seq"].size(0), self.vocab.n_elem + 1)
             cond["rel_centers"] = torch.stack([torch.as_tensor(c, dtype=torch.float32).view(-1) for c in self.bbox_centers])
             cond["rel_lambda"] = float(_cfg_get(sampling_cfg, "relation_lambda", 3e6))
@@ -468,11 +475,22 @@ class LayoutDMB200:
 
     @classmethod
     def from_state_dict(cls, sd, dataset: str = "rico25", num_timesteps: int = 100, q_type: str = "constrained",
-                        operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None, noise: str = "contract") -> "LayoutDMB200":
-        """noise: "contract" (the project's Philox contract) or "torch" (torch's CUDA generator, FusedMaskAndReplaceDiffusion)"""
-        vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else Vocab.for_dataset(dataset)
+                        operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None, noise: str = "contract",
+                        max_seq_length: Optional[int] = None) -> "LayoutDMB200":
+        """noise: "contract" (the project's Philox contract) or "torch" (torch's CUDA generator, FusedMaskAndReplaceDiffusion).
+        The layout length comes from the tokenizer if given, else from the state_dict's positional table (`layout_length`);
+        an explicit max_seq_length must agree with the table."""
+        vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else cls.vocab_for(sd, dataset, max_seq_length)
         eng = Engine.from_state_dict(sd, vocab, num_timesteps=num_timesteps, q_type=q_type, operand_dtype=operand_dtype, device=device)
         return cls(eng, tokenizer, bbox_centers, noise=noise)
+
+    @staticmethod
+    def vocab_for(sd, dataset: str = "rico25", max_seq_length: Optional[int] = None) -> Vocab:
+        """the dataset's vocabulary at the layout length the state_dict was trained for"""
+        n = layout_length(sd)
+        if max_seq_length is not None and int(max_seq_length) != n:
+            raise ValueError(f"max_seq_length={max_seq_length}, but the state_dict's positional table is for {n} elements")
+        return Vocab.for_dataset(dataset, n)
 
     def eval(self):
         return self

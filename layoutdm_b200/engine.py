@@ -20,6 +20,20 @@ def _find_prefix(sd) -> str:
     raise KeyError("state_dict does not contain '<prefix>cat_emb.weight' (expected the reference's LayoutDM keys)")
 
 
+def layout_length(sd) -> int:
+    """the layout length (max_seq_length, elements per layout) a reference state_dict was trained for: the rows of its
+    ElementPositionalEmbedding's element table, or those of its PositionalEmbedding's token table / 5 (nn_lib.py:73-127)"""
+    p = _find_prefix(sd)
+    if p + "pos_emb.elem_emb" in sd:
+        return int(sd[p + "pos_emb.elem_emb"].shape[0])
+    if p + "pos_emb.pos_emb" in sd:
+        rows = int(sd[p + "pos_emb.pos_emb"].shape[0])
+        if rows % 5:
+            raise ValueError(f"pos_emb.pos_emb has {rows} rows, not 5 tokens (c-x-y-w-h) per element")
+        return rows // 5
+    raise KeyError("state_dict has no positional table ('<prefix>pos_emb.elem_emb' or '<prefix>pos_emb.pos_emb')")
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
 
@@ -70,6 +84,11 @@ class Engine:
         _lib.check(self.lib.ldm_create(C.byref(desc), C.byref(w), C.byref(h)))
         self._h = h
 
+    @property
+    def layout_rows(self) -> int:
+        """rows a layout takes in the workspace (ldm_debug_read): 128 R, R = ceil(S / 128) row tiles; rows S .. are pad rows"""
+        return 128 * ((self.vocab.S + 127) // 128)
+
     # ------------------------------------------------------------------------------------------------
     @classmethod
     def from_state_dict(cls, sd: Dict[str, torch.Tensor], vocab: Vocab, num_timesteps: int = 100, **kw) -> "Engine":
@@ -87,10 +106,16 @@ class Engine:
         while f"{p}backbone.layers.{L}.linear1.weight" in sd:
             L += 1
         st = lambda k: torch.stack([g(f"backbone.layers.{l}.{k}") for l in range(L)]).contiguous()
+        if p + "pos_emb.elem_emb" in sd and sd[p + "pos_emb.elem_emb"].shape[0] != vocab.n_elem:
+            raise ValueError(f"the state_dict's positional table is for {sd[p + 'pos_emb.elem_emb'].shape[0]} elements, the vocabulary "
+                             f"has {vocab.n_elem}: a model of another max_seq_length")
         if p + "pos_emb.elem_emb" in sd:      # ElementPositionalEmbedding, nn_lib.py:112-127
             pos = (g("pos_emb.elem_emb").repeat_interleave(vocab.n_attr, dim=0) + g("pos_emb.attr_emb").repeat(vocab.n_elem, 1))[: vocab.S]
         else:                                  # PositionalEmbedding, nn_lib.py:73-88
             pos = g("pos_emb.pos_emb")[: vocab.S]
+        if pos.shape[0] != vocab.S:
+            raise ValueError(f"the state_dict's positional table covers {pos.shape[0]} tokens, the vocabulary has S = {vocab.S} "
+                             f"({vocab.n_elem} elements): a model of another max_seq_length")
         return dict(
             cat_emb=g("cat_emb.weight"), pos_table=pos.contiguous(),
             in_proj_w=st("self_attn.in_proj_weight"), in_proj_b=st("self_attn.in_proj_bias"),

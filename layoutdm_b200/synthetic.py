@@ -43,7 +43,7 @@ def random_state_dict(vocab: Vocab, num_timesteps: int = 100, d: int = 464, ff: 
 
 
 def synthetic_cond(vocab: Vocab, B: int, cond_type: str = "c", seed: int = 0, refine: Optional[dict] = None) -> Dict:
-    """cond dict for `c` / `cwh` / `refinement` built from random layouts (n_elem ~ U{1..25}, labels uniform, boxes uniform,
+    """cond dict for `c` / `cwh` / `refinement` built from random layouts (n_elem ~ U{1..vocab.n_elem}, labels uniform, boxes uniform,
     linear quantisation), following get_cond (task.py:94-110, 126-140) and tokenizer.encode (layout_tokenizer.py:208-253)."""
     assert cond_type in ("c", "cwh", "refinement")
     g = torch.Generator().manual_seed(seed)

@@ -24,8 +24,9 @@ class Vocab:
     n_attr: int = 5
 
     @classmethod
-    def for_dataset(cls, name: str) -> "Vocab":
-        return cls(n_cat=DATASET_NUM_CATEGORIES[name])
+    def for_dataset(cls, name: str, max_seq_length: int = 25) -> "Vocab":
+        """the dataset's vocabulary for layouts of up to `max_seq_length` elements (config/dataset/*.yaml: dataset.max_seq_length)"""
+        return cls(n_cat=DATASET_NUM_CATEGORIES[name], n_elem=int(max_seq_length))
 
     @classmethod
     def from_tokenizer(cls, tok) -> "Vocab":
