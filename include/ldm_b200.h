@@ -34,10 +34,12 @@ extern "C" {
 typedef struct LdmHandle LdmHandle;
 
 /* Model description: tokenizer vocabulary (layout_tokenizer.py:79-82,296-313) + denoiser dims
- * (config/backbone/medium.yaml shrunk by 29/32, layoutdm.py:54) + diffusion schedule (base.py:35-69). */
+ * (config/backbone/medium.yaml shrunk by 29/32, layoutdm.py:54) + diffusion schedule (base.py:35-69).
+ * The vocabulary holds C = n_cat + (bbox_vocab ? 1 : 4) * n_bins + 2 ids (categories, bbox bins, PAD, MASK); the kernels are
+ * built for C <= 160 with n_cat >= 1 and n_bins >= 2 (LDM_ERR_UNSUPPORTED otherwise). */
 typedef struct {
   int32_t n_cat;          /* 25 rico25, 5 publaynet */
-  int32_t n_bins;         /* 32 */
+  int32_t n_bins;         /* num_bin_bboxes: 32 by default */
   int32_t n_elem;         /* max_seq_length: 25 by default; S = n_elem * n_attr <= 256 (51 elements of c-x-y-w-h) */
   int32_t n_attr;         /* 5  (c,x,y,w,h) */
   int32_t d_model;        /* 464 */
@@ -52,10 +54,14 @@ typedef struct {
                              other values: LDM_ERR_INVALID */
   int32_t device;         /* CUDA device ordinal */
   double att_1, att_T, ctt_1, ctt_T;  /* alpha_schedule() endpoints, util.py:47-49 */
+  int32_t bbox_vocab;     /* shared_bbox_vocab (bbox_tokenizer.py:17-20): 0 = "x-y-w-h" (x, y, w, h take n_bins ids each, in
+                             that order), 1 = "xywh" (the four share one range of n_bins ids); other values: LDM_ERR_INVALID */
+  int32_t var_order;      /* var_order of an element's token slots: 0 = "c-x-y-w-h", 1 = "c-w-h-x-y" (needs n_attr = 5);
+                             other values: LDM_ERR_INVALID */
 } LdmModelDesc;
 
 /* fp32 arrays (host for ldm_create, device for ldm_load_weights) in the reference's own parameter layout (state_dict, SURVEY.md 8a-a5), layers stacked on dim 0.
- * C = n_cat + 4*n_bins + 2, S = n_elem*n_attr, d = d_model, f = d_ff, L = n_layers, T = num_timesteps. */
+ * C = n_cat + (bbox_vocab ? 1 : 4)*n_bins + 2, S = n_elem*n_attr, d = d_model, f = d_ff, L = n_layers, T = num_timesteps. */
 typedef struct {
   const float* cat_emb;      /* [C][d]        transformer.cat_emb.weight */
   const float* pos_table;    /* [S][d]        elem_emb[s/5] + attr_emb[s%5]  (or pos_emb[s]) */
@@ -88,7 +94,9 @@ typedef struct {
    * `update` (logit_adjustment.py:88-126; relation_mode "average").  rel_adj == NULL: off. */
   const int32_t* rel_adj;      /* [B][1+n_elem][1+n_elem] edge_attr bit masks (data/util.py:14-27) of the edge i -> j of
                                   cond["batch_w_canvas"], node 0 = canvas (AddCanvasElement), 0 = no edge */
-  const float* rel_centers;    /* [4][n_bins] bbox bin centres (x, y, w, h) or NULL = linear quantisation */
+  const float* rel_centers;    /* [4][n_bins] bbox bin centres (x, y, w, h) or NULL = linear quantisation.
+                                  The update holds one bin per lane and reads slot 1+a as variable a: it needs var_order
+                                  c-x-y-w-h, n_bins <= 32 and n_elem <= 31 (LDM_ERR_UNSUPPORTED otherwise) */
   float rel_lambda;            /* sampling_cfg.relation_lambda: SGD learning rate (logit_adjustment.py:101-103) */
   int32_t rel_num_update;      /* sampling_cfg.relation_num_update (applied for t_model >= 10 only, :105) */
   int32_t rel_batch_total;     /* batch size the reference's loss.mean() runs over (the GLOBAL batch when sharded); <= 0: B */

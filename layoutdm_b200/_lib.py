@@ -16,10 +16,16 @@ SAMPLING_MODES = {"deterministic": 0, "random": 1, "top_k": 2, "top_p": 3, "gumb
 OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "bf16x3": 2}
 
 
+# LdmModelDesc.bbox_vocab / var_order: the tokenizer's shared_bbox_vocab and var_order (helpers/layout_tokenizer.py:16-20)
+BBOX_VOCABS = {"x-y-w-h": 0, "xywh": 1}
+VAR_ORDERS = {"c-x-y-w-h": 0, "c-w-h-x-y": 1}
+
+
 class LdmModelDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_cat", "n_bins", "n_elem", "n_attr", "d_model", "n_heads", "d_ff", "n_layers",
                                          "num_timesteps", "q_type", "operand_dtype", "device")] + \
-               [(n, C.c_double) for n in ("att_1", "att_T", "ctt_1", "ctt_T")]
+               [(n, C.c_double) for n in ("att_1", "att_T", "ctt_1", "ctt_T")] + \
+               [(n, C.c_int32) for n in ("bbox_vocab", "var_order")]
 
 
 _W_FIELDS = ("cat_emb", "pos_table", "in_proj_w", "in_proj_b", "out_proj_w", "out_proj_b", "linear1_w", "linear1_b",

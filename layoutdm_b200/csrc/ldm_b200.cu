@@ -157,6 +157,7 @@ struct Op16 {
 struct LdmHandle {
   LdmModelDesc desc;
   int C = 0, S = 0, L = 0, T = 0, G = 0;
+  TokenLayout tl{};           // what each token slot holds (token_layout): the one place that knows the vocabulary layout
   int R = 1;                  // row tiles of kBM rows per layout: ceil(S / 128), 1 or 2.  Every row map and grid reads it
   int layout_rows() const { return kBM * R; }
   int mode = OP_F16;          // operand mode (LdmModelDesc::operand_dtype)
@@ -643,15 +644,29 @@ int validate_noise(const LdmHandle* h, int B, int64_t b_global0, const LdmNoise*
   return LDM_OK;
 }
 
+// The token layout of a model description (bbox_tokenizer.py:17-20,105-113; layout_tokenizer.py:296-313): slot 0 is the
+// category, slots 1..4 the bbox variables in var_order; a bbox variable's ids start at n_cat, plus its index in x, y, w, h times
+// n_bins unless the vocabulary is shared.  Slots past the fifth (n_attr > 5, var_order 0 only) continue the per-variable ranges.
+TokenLayout token_layout(const LdmModelDesc& d) {
+  static const int kOrder[2][4] = {{1, 2, 3, 4}, {3, 4, 1, 2}};     // c-x-y-w-h, c-w-h-x-y
+  TokenLayout tl{};
+  tl.n_attr = d.n_attr; tl.n_cat = d.n_cat; tl.n_bins = d.n_bins;
+  tl.n_bbox_ids = (d.bbox_vocab ? 1 : 4) * d.n_bins;
+  for (int k = 0; k < d.n_attr && k < kMaxAttr; ++k) {
+    const int var = k == 0 ? 0 : (k <= 4 ? kOrder[d.var_order][k - 1] : k);
+    tl.var[k] = var;
+    tl.start[k] = var == 0 ? 0 : d.n_cat + (d.bbox_vocab ? 0 : (var - 1) * d.n_bins);
+    tl.n[k] = var == 0 ? d.n_cat : d.n_bins;
+  }
+  return tl;
+}
+
 StepParams base_step_params(const LdmHandle* h, int B) {
   StepParams p{};
   p.n_layouts = B; p.S = h->S; p.C = h->C; p.n_attr = h->desc.n_attr;
   p.pad_id = h->C - 2; p.mask_id = h->C - 1;
   p.constrained = h->desc.q_type == 0;
-  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) {
-    p.grp_start[g] = g == 0 ? 0 : h->desc.n_cat + (g - 1) * h->desc.n_bins;
-    p.grp_n[g] = g == 0 ? h->desc.n_cat : h->desc.n_bins;
-  }
+  for (int g = 0; g < h->desc.n_attr && g < kMaxAttr; ++g) { p.grp_start[g] = h->tl.start[g]; p.grp_n[g] = h->tl.n[g]; }
   p.T = h->T; p.sched = h->sched; p.lae = h->lae;
   p.logits = h->logits; p.ld_logits = kLogitLd; p.layout_rows = h->layout_rows();
   p.mode = SAMP_DETERMINISTIC; p.temperature = 1.0f;
@@ -708,8 +723,8 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
   //   3. draw kernel from rel_lp with PAD-disable.  `update` does nothing for t < 10 (logit_adjustment.py:105): plain path then.
   const bool relation = cond && cond->seq && cond->rel_adj && logprob_in == nullptr && cond->rel_num_update > 0 && t_model >= 10;
   if (relation) {
-    if (h->desc.n_attr != 5 || h->desc.n_elem + 1 > kRelMaxNodes || h->desc.n_bins > 32)
-      return fail(LDM_ERR_UNSUPPORTED, "relation update needs the c-x-y-w-h layout with <= 31 elements and <= 32 bins");
+    if (h->desc.n_attr != 5 || h->desc.var_order != 0 || h->desc.n_elem + 1 > kRelMaxNodes || h->desc.n_bins > 32)
+      return fail(LDM_ERR_UNSUPPORTED, "relation update needs var_order c-x-y-w-h, <= 31 elements and <= 32 bins (take the log-prob hook otherwise)");
     if (!h->rel_lp) CK(cudaMalloc(reinterpret_cast<void**>(&h->rel_lp), static_cast<size_t>(h->cap) * h->S * h->C * sizeof(float)));
     StepParams p1 = p;
     p1.cond_flags &= ~COND_PAD_DISABLE; p1.logprob_out = h->rel_lp; p1.emb_adaln = nullptr;    // its draw is discarded: no embedding
@@ -720,6 +735,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
     RelationParams r{};
     r.n_layouts = B; r.S = h->S; r.C = h->C; r.n_attr = h->desc.n_attr; r.n_elem = h->desc.n_elem; r.n_cat = h->desc.n_cat;
     r.n_bins = h->desc.n_bins; r.pad_id = h->C - 2; r.lp = h->rel_lp; r.cond_seq = p.cond_seq; r.adj = cond->rel_adj; r.centers = cond->rel_centers;
+    for (int a = 0; a < 4; ++a) r.bin_start[a] = h->tl.start[1 + a];
     const int btot = cond->rel_batch_total > 0 ? cond->rel_batch_total : B;
     r.step = cond->rel_lambda / static_cast<float>(btot * 14);            // len(const.relation) = 14 cost functions (const.py:226-241)
     r.n_update = cond->rel_num_update;
@@ -751,19 +767,26 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
 extern "C" {
 
 const char* ldm_last_error(void) { return g_err; }
-const char* ldm_version(void) { return "ldm_b200 0.2 (sm_90a, wgmma)"; }
+const char* ldm_version(void) { return "ldm_b200 0.3 (sm_90a, wgmma)"; }
 
 int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (!desc || !w || !out) return fail(LDM_ERR_INVALID, "null argument");
   const int d = desc->d_model, ff = desc->d_ff, L = desc->n_layers, T = desc->num_timesteps;
-  const int C = desc->n_cat + 4 * desc->n_bins + 2, S = desc->n_elem * desc->n_attr;
+  if (desc->bbox_vocab != 0 && desc->bbox_vocab != 1)
+    return fail(LDM_ERR_INVALID, "bbox_vocab must be 0 (x-y-w-h) or 1 (shared xywh), got %d", desc->bbox_vocab);
+  if (desc->var_order != 0 && desc->var_order != 1)
+    return fail(LDM_ERR_INVALID, "var_order must be 0 (c-x-y-w-h) or 1 (c-w-h-x-y), got %d", desc->var_order);
+  if (desc->var_order != 0 && desc->n_attr != 5) return fail(LDM_ERR_INVALID, "var_order c-w-h-x-y needs 5 attributes (got %d)", desc->n_attr);
+  const int C = desc->n_cat + (desc->bbox_vocab ? 1 : 4) * desc->n_bins + 2, S = desc->n_elem * desc->n_attr;
   if (d != kDModel || desc->n_heads != 8 || ff != 4 * kDModel)
     return fail(LDM_ERR_UNSUPPORTED, "kernels are built for d_model=464, 8 heads, d_ff=1856 (got %d, %d, %d)", d, desc->n_heads, ff);
   if (L < 1 || L > kMaxLayers || T < 2) return fail(LDM_ERR_UNSUPPORTED, "n_layers must be in [1,%d], T >= 2", kMaxLayers);
-  if (C < 129 || C > kLogitLd || S > kAttMaxR * kBM || S < 1 || desc->n_attr > kMaxAttr || desc->n_attr < 1)
-    return fail(LDM_ERR_UNSUPPORTED, "vocabulary C=%d must be in [129,160] and S=%d <= %d (a layout spans at most %d row tiles of %d tokens: "
-                "max_seq_length <= %d with %d attributes)", C, S, kAttMaxR * kBM, kAttMaxR, kBM, desc->n_attr > 0 ? kAttMaxR * kBM / desc->n_attr : 0,
-                desc->n_attr);
+  if (desc->n_cat < 1 || desc->n_bins < 2 || C > kLogitLd)
+    return fail(LDM_ERR_UNSUPPORTED, "vocabulary C=%d: the kernels hold at most C = %d classes (the padded logits row), with n_cat >= 1 "
+                "and n_bins >= 2 (got n_cat=%d, n_bins=%d)", C, kLogitLd, desc->n_cat, desc->n_bins);
+  if (S > kAttMaxR * kBM || S < 1 || desc->n_attr > kMaxAttr || desc->n_attr < 1)
+    return fail(LDM_ERR_UNSUPPORTED, "the kernels need S=%d <= %d (a layout spans at most %d row tiles of %d tokens: max_seq_length <= %d "
+                "with %d attributes)", S, kAttMaxR * kBM, kAttMaxR, kBM, desc->n_attr > 0 ? kAttMaxR * kBM / desc->n_attr : 0, desc->n_attr);
   if (desc->q_type != 0 && desc->q_type != 1) return fail(LDM_ERR_INVALID, "q_type must be 0 (constrained) or 1 (vanilla)");
   if (desc->q_type == 0 && desc->n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "constrained q_type needs the c-x-y-w-h layout (5 attributes)");
   if (desc->operand_dtype < OP_F16 || desc->operand_dtype > OP_BF16X3)
@@ -777,6 +800,7 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
 
   LdmHandle* h = new LdmHandle();
   h->desc = *desc; h->C = C; h->S = S; h->L = L; h->T = T;
+  h->tl = token_layout(*desc);
   h->R = (S + kBM - 1) / kBM;
   h->mode = desc->operand_dtype; h->bf16 = h->mode != OP_F16; h->split = h->mode == OP_BF16X3;
   h->G = desc->q_type == 0 ? desc->n_attr : 1;
@@ -1126,14 +1150,14 @@ int ldm_q_sample(LdmHandle* h, int32_t B, const int64_t* x0, const int32_t* t, u
 
 int ldm_decode(LdmHandle* h, int32_t B, const int64_t* ids, const float* centers, float* bbox, int64_t* label, uint8_t* mask, void* stream) {
   if (!h || !ids || !bbox || !label || !mask || B <= 0) return fail(LDM_ERR_INVALID, "bad ldm_decode arguments");
-  if (h->desc.n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "decode needs the c-x-y-w-h token layout");
+  if (h->desc.n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "decode needs 5 token slots per element (c and x, y, w, h)");
   CK(cudaSetDevice(h->desc.device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int n = B * h->desc.n_elem;
   {
     ProfScope ps(h, CAT_MISC, st);
     decode_kernel<<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const long long*>(ids), centers, bbox, reinterpret_cast<long long*>(label), mask,
-                                                  B, h->desc.n_elem, h->desc.n_attr, h->desc.n_cat, h->desc.n_bins);
+                                                  B, h->desc.n_elem, h->tl);
   }
   CK(cudaGetLastError());
   return LDM_OK;
@@ -1142,7 +1166,7 @@ int ldm_decode(LdmHandle* h, int32_t B, const int64_t* ids, const float* centers
 int ldm_make_cond(LdmHandle* h, int32_t B, int32_t cond_type, const int64_t* label, const float* bbox, const uint8_t* elem_mask,
                   const float* centers, int64_t* seq, uint8_t* mask, int64_t* seq_orig, void* stream) {
   if (!h || !label || !bbox || !elem_mask || !seq || !mask || B <= 0) return fail(LDM_ERR_INVALID, "bad ldm_make_cond arguments");
-  if (h->desc.n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "make_cond needs the c-x-y-w-h token layout");
+  if (h->desc.n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "make_cond needs 5 token slots per element (c and x, y, w, h)");
   if (cond_type < COND_TYPE_C || cond_type > COND_TYPE_GT)
     return fail(LDM_ERR_UNSUPPORTED, "cond_type %d: only c / cwh / refinement / gt are built on the device (task.py:27-151 raises NotImplementedError for unknown types)", cond_type);
   if (cond_type == COND_TYPE_REFINEMENT && !seq_orig) return fail(LDM_ERR_INVALID, "refinement needs seq_orig_out");
@@ -1155,7 +1179,7 @@ int ldm_make_cond(LdmHandle* h, int32_t B, int32_t cond_type, const int64_t* lab
     make_cond_kernel<<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const long long*>(label), bbox, elem_mask, centers,
                                                      reinterpret_cast<long long*>(seq), mask,
                                                      cond_type == COND_TYPE_REFINEMENT ? reinterpret_cast<long long*>(seq_orig) : nullptr, B,
-                                                     h->desc.n_elem, h->desc.n_cat, h->desc.n_bins, h->C - 2, h->C - 1, cond_type,
+                                                     h->desc.n_elem, h->tl, h->C - 2, h->C - 1, cond_type,
                                                      static_cast<float>(dd), static_cast<float>(1.0 - dd));
   }
   CK(cudaGetLastError());

@@ -22,6 +22,16 @@ enum : int { SAMP_DETERMINISTIC = 0, SAMP_RANDOM = 1, SAMP_TOP_K = 2, SAMP_TOP_P
 enum : int { COND_HAS_MASK = 1, COND_PAD_DISABLE = 2, COND_REFINE = 4 };
 constexpr int kMaxAttr = 8;
 
+// The token layout (LayoutSequenceTokenizer / BboxTokenizer, T/helpers/layout_tokenizer.py:296-313, bbox_tokenizer.py:84-135):
+// slot k of an element's n_attr tokens carries variable var[k] (0 = c, 1..4 = x, y, w, h) and draws from the full-vocabulary
+// ids [start[k], start[k] + n[k]) plus PAD and MASK.  The bbox ids are [n_cat, n_cat + n_bbox_ids): n_bbox_ids = 4 n_bins with
+// per-variable ranges (x-y-w-h) or n_bins shared by all four (xywh).  ldm_create builds it once; the step kernels' vocabulary
+// groups, decode, make_cond and the relation update read it.
+struct TokenLayout {
+  int n_attr, n_cat, n_bins, n_bbox_ids;
+  int var[kMaxAttr], start[kMaxAttr], n[kMaxAttr];
+};
+
 struct StepParams {
   int n_layouts, S, C, n_attr, pad_id, mask_id;
   int constrained;                       // 1: per-attribute groups, 0: vanilla (single group over all classes)
@@ -710,20 +720,24 @@ __global__ void __launch_bounds__(256) q_sample_kernel(const StepParams p, const
 // ---------------------------------------------------------------------------------------------------------
 // ids -> layouts on the device: LayoutSequenceTokenizer.decode (T/helpers/layout_tokenizer.py:255-266, :106-114) +
 // BboxTokenizer.decode (T/helpers/bbox_tokenizer.py:117-174).  One thread per element; centers == nullptr: linear bins.
+// An element is valid when its label is a category and every bbox slot holds a bbox id (any of the n_bbox_ids, whatever its
+// variable); each slot's bin is its id minus the first id of its variable, clamped, and lands at its variable's place in xywh.
 __global__ void decode_kernel(const long long* __restrict__ ids, const float* __restrict__ centers /*[4][n_bins] or null*/,
                               float* __restrict__ bbox /*[B][E][4]*/, long long* __restrict__ label /*[B][E]*/,
-                              unsigned char* __restrict__ mask /*[B][E]*/, int n_layouts, int n_elem, int n_attr, int n_cat, int n_bins) {
+                              unsigned char* __restrict__ mask /*[B][E]*/, int n_layouts, int n_elem, const TokenLayout tl) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_layouts * n_elem) return;
-  const long long* tk = ids + static_cast<size_t>(i) * n_attr;
+  const int n_bins = tl.n_bins;
+  const long long* tk = ids + static_cast<size_t>(i) * tl.n_attr;
   const long long lab = tk[0];
-  bool valid = lab >= 0 && lab < n_cat;
+  bool valid = lab >= 0 && lab < tl.n_cat;
   float bb[4];
 #pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const long long v = tk[1 + a] - n_cat;                                // shared_bbox_vocab x-y-w-h: 4 * n_bins ids
-    valid = valid && v >= 0 && v < 4LL * n_bins;
-    long long bin = v - static_cast<long long>(a) * n_bins;
+  for (int k = 1; k < 5; ++k) {
+    const long long v = tk[k] - tl.n_cat;
+    valid = valid && v >= 0 && v < tl.n_bbox_ids;
+    const int a = tl.var[k] - 1;                                          // x, y, w, h
+    long long bin = tk[k] - tl.start[k];
     bin = bin < 0 ? 0 : (bin > n_bins - 1 ? n_bins - 1 : bin);            // clamp (avoid OOV)
     if (centers != nullptr) bb[a] = fminf(fmaxf(centers[a * n_bins + bin], 0.0f), 1.0f);
     else bb[a] = static_cast<float>(a < 2 ? bin : bin + 1) * (1.0f / n_bins);
@@ -743,15 +757,15 @@ enum : int { COND_TYPE_C = 0, COND_TYPE_CWH = 1, COND_TYPE_REFINEMENT = 2, COND_
 __global__ void make_cond_kernel(const long long* __restrict__ label /*[B][E]*/, const float* __restrict__ bbox /*[B][E][4]*/,
                                  const unsigned char* __restrict__ elem_mask /*[B][E]*/, const float* __restrict__ centers /*[4][n_bins] or null*/,
                                  long long* __restrict__ seq /*[B][E*5]*/, unsigned char* __restrict__ mask /*[B][E*5]*/,
-                                 long long* __restrict__ seq_orig /*[B][E*5] or null*/, int n_layouts, int n_elem, int n_cat, int n_bins,
+                                 long long* __restrict__ seq_orig /*[B][E*5] or null*/, int n_layouts, int n_elem, const TokenLayout tl,
                                  int pad_id, int mask_id, int cond_type, float d32 /*float(1/n_bins)*/, float hi32 /*float(1 - 1/n_bins)*/) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_layouts * n_elem) return;
+  const int n_bins = tl.n_bins;
   const bool valid = elem_mask[i] != 0;
-  long long tok[5];
-  tok[0] = label[i];
   const float4 bb = reinterpret_cast<const float4*>(bbox)[i];
   const float v[4] = {bb.x, bb.y, bb.z, bb.w};
+  int bins[4];
 #pragma unroll
   for (int a = 0; a < 4; ++a) {
     int bin;
@@ -768,19 +782,26 @@ __global__ void make_cond_kernel(const long long* __restrict__ label /*[B][E]*/,
         if (dist < best) { best = dist; bin = k; }
       }
     }
-    tok[1 + a] = static_cast<long long>(bin) + static_cast<long long>(a) * n_bins + n_cat;
+    bins[a] = bin;
   }
+  // slot k: its variable's bin plus the first id of that variable (the offsets and the reorder of bbox_tokenizer.py:105-113)
+  long long tok[5];
+  tok[0] = label[i];
 #pragma unroll
-  for (int a = 0; a < 5; ++a) {
-    const long long t = valid ? tok[a] : pad_id;                          // _fix_padded_sequences
+  for (int k = 1; k < 5; ++k) tok[k] = static_cast<long long>(bins[tl.var[k] - 1]) + tl.start[k];
+#pragma unroll
+  for (int k = 0; k < 5; ++k) {
+    const long long t = valid ? tok[k] : pad_id;                          // _fix_padded_sequences
+    // get_cond keeps slots by variable name (task.py:103-105): c for c / refinement, c, w, h for cwh
+    const int var = tl.var[k];
     bool keep;
-    if (cond_type == COND_TYPE_C) keep = a == 0;
-    else if (cond_type == COND_TYPE_CWH) keep = a == 0 || a == 3 || a == 4;
-    else if (cond_type == COND_TYPE_REFINEMENT) keep = a == 0;
+    if (cond_type == COND_TYPE_C) keep = var == 0;
+    else if (cond_type == COND_TYPE_CWH) keep = var == 0 || var == 3 || var == 4;
+    else if (cond_type == COND_TYPE_REFINEMENT) keep = var == 0;
     else keep = true;
     long long s = keep ? t : mask_id;
     if (!valid) s = pad_id;
-    const size_t o = static_cast<size_t>(i) * 5 + a;
+    const size_t o = static_cast<size_t>(i) * 5 + k;
     seq[o] = s;
     mask[o] = cond_type == COND_TYPE_GT ? (valid ? 1 : 0) : ((valid && keep) || !valid ? 1 : 0);
     if (seq_orig != nullptr) seq_orig[o] = t;

@@ -22,6 +22,7 @@ struct RelationParams {
   const long long* cond_seq;    // [n_layouts][S]: an element is valid when its category slot is not PAD (logit_adjustment.py:44)
   const int* adj;               // [n_layouts][1 + n_elem][1 + n_elem] edge_attr of the edge i -> j, 0 = no edge
   const float* centers;         // [4][n_bins] bin centres (x, y, w, h) or nullptr = linear quantisation
+  int bin_start[4];             // first id of the bins slot 1+a reads (TokenLayout::start[1+a]); slot 1+a holds variable a (c-x-y-w-h)
   float step;                   // relation_lambda / (batch_total * 14): SGD lr times the mean() over (layout, cost function)
   int n_update;
 };
@@ -88,7 +89,7 @@ __global__ void __launch_bounds__(kRelThreads) relation_update_kernel(const Rela
     for (int a = 0; a < 4; ++a) {
       v[k][a] = -INFINITY;
       if (e < N && s_valid[e] && lane_on)
-        v[k][a] = p.lp[(static_cast<size_t>(b) * p.S + (e - 1) * p.n_attr + 1 + a) * p.C + p.n_cat + a * p.n_bins + lane];
+        v[k][a] = p.lp[(static_cast<size_t>(b) * p.S + (e - 1) * p.n_attr + 1 + a) * p.C + p.bin_start[a] + lane];
     }
   }
 
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(kRelThreads) relation_update_kernel(const Rela
     if (e < N && s_valid[e] && lane_on) {
 #pragma unroll
       for (int a = 0; a < 4; ++a)
-        p.lp[(static_cast<size_t>(b) * p.S + (e - 1) * p.n_attr + 1 + a) * p.C + p.n_cat + a * p.n_bins + lane] = v[k][a];
+        p.lp[(static_cast<size_t>(b) * p.S + (e - 1) * p.n_attr + 1 + a) * p.C + p.bin_start[a] + lane] = v[k][a];
     }
   }
 }

@@ -172,13 +172,22 @@ class FusedMaskAndReplaceDiffusion:
             cond["refine_table"] = refinement_table(self.vocab, self.bbox_centers, _cfg_get(sampling_cfg, "refine_mode", "uniform"),
                                                     _cfg_get(sampling_cfg, "refine_offset_ratio", 0.1),
                                                     _cfg_get(sampling_cfg, "refine_lambda", 3.0))
-        if self.relation_on_device and cond.get("type") == "relation" and "batch_w_canvas" in cond and "rel_adj" not in cond \
-                and self.vocab.n_elem + 1 <= RELATION_MAX_NODES \
-                and _cfg_get(sampling_cfg, "relation_mode", "average") == "average" and float(_cfg_get(sampling_cfg, "relation_lambda", 0.0)) > 0.0:
+        device_relation = self.relation_on_device and cond.get("type") == "relation" and "batch_w_canvas" in cond \
+            and "rel_adj" not in cond and self.vocab.n_elem + 1 <= RELATION_MAX_NODES \
+            and _cfg_get(sampling_cfg, "relation_mode", "average") == "average" and float(_cfg_get(sampling_cfg, "relation_lambda", 0.0)) > 0.0
+        if device_relation and not self.vocab.relation_on_device:
+            # the device update does not read this vocabulary: the reference's own `update` must run through logit_adjust_fn, and
+            # without one sampling would silently skip the update
+            if self.logit_adjust_fn is None:
+                raise NotImplementedError(
+                    f"cond=relation with var_order {self.vocab.var_order} and {self.vocab.n_bins} bins: the device update needs "
+                    "c-x-y-w-h and <= 32 bins; patch a live reference model (patch_reference_model) to run the reference's own update")
+            device_relation = False
+        if device_relation:
             # logit_adjustment.update (:88-126) on the device: dense edge table + bin centres + SGD hyper-parameters.
             # relation_mode "gumbel" draws torch noise inside the update and stays on the reference's autograd path (logit_adjust_fn),
-            # and so does a layout of more elements than the update kernel holds (the canvas + 31): without rel_adj the step
-            # takes the log-prob hook path.
+            # and so do a layout of more elements than the update kernel holds (the canvas + 31) and a vocabulary it does not
+            # read (Vocab.relation_on_device): without rel_adj the step takes the log-prob hook path.
             cond["rel_adj"] = relation_edge_table(cond["batch_w_canvas"], cond["seq"].size(0), self.vocab.n_elem + 1)
             cond["rel_centers"] = torch.stack([torch.as_tensor(c, dtype=torch.float32).view(-1) for c in self.bbox_centers])
             cond["rel_lambda"] = float(_cfg_get(sampling_cfg, "relation_lambda", 3e6))
@@ -300,10 +309,9 @@ class FusedMaskAndReplaceDiffusion:
         return index_to_log_onehot(out, self.num_classes)
 
     # ---- training-side API (SURVEY 8b: "signatures that must keep working"; forward only, no autograd) -----------------
-    VAR_NAMES = ("c", "x", "y", "w", "h")
-
     def _key_index(self, key: str) -> int:
-        return self.VAR_NAMES.index(key) if self.engine.q_type == "constrained" else 0
+        """the token slot of variable `key` (tokenizer.var_names.index, constrained.py:162)"""
+        return self.vocab.var_order.split("-").index(key) if self.engine.q_type == "constrained" else 0
 
     def predict_start(self, log_x_t: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
         """base.py:127-146: log_x_t (B,C,S) log one-hot, t (B,) -> log p(x0|xt) (B,C,S)"""
@@ -476,21 +484,26 @@ class LayoutDMB200:
     @classmethod
     def from_state_dict(cls, sd, dataset: str = "rico25", num_timesteps: int = 100, q_type: str = "constrained",
                         operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None, noise: str = "contract",
-                        max_seq_length: Optional[int] = None) -> "LayoutDMB200":
+                        max_seq_length: Optional[int] = None, num_bin_bboxes: int = 32, shared_bbox_vocab: str = "x-y-w-h",
+                        var_order: str = "c-x-y-w-h") -> "LayoutDMB200":
         """noise: "contract" (the project's Philox contract) or "torch" (torch's CUDA generator, FusedMaskAndReplaceDiffusion).
         The layout length comes from the tokenizer if given, else from the state_dict's positional table (`layout_length`);
-        an explicit max_seq_length must agree with the table."""
-        vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else cls.vocab_for(sd, dataset, max_seq_length)
+        an explicit max_seq_length must agree with the table.  num_bin_bboxes / shared_bbox_vocab / var_order are the
+        tokenizer settings (DataConfig, hydra_configs.py:64-83); a given tokenizer's own settings win.  A state_dict whose
+        cat_emb does not have the C rows these settings describe is a ValueError."""
+        vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else \
+            cls.vocab_for(sd, dataset, max_seq_length, num_bin_bboxes, shared_bbox_vocab, var_order)
         eng = Engine.from_state_dict(sd, vocab, num_timesteps=num_timesteps, q_type=q_type, operand_dtype=operand_dtype, device=device)
         return cls(eng, tokenizer, bbox_centers, noise=noise)
 
     @staticmethod
-    def vocab_for(sd, dataset: str = "rico25", max_seq_length: Optional[int] = None) -> Vocab:
-        """the dataset's vocabulary at the layout length the state_dict was trained for"""
+    def vocab_for(sd, dataset: str = "rico25", max_seq_length: Optional[int] = None, num_bin_bboxes: int = 32,
+                  shared_bbox_vocab: str = "x-y-w-h", var_order: str = "c-x-y-w-h") -> Vocab:
+        """the dataset's vocabulary at the layout length the state_dict was trained for, with these tokenizer settings"""
         n = layout_length(sd)
         if max_seq_length is not None and int(max_seq_length) != n:
             raise ValueError(f"max_seq_length={max_seq_length}, but the state_dict's positional table is for {n} elements")
-        return Vocab.for_dataset(dataset, n)
+        return Vocab.for_dataset(dataset, n, num_bin_bboxes, shared_bbox_vocab, var_order)
 
     def eval(self):
         return self

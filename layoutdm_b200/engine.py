@@ -73,7 +73,7 @@ class Engine:
         self.n_layers, self.d_model, self.d_ff = L, d_model, d_ff
         desc = _lib.LdmModelDesc(vocab.n_cat, vocab.n_bins, vocab.n_elem, vocab.n_attr, d_model, n_heads, d_ff, L, num_timesteps,
                                  {"constrained": 0, "vanilla": 1}[q_type], _lib.OPERAND_DTYPES[operand_dtype], self.device_index,
-                                 att_1, att_T, ctt_1, ctt_T)
+                                 att_1, att_T, ctt_1, ctt_T, _lib.BBOX_VOCABS[vocab.shared_bbox_vocab], _lib.VAR_ORDERS[vocab.var_order])
         w = _lib.LdmWeights()
         keep = []
         for name in _lib._W_FIELDS:
@@ -106,6 +106,10 @@ class Engine:
         while f"{p}backbone.layers.{L}.linear1.weight" in sd:
             L += 1
         st = lambda k: torch.stack([g(f"backbone.layers.{l}.{k}") for l in range(L)]).contiguous()
+        if sd[p + "cat_emb.weight"].shape[0] != vocab.C:
+            raise ValueError(f"the state_dict's cat_emb has {sd[p + 'cat_emb.weight'].shape[0]} rows, the vocabulary has C = {vocab.C} "
+                             f"({vocab.n_cat} categories, {vocab.n_bins} bins, shared_bbox_vocab {vocab.shared_bbox_vocab}): a model of "
+                             "other tokenizer settings")
         if p + "pos_emb.elem_emb" in sd and sd[p + "pos_emb.elem_emb"].shape[0] != vocab.n_elem:
             raise ValueError(f"the state_dict's positional table is for {sd[p + 'pos_emb.elem_emb'].shape[0]} elements, the vocabulary "
                              f"has {vocab.n_elem}: a model of another max_seq_length")

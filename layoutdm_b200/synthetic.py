@@ -7,7 +7,7 @@ from typing import Dict, Optional
 
 import torch
 
-from .vocab import Vocab, linear_centers, refinement_table
+from .vocab import BBOX_VARS, Vocab, linear_centers, refinement_table
 
 PREFIX = "model.module.transformer."
 
@@ -58,13 +58,16 @@ def synthetic_cond(vocab: Vocab, B: int, cond_type: str = "c", seed: int = 0, re
     q = torch.zeros_like(bbox)
     q[..., :2] = torch.clamp(bbox[..., :2], 0.0, 1.0 - d)
     q[..., 2:] = torch.clamp(bbox[..., 2:], d, 1.0) - d
-    idx = (nb * q).round().long() + torch.arange(4) * nb + vocab.n_cat  # bbox_tokenizer.py:88-108 + layout_tokenizer.py:223
+    bins = (nb * q).round().long()                                      # bbox_tokenizer.py:88-91, x y w h
+    slots = vocab.slots()
+    # each slot: its variable's bin plus the first id of that variable (bbox_tokenizer.py:105-113 + layout_tokenizer.py:223)
+    idx = torch.stack([bins[..., BBOX_VARS.index(name)] + sl.start for name, sl in slots[1:]], dim=-1)
     full = torch.cat([label[..., None], idx], dim=-1)                   # (B,E,5)
     full[~valid] = vocab.pad_id
     seq_full = full.view(B, E * A)
     elem_valid = valid[..., None].expand(B, E, A).reshape(B, E * A)
-    attr = torch.arange(E * A)[None] % A
-    keep = {"c": attr == 0, "cwh": (attr == 0) | (attr == 3) | (attr == 4), "refinement": attr == 0}[cond_type]
+    kept = {"c": "c", "cwh": "cwh", "refinement": "c"}[cond_type]     # get_cond keeps slots by variable name (task.py:103-105)
+    keep = torch.tensor([slots[s % A][0] in kept for s in range(E * A)])[None]
     mask = (elem_valid & keep) | ~elem_valid
     seq = torch.where(mask, seq_full, torch.full_like(seq_full, vocab.mask_id))
     seq = torch.where(elem_valid, seq, torch.full_like(seq, vocab.pad_id))

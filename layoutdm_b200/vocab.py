@@ -1,6 +1,7 @@
 """Host-side neighbours of the hot path: vocabulary layout, timestep plan, refinement table, token decode.
 Mirrors (file:line under src/trainer/trainer/):
-  Vocab              helpers/layout_tokenizer.py:79-82,296-313 (var_order c-x-y-w-h, shared_bbox_vocab x-y-w-h, pad+mask)
+  Vocab              helpers/layout_tokenizer.py:79-82,296-313 + helpers/bbox_tokenizer.py:17-20,105-113 (either var_order,
+                     either shared_bbox_vocab, special tokens pad+mask)
   timestep_plan      models/categorical_diffusion/base.py:310-315,348-358 (+ :218-240 posterior timestep)
   refinement_table   helpers/task.py:154-224
   decode_ids         helpers/layout_tokenizer.py:255-266 + helpers/bbox_tokenizer.py:117-174
@@ -16,28 +17,62 @@ import torch
 DATASET_NUM_CATEGORIES = {"rico25": 25, "publaynet": 5}   # datasets/rico.py:42-68, datasets/publaynet.py:13-19
 
 
+BBOX_VOCABS = ("x-y-w-h", "xywh")          # helpers/layout_tokenizer.py:16-20 CHOICES
+VAR_ORDERS = ("c-x-y-w-h", "c-w-h-x-y")
+BBOX_VARS = ("x", "y", "w", "h")              # BboxTokenizer.var_names: the order of bbox values and bin centres
+
+
 @dataclass(frozen=True)
 class Vocab:
     n_cat: int = 25
     n_bins: int = 32
     n_elem: int = 25
     n_attr: int = 5
+    shared_bbox_vocab: str = "x-y-w-h"        # "xywh": x, y, w and h share one range of n_bins ids
+    var_order: str = "c-x-y-w-h"              # the variables of an element's token slots
+
+    def __post_init__(self):
+        if self.shared_bbox_vocab not in BBOX_VOCABS:
+            raise ValueError(f"shared_bbox_vocab must be one of {BBOX_VOCABS}, got {self.shared_bbox_vocab!r}")
+        if self.var_order not in VAR_ORDERS:
+            raise ValueError(f"var_order must be one of {VAR_ORDERS}, got {self.var_order!r}")
 
     @classmethod
-    def for_dataset(cls, name: str, max_seq_length: int = 25) -> "Vocab":
-        """the dataset's vocabulary for layouts of up to `max_seq_length` elements (config/dataset/*.yaml: dataset.max_seq_length)"""
-        return cls(n_cat=DATASET_NUM_CATEGORIES[name], n_elem=int(max_seq_length))
+    def for_dataset(cls, name: str, max_seq_length: int = 25, num_bin_bboxes: int = 32, shared_bbox_vocab: str = "x-y-w-h",
+                    var_order: str = "c-x-y-w-h") -> "Vocab":
+        """the dataset's vocabulary for layouts of up to `max_seq_length` elements (config/dataset/*.yaml: dataset.max_seq_length)
+        and the tokenizer settings of DataConfig (hydra_configs.py:64-83)"""
+        return cls(n_cat=DATASET_NUM_CATEGORIES[name], n_bins=int(num_bin_bboxes), n_elem=int(max_seq_length),
+                   shared_bbox_vocab=shared_bbox_vocab, var_order=var_order)
 
     @classmethod
     def from_tokenizer(cls, tok) -> "Vocab":
-        """from a reference LayoutSequenceTokenizer"""
-        assert tok.var_order == "c-x-y-w-h" and list(tok.special_tokens) == ["pad", "mask"]
-        assert tok.bbox_tokenizer.shared_bbox_vocab == "x-y-w-h"
-        return cls(n_cat=tok.N_category, n_bins=tok.N_bbox_per_var, n_elem=tok.max_seq_length, n_attr=tok.N_var_per_element)
+        """from a reference LayoutSequenceTokenizer with special tokens (pad, mask)"""
+        if list(tok.special_tokens) != ["pad", "mask"]:
+            raise NotImplementedError(f"special tokens {list(tok.special_tokens)}: only ['pad', 'mask'] (the diffusion models') are supported")
+        return cls(n_cat=tok.N_category, n_bins=tok.N_bbox_per_var, n_elem=tok.max_seq_length, n_attr=tok.N_var_per_element,
+                   shared_bbox_vocab=tok.bbox_tokenizer.shared_bbox_vocab, var_order=tok.var_order)
+
+    def var_slice(self, name: str) -> slice:
+        """the full-vocabulary ids of variable `name` (LayoutSequenceTokenizer.get_slice, layout_tokenizer.py:296-313)"""
+        if name == "c":
+            return slice(0, self.n_cat)
+        start = self.n_cat + (0 if self.shared_bbox_vocab == "xywh" else BBOX_VARS.index(name) * self.n_bins)
+        return slice(start, start + self.n_bins)
+
+    def slots(self) -> List[Tuple[str, slice]]:
+        """(variable, full-vocabulary ids) of each token slot of an element, in var_order: the one description of the token
+        layout every host consumer reads (the device builds the same table in ldm_create)"""
+        return [(name, self.var_slice(name)) for name in self.var_order.split("-")]
+
+    @property
+    def n_bbox_ids(self) -> int:
+        """ids of the bbox vocabulary (BboxTokenizer.bbox_vocab_len): n_bins shared, 4 n_bins per variable"""
+        return self.n_bins * (1 if self.shared_bbox_vocab == "xywh" else 4)
 
     @property
     def C(self) -> int:
-        return self.n_cat + 4 * self.n_bins + 2
+        return self.n_cat + self.n_bbox_ids + 2
 
     @property
     def S(self) -> int:
@@ -45,18 +80,22 @@ class Vocab:
 
     @property
     def pad_id(self) -> int:
-        return self.n_cat + 4 * self.n_bins
+        return self.n_cat + self.n_bbox_ids
 
     @property
     def mask_id(self) -> int:
         return self.pad_id + 1
 
+    @property
+    def relation_on_device(self) -> bool:
+        """the device relation update reads slot 1+a as variable a with one lane per bin: c-x-y-w-h and at most 32 bins"""
+        return self.var_order == "c-x-y-w-h" and self.n_bins <= 32
+
 
 def group_full_ids(vocab: "Vocab", g: int) -> List[int]:
-    """full-vocabulary ids of attribute g's partial vocabulary [its classes..., PAD, MASK] (Converter, layout_tokenizer.py:429-467)"""
-    lo = 0 if g == 0 else vocab.n_cat + (g - 1) * vocab.n_bins
-    n = vocab.n_cat if g == 0 else vocab.n_bins
-    return list(range(lo, lo + n)) + [vocab.pad_id, vocab.mask_id]
+    """full-vocabulary ids of slot g's partial vocabulary [its classes..., PAD, MASK] (Converter, layout_tokenizer.py:429-467)"""
+    sl = vocab.slots()[g][1]
+    return list(range(sl.start, sl.stop)) + [vocab.pad_id, vocab.mask_id]
 
 
 def timestep_plan(T: int, T_eval: int, time_difference: float = 0.0) -> List[Tuple[int, int]]:
@@ -85,15 +124,17 @@ def linear_centers(n_bins: int = 32) -> List[np.ndarray]:
 
 def refinement_table(vocab: Vocab, centers: Sequence[np.ndarray], mode: str = "uniform", offset_ratio: float = 0.1,
                      weight: float = 3.0) -> torch.Tensor:
-    """(C, C) fp32 table, weak_logits[b, c, s] == table[seq_orig[b, s], c]; already multiplied by +-refine_lambda."""
+    """(C, C) fp32 table, weak_logits[b, c, s] == table[seq_orig[b, s], c]; already multiplied by +-refine_lambda.
+    centers: per variable x, y, w, h.  Each variable writes the block of its own ids; with a shared vocabulary the four write
+    the same block and the last one (h) wins, as in the reference."""
     assert mode in ("uniform", "gaussian", "negative")
     w = -weight if mode == "negative" else weight
     tbl = torch.zeros(vocab.C, vocab.C)
     tbl.fill_diagonal_(1.0)
-    for i in range(4):
+    for i, name in enumerate(BBOX_VARS):
         cc = torch.from_numpy(np.asarray(centers[i], dtype=np.float64)).view(-1)
         ii, jj = torch.meshgrid(cc, cc, indexing="ij")
-        sl = slice(vocab.n_cat + i * vocab.n_bins, vocab.n_cat + (i + 1) * vocab.n_bins)
+        sl = vocab.var_slice(name)
         if mode == "uniform":
             tbl[sl, sl] = (torch.abs(ii - jj) < offset_ratio).float()
         elif mode == "negative":
@@ -107,11 +148,13 @@ def decode_ids(ids: torch.Tensor, vocab: Vocab, centers: Optional[Sequence[np.nd
     """ids (B, S) int64 (CPU) -> {"bbox": (B, n_elem, 4) f32, "label": (B, n_elem) i64, "mask": (B, n_elem) bool}.
     centers=None: linear quantisation; else per-variable cluster centres (kmeans / percentile)."""
     x = ids.view(ids.shape[0], vocab.n_elem, vocab.n_attr)
-    label, bbox = x[..., 0].clone(), x[..., 1:].clone() - vocab.n_cat
+    label = x[..., 0].clone()
     label_valid = (0 <= label) & (label < vocab.n_cat)
-    bbox_valid = ((0 <= bbox) & (bbox < 4 * vocab.n_bins)).all(dim=-1)
+    bbox_valid = ((0 <= x[..., 1:] - vocab.n_cat) & (x[..., 1:] - vocab.n_cat < vocab.n_bbox_ids)).all(dim=-1)
     invalid = ~(label_valid & bbox_valid)
-    arr = torch.clamp(bbox - torch.arange(4) * vocab.n_bins, 0, vocab.n_bins - 1)
+    # each slot's bin within its variable's ids, back in x, y, w, h order (BboxTokenizer.decode, bbox_tokenizer.py:117-141)
+    bins = {name: x[..., k] - sl.start for k, (name, sl) in enumerate(vocab.slots()) if name != "c"}
+    arr = torch.clamp(torch.stack([bins[name] for name in BBOX_VARS], dim=-1), 0, vocab.n_bins - 1)
     if centers is None:
         d = 1 / vocab.n_bins
         out = torch.zeros(arr.shape, dtype=torch.float32)
