@@ -54,6 +54,14 @@ typedef struct {
                              other values: LDM_ERR_INVALID */
   int32_t device;         /* CUDA device ordinal */
   double att_1, att_T, ctt_1, ctt_T;  /* alpha_schedule() endpoints, util.py:47-49 */
+  /* The denoiser block (transformer_utils.py:103-210, backbone.encoder_layer.timestep_type / activation).  norm1 is
+   * norm(x) * (1 + scale_t) + shift_t with (scale_t, shift_t) from the AdaLN table of LdmWeights' norm1_* arrays; every
+   * timestep_type is a filling of those arrays (None: norm1_emb = 0, norm1_w = 0, norm1_b = [w - 1, b]; *_abs: norm1_emb[l][t]
+   * = the sinusoidal embedding of t) plus the norm below.  Other values: LDM_ERR_INVALID.  Zero-filled: the default block
+   * (adalayernorm + relu).  Since 0.4; they sit before the tokenizer fields, which stay the struct's last two. */
+  int32_t norm1_kind;     /* 0 = LayerNorm over a token's d channels (adalayernorm*, None); 1 = InstanceNorm1d (adainnorm*): per
+                             layout and channel, mean and biased variance over the layout's S tokens, eps 1e-5 */
+  int32_t activation;     /* feed-forward activation: 0 = relu, 1 = gelu (exact, erf), 2 = gelu2 (x * sigmoid(1.702 x)) */
   int32_t bbox_vocab;     /* shared_bbox_vocab (bbox_tokenizer.py:17-20): 0 = "x-y-w-h" (x, y, w, h take n_bins ids each, in
                              that order), 1 = "xywh" (the four share one range of n_bins ids); other values: LDM_ERR_INVALID */
   int32_t var_order;      /* var_order of an element's token slots: 0 = "c-x-y-w-h", 1 = "c-w-h-x-y" (needs n_attr = 5);

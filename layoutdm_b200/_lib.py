@@ -19,13 +19,17 @@ OPERAND_DTYPES = {"fp16": 0, "bf16": 1, "bf16x3": 2}
 # LdmModelDesc.bbox_vocab / var_order: the tokenizer's shared_bbox_vocab and var_order (helpers/layout_tokenizer.py:16-20)
 BBOX_VOCABS = {"x-y-w-h": 0, "xywh": 1}
 VAR_ORDERS = {"c-x-y-w-h": 0, "c-w-h-x-y": 1}
+# LdmModelDesc.norm1_kind / activation: the denoiser block's timestep_type and activation (transformer_utils.py:17-31,103-170).
+# The keys are every timestep_type the reference can sample with; it cannot with the *_mlp types (their MLP gets long timesteps)
+NORM1_KINDS = {None: 0, "adalayernorm": 0, "adalayernorm_abs": 0, "adainnorm": 1, "adainnorm_abs": 1}
+ACTIVATIONS = {"relu": 0, "gelu": 1, "gelu2": 2}
 
 
 class LdmModelDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_cat", "n_bins", "n_elem", "n_attr", "d_model", "n_heads", "d_ff", "n_layers",
                                          "num_timesteps", "q_type", "operand_dtype", "device")] + \
                [(n, C.c_double) for n in ("att_1", "att_T", "ctt_1", "ctt_T")] + \
-               [(n, C.c_int32) for n in ("bbox_vocab", "var_order")]
+               [(n, C.c_int32) for n in ("norm1_kind", "activation", "bbox_vocab", "var_order")]
 
 
 _W_FIELDS = ("cat_emb", "pos_table", "in_proj_w", "in_proj_b", "out_proj_w", "out_proj_b", "linear1_w", "linear1_b",

@@ -123,7 +123,9 @@ LDM_DEVINL void embed_token_row(const long long id, const int s, const size_t ro
   }
 }
 
-template <int MODE>
+// NORM = false (instance-norm blocks): the token rows get the raw h = cat_emb[id] + pos[s] in x32 only, which
+// instance_norm_kernel then normalises over the layout's tokens; pad rows as with NORM
+template <int MODE, bool NORM = true>
 __global__ void __launch_bounds__(256)
 embed_adaln_kernel(const long long* __restrict__ ids /*[B][S]*/, const float* __restrict__ cat_emb /*[C][d]*/,
                    const float* __restrict__ pos /*[S][d]*/, const float* __restrict__ adaln_tab /*[T][2d] of layer 0*/, int t_model,
@@ -149,8 +151,104 @@ embed_adaln_kernel(const long long* __restrict__ ids /*[B][S]*/, const float* __
     return;
   }
   const long long id = ids[static_cast<size_t>(b) * S + s];
-  const float* adaln = adaln_tab + static_cast<size_t>(t_layout != nullptr ? __ldg(t_layout + b) : t_model) * 2 * d;
-  embed_token_row<MODE>(id, s, row, cat_emb, pos, adaln, x32, x16_, d, lane, x16_lo);
+  if constexpr (NORM) {
+    const float* adaln = adaln_tab + static_cast<size_t>(t_layout != nullptr ? __ldg(t_layout + b) : t_model) * 2 * d;
+    embed_token_row<MODE>(id, s, row, cat_emb, pos, adaln, x32, x16_, d, lane, x16_lo);
+  } else {
+    const float4* e = reinterpret_cast<const float4*>(cat_emb + static_cast<size_t>(id) * d);
+    const float4* p = reinterpret_cast<const float4*>(pos + static_cast<size_t>(s) * d);
+    float4* o32 = reinterpret_cast<float4*>(x32 + row * d);
+    for (int i = lane; i < d / 4; i += 32) {
+      const float4 a = __ldg(e + i), c = __ldg(p + i);
+      o32[i] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
+    }
+  }
+}
+
+// norm1 of the instance-norm blocks (AdaInsNorm, transformer_utils.py:86-100): x = InstanceNorm1d(h) * (1 + scale_t) + shift_t,
+// the statistics per layout and channel over the layout's S token rows (mean and biased variance, eps 1e-5, no affine), in place
+// on the fp32 rows x32 (the raw embedding or FF2's pre-norm sum) -> x32 and the 16-bit operand rows (split mode: + the lo plane).
+// grid (d / (4 kInCols4), n_layouts); a block holds kInCols4 float4 columns of one layout in 8 R row slices, thread (slice, col)
+// rows slice, slice + 8 R, .. < S in registers (at most kInRows): one read of the rows, and the variance is taken about the mean.
+// The sums run over h - h[row 0] (offset invariance, as in the LayerNorm epilogues).  Pad rows (s >= S) are neither read nor
+// written: after the fused embedding of the draw kernels they may hold stale values, and the GEMMs keep them finite.
+// The row stride is the compile-time kInD, so a thread's rows are immediate offsets of one address.
+constexpr int kInD = 464, kInCols4 = 29, kInRows = 16;
+static_assert(kInD % (4 * kInCols4) == 0, "whole column blocks");
+template <int MODE, int R>
+__global__ void __launch_bounds__(kInCols4 * 8 * R)
+instance_norm_kernel(float* __restrict__ x32 /*[B*128R][kInD]*/, void* __restrict__ x16_, void* __restrict__ x16_lo,
+                     const float* __restrict__ adaln_tab /*[T][2 kInD] of the layer*/, int t_model,
+                     const int* __restrict__ t_layout /*[n_layouts] per-layout timesteps (training-side calls) or nullptr*/, int S) {
+  using O = OpT<MODE>;
+  constexpr int d = kInD;
+  constexpr int kSlices = 8 * R;
+  static_assert(kSlices * kInRows >= 128 * R, "a thread's registers cover its slice of the layout's rows");
+  __shared__ float4 red[kSlices][kInCols4];
+  const int col = threadIdx.x % kInCols4, slice = threadIdx.x / kInCols4, b = blockIdx.y;
+  const int c = (blockIdx.x * kInCols4 + col) * 4;
+  const size_t row0 = static_cast<size_t>(b) * 128 * R;
+  pdl_sync();                                  // x32 comes from the previous kernel
+  const float4 piv = *reinterpret_cast<const float4*>(x32 + row0 * d + c);
+  float4 v[kInRows];
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int k = 0; k < kInRows; ++k) {
+    const int s = slice + k * kSlices;
+    if (s < S) {
+      v[k] = *reinterpret_cast<const float4*>(x32 + (row0 + s) * d + c);
+      acc.x += v[k].x - piv.x; acc.y += v[k].y - piv.y; acc.z += v[k].z - piv.z; acc.w += v[k].w - piv.w;
+    }
+  }
+  // the slices' partial sums, added in slice order by every thread of the column
+  const auto column_total = [&](float4 part) {
+    red[slice][col] = part;
+    __syncthreads();
+    float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < kSlices; ++i) { const float4 r = red[i][col]; t.x += r.x; t.y += r.y; t.z += r.z; t.w += r.w; }
+    __syncthreads();
+    return t;
+  };
+  const float inv_s = 1.0f / static_cast<float>(S);
+  const float4 sum = column_total(acc);
+  const float4 mean = make_float4(piv.x + sum.x * inv_s, piv.y + sum.y * inv_s, piv.z + sum.z * inv_s, piv.w + sum.w * inv_s);
+  acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int k = 0; k < kInRows; ++k) {
+    if (slice + k * kSlices < S) {
+      const float a = v[k].x - mean.x, e = v[k].y - mean.y, f = v[k].z - mean.z, g = v[k].w - mean.w;
+      acc.x = fmaf(a, a, acc.x); acc.y = fmaf(e, e, acc.y); acc.z = fmaf(f, f, acc.z); acc.w = fmaf(g, g, acc.w);
+    }
+  }
+  const float4 q = column_total(acc);
+  const float4 rstd = make_float4(1.0f / sqrtf(q.x * inv_s + 1e-5f), 1.0f / sqrtf(q.y * inv_s + 1e-5f), 1.0f / sqrtf(q.z * inv_s + 1e-5f),
+                                  1.0f / sqrtf(q.w * inv_s + 1e-5f));
+  const float* tab = adaln_tab + static_cast<size_t>(t_layout != nullptr ? __ldg(t_layout + b) : t_model) * 2 * d;
+  const float4 g = __ldg(reinterpret_cast<const float4*>(tab + c)), sh = __ldg(reinterpret_cast<const float4*>(tab + d + c));
+  typename O::T* x16 = static_cast<typename O::T*>(x16_);
+#pragma unroll
+  for (int k = 0; k < kInRows; ++k) {
+    const int s = slice + k * kSlices;
+    if (s < S) {
+      const size_t off = (row0 + s) * d + c;
+      float4 r;
+      r.x = (v[k].x - mean.x) * rstd.x * (1.0f + g.x) + sh.x;
+      r.y = (v[k].y - mean.y) * rstd.y * (1.0f + g.y) + sh.y;
+      r.z = (v[k].z - mean.z) * rstd.z * (1.0f + g.z) + sh.z;
+      r.w = (v[k].w - mean.w) * rstd.w * (1.0f + g.w) + sh.w;
+      *reinterpret_cast<float4*>(x32 + off) = r;
+      if constexpr (kOpSplit<MODE>) {
+        uint2 hi, lo;
+        O::pack_pair(r.x, r.y, hi.x, lo.x);
+        O::pack_pair(r.z, r.w, hi.y, lo.y);
+        *reinterpret_cast<uint2*>(x16 + off) = hi;
+        *reinterpret_cast<uint2*>(static_cast<typename O::T*>(x16_lo) + off) = lo;
+      } else {
+        *reinterpret_cast<uint2*>(x16 + off) = make_uint2(O::pack(r.x, r.y), O::pack(r.z, r.w));
+      }
+    }
+  }
 }
 
 }  // namespace ldm

@@ -37,7 +37,9 @@ constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // persistent block: 12
 // K elements per ring k-block of gemm_tc_kernel: 64 with one plane, 32 per plane in the split mode (the stage keeps its bytes)
 constexpr int gemm_kb(bool split) { return split ? 32 : 64; }
 
-enum : int { EPI_QKV = 0, EPI_RELU = 1, EPI_F32 = 2, EPI_LN = 3 };
+// EPI_GELU / EPI_GELU2: FF1 with the block's other activations (transformer_utils.py:17-31): F.gelu (erf form) and
+// x * sigmoid(1.702 x)
+enum : int { EPI_QKV = 0, EPI_RELU = 1, EPI_F32 = 2, EPI_LN = 3, EPI_GELU = 4, EPI_GELU2 = 5 };
 
 struct GemmParams {
   int M, N, K;            // M multiple of the tile rows; N <= n_tiles * tile columns (columns past N are computed on zero weights, not stored)
@@ -196,6 +198,11 @@ LDM_DEVINL void bias_act(const float (&acc)[N], int j, const float* bias, int c,
   for (int e = 0; e < 4; ++e) {
     if constexpr (EPI == EPI_QKV) v[e] *= scale;
     if constexpr (EPI == EPI_RELU) v[e] = fmaxf(v[e], 0.0f);
+    if constexpr (EPI == EPI_GELU) v[e] = 0.5f * v[e] * (1.0f + erff(v[e] * 0.70710678118654752f));
+    // x / (1 + e^(-1.702 x)) with the approximate exp / divide: within a few fp32 ulps, below any 16-bit operand's rounding, at
+    // a fraction of the epilogue's issue slots (expf and a true division made gelu2's FF1 1.7x ReLU's).  x very negative:
+    // the denominator overflows and the result is 0, as x sigmoid(1.702 x) is to fp32 there
+    if constexpr (EPI == EPI_GELU2) v[e] = __fdividef(v[e], 1.0f + __expf(-1.702f * v[e]));
   }
 }
 
@@ -405,7 +412,7 @@ template <int EPI, int MODE>
 __global__ void __launch_bounds__(kRbThreads, 1)
 gemm_rowblock_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/, const __grid_constant__ OpMaps<MODE> map_b /*box 32 x 128 rows*/,
                      const __grid_constant__ CUtensorMap map_out /*box 64 x 128 rows*/, const GemmParams p) {
-  static_assert(EPI == EPI_QKV || EPI == EPI_RELU, "16-bit plain epilogues only");
+  static_assert(EPI == EPI_QKV || EPI == EPI_RELU || EPI == EPI_GELU || EPI == EPI_GELU2, "16-bit plain epilogues only");
   static_assert(!kOpSplit<MODE>, "the split mode runs gemm_tc_kernel");
   using SM = RbSmem;
   using R = SM::R;

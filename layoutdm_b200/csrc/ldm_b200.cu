@@ -43,6 +43,7 @@ constexpr int kAttN = 8 * kHeadPad;        // 512: attention output, heads padde
 constexpr int kMaxLayouts = 32767;  // layouts per call
 constexpr int kLogitLd = 160;       // padded logits row (C <= 160)
 constexpr int kDModel = 464;        // the kernels are laid out for the paper's backbone: d = 464 (LN tiles 224 + 240), ff = 4 d
+static_assert(kInD == kDModel, "instance_norm_kernel's row stride");
 // GEMM instantiations: <warpgroup tile width, row warpgroups, ring stages, epilogue, operand mode>
 // QKV / FF1: fp16 / bf16: gemm_rowblock_kernel (resident A rows, 128-column tiles); the split mode: 128 x 256 tiles of
 // gemm_tc_kernel, 4 ring stages
@@ -198,7 +199,7 @@ struct LdmHandle {
   int ln_clusters = 0;         // one-plane modes: the CTA pairs of gemm_ln_kernel that can be resident at once
   int gemm_split = 0;          // env LDM_GEMM_SPLIT=g (g >= 1): column ranges per row block of the row-block GEMMs; 0: automatic
   int fuse_embed = 1;          // env LDM_FUSE_EMBED=0: the loop launches the embedding kernel in every step instead of fusing it into the previous draw.
-                               // The split mode always launches it: the draw kernels write one 16-bit plane only
+                               // The split mode and instance-norm handles always launch it (ldm_create)
   cudaStream_t cap_stream = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
   uint64_t graph_key = 0;
@@ -393,9 +394,13 @@ int set_smem(LdmHandle* h) {
   if constexpr (kOpSplit<MODE>) {
     CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_QKV, MODE>, attr, kPlainSmem));
     CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_RELU, MODE>, attr, kPlainSmem));
+    CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_GELU, MODE>, attr, kPlainSmem));
+    CK(cudaFuncSetAttribute(kGemmPlainSplit<EPI_GELU2, MODE>, attr, kPlainSmem));
   } else {
     CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_QKV, MODE>, attr, RbSmem::kBytes));
     CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_RELU, MODE>, attr, RbSmem::kBytes));
+    CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_GELU, MODE>, attr, RbSmem::kBytes));
+    CK(cudaFuncSetAttribute(gemm_rowblock_kernel<EPI_GELU2, MODE>, attr, RbSmem::kBytes));
   }
   CK(cudaFuncSetAttribute(kGemmHead<MODE>, attr, kHeadSmem));
   if constexpr (kOpSplit<MODE>) CK(cudaFuncSetAttribute(kGemmLn<MODE>, attr, kLnSmem));
@@ -525,6 +530,15 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, res, st32, p);
     }
   };
+  // instance-norm blocks (norm1_kind 1): norm1 of layer l is its own pass over the fp32 rows x32 (instance_norm_kernel); layer 0's
+  // embedding writes them raw, and the FF2 before layer l > 0 writes its pre-norm sum there (DESIGN §4)
+  const bool inorm = h->desc.norm1_kind == 1;
+  const auto instance_norm = [&](int l) {
+    const float* tab = h->adaln + static_cast<size_t>(l) * T * 2 * d;
+    const dim3 g(kInD / (4 * kInCols4), n);
+    if (R == 1) return launch_step(h, instance_norm_kernel<MODE, 1>, g, kInCols4 * 8, 0, st, h->x32, h->x16.hi, h->x16.lo, tab, t_model, t_layout, h->S);
+    return launch_step(h, instance_norm_kernel<MODE, 2>, g, kInCols4 * 16, 0, st, h->x32, h->x16.hi, h->x16.lo, tab, t_model, t_layout, h->S);
+  };
   int done = 0;
   // alternating sweep direction: every kernel walks the row blocks opposite to its predecessor (GemmParams::rev); the embedding /
   // draw kernels run their blocks in ascending order, so the first GEMM starts from the end.  LDM_SWEEP=0: always ascending
@@ -535,11 +549,17 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
   if (!skip_embed) {     // skipped inside the loop: the previous step's draw kernel has already written this step's x32 / x16 rows
     const int warps = M, blocks = (warps * 32 + 255) / 256;    // one warp per row, pad rows included
     ProfScope ps(h, CAT_EMBED, st);
-    CK(launch_step(h, embed_adaln_kernel<MODE>, dim3(blocks), 256, 0, st, ids_in, (const float*)h->cat_emb, (const float*)h->pos,
-                   (const float*)h->adaln, t_model, t_layout, h->x32, h->x16.hi, n, R == 1 ? 7 : 8, h->S, d, h->x16.lo));
+    CK(launch_step(h, inorm ? embed_adaln_kernel<MODE, false> : embed_adaln_kernel<MODE>, dim3(blocks), 256, 0, st, ids_in,
+                   (const float*)h->cat_emb, (const float*)h->pos, (const float*)h->adaln, t_model, t_layout, h->x32, h->x16.hi, n,
+                   R == 1 ? 7 : 8, h->S, d, h->x16.lo));
   }
   if (!skip_embed) LDM_STAGE_DONE();
   for (int l = 0; l < L; ++l) {
+    if (inorm) {
+      ProfScope ps(h, CAT_EMBED, st);
+      CK(instance_norm(l));
+      LDM_STAGE_DONE();
+    }
     {  // QKV projection (+bias, q * 1/sqrt(head_dim))
       GemmParams p{M, kQkvN, d, 0, h->bqkv[l], h->qkv16.hi, kQkvN, 1.0f / sqrtf(static_cast<float>(d / h->desc.n_heads)), 8 * kHeadPad};
       p.rev = next_rev(); p.out_lo = h->qkv16.lo;
@@ -565,16 +585,23 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       CK(ln_gemm(h->att16.maps<MODE>(), h->wo[l].maps<MODE>(), h->m_x32, h->m_y32, p));
     }
     LDM_STAGE_DONE();
-    {  // FF1 + ReLU
+    {  // FF1 + activation (ReLU | GELU | GELU2)
       GemmParams p{M, ff, d, 0, h->b1[l], h->hid16.hi, ff, 1.0f, 0};   // 14 tiles of 128 columns + one of 64 (split mode: 7 of 256 + one of 64)
       p.rev = next_rev(); p.out_lo = h->hid16.lo;
       ProfScope ps(h, CAT_FF1, st);
-      CK(plain_gemm(std::integral_constant<int, EPI_RELU>{}, h->z16.maps<MODE>(), h->w1[l].maps<MODE>(), h->m_hid16_st, p));
+      const auto ff1 = [&](auto epi) { return plain_gemm(epi, h->z16.maps<MODE>(), h->w1[l].maps<MODE>(), h->m_hid16_st, p); };
+      if (h->desc.activation == 1) CK(ff1(std::integral_constant<int, EPI_GELU>{}));
+      else if (h->desc.activation == 2) CK(ff1(std::integral_constant<int, EPI_GELU2>{}));
+      else CK(ff1(std::integral_constant<int, EPI_RELU>{}));
     }
     LDM_STAGE_DONE();
     {  // FF2 + bias + residual ; next block's AdaLN(h, t) (fp32 residual + 16-bit operand) or the head LayerNorm   [fused epilogue]
       GemmParams p{M, d, ff, 1, h->b2[l], nullptr, d, 1.0f, 0, h->y32, nullptr, nullptr, nullptr, 0, nullptr};
-      if (l + 1 < L) {
+      if (l + 1 < L && inorm) {
+        // the pre-norm sum h = acc + bias + resid to x32 (y_out), for the next layer's instance norm; the LN output the kernel
+        // also writes (a plain LayerNorm into x16) is overwritten by that pass
+        p.y_out = h->x32; p.ln_scale = h->hlnw; p.ln_shift = h->hlnb; p.adaln = 0; p.out = h->x16.hi; p.out_lo = h->x16.lo;
+      } else if (l + 1 < L) {
         const float* tab = h->adaln + (static_cast<size_t>(l + 1) * T + t_model) * 2 * d;
         p.ln_scale = tab; p.ln_shift = tab + d; p.adaln = 1; p.out32 = h->x32; p.out = h->x16.hi; p.out_lo = h->x16.lo;
         if (t_layout) {   // per-layout rows
@@ -767,7 +794,7 @@ int step_impl(LdmHandle* h, int B, const long long* ids_in, int t_model, int t_p
 extern "C" {
 
 const char* ldm_last_error(void) { return g_err; }
-const char* ldm_version(void) { return "ldm_b200 0.3 (sm_90a, wgmma)"; }
+const char* ldm_version(void) { return "ldm_b200 0.4 (sm_90a, wgmma)"; }
 
 int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (!desc || !w || !out) return fail(LDM_ERR_INVALID, "null argument");
@@ -789,6 +816,11 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
                 "with %d attributes)", S, kAttMaxR * kBM, kAttMaxR, kBM, desc->n_attr > 0 ? kAttMaxR * kBM / desc->n_attr : 0, desc->n_attr);
   if (desc->q_type != 0 && desc->q_type != 1) return fail(LDM_ERR_INVALID, "q_type must be 0 (constrained) or 1 (vanilla)");
   if (desc->q_type == 0 && desc->n_attr != 5) return fail(LDM_ERR_UNSUPPORTED, "constrained q_type needs the c-x-y-w-h layout (5 attributes)");
+  if (desc->norm1_kind != 0 && desc->norm1_kind != 1)
+    return fail(LDM_ERR_INVALID, "norm1_kind must be 0 (layer norm) or 1 (instance norm), got %d", desc->norm1_kind);
+  if (desc->activation < 0 || desc->activation > 2)
+    return fail(LDM_ERR_INVALID, "activation must be 0 (relu), 1 (gelu) or 2 (gelu2), got %d (transformer_utils.py:28-31 raises RuntimeError)",
+                desc->activation);
   if (desc->operand_dtype < OP_F16 || desc->operand_dtype > OP_BF16X3)
     return fail(LDM_ERR_INVALID, "operand_dtype must be 0 (fp16), 1 (bf16) or 2 (bf16x3), got %d", desc->operand_dtype);
   CK(cudaSetDevice(desc->device));
@@ -807,7 +839,9 @@ int ldm_create(const LdmModelDesc* desc, const LdmWeights* w, LdmHandle** out) {
   if (const char* e = getenv("LDM_PDL")) h->pdl = atoi(e);
   if (const char* e = getenv("LDM_GRAPH")) h->use_graph = atoi(e);
   if (const char* e = getenv("LDM_FUSE_EMBED")) h->fuse_embed = atoi(e);
-  if (h->split) h->fuse_embed = 0;
+  // the split mode's draw kernels write one 16-bit plane only, and an instance norm needs the layout's whole rows: the
+  // embedding is its own launch in every step
+  if (h->split || desc->norm1_kind == 1) h->fuse_embed = 0;
   if (const char* e = getenv("LDM_SWEEP")) h->sweep = atoi(e);
   h->num_sms = prop.multiProcessorCount;
   h->max_threads_sm = prop.maxThreadsPerMultiProcessor;

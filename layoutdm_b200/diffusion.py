@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import copy
 import weakref
-from typing import Any, Dict, List, Optional, Union
+from typing import Any, Dict, List, Optional, Tuple, Union
 
 import torch
 import torch.nn.functional as F
@@ -103,8 +103,10 @@ class WeightFollower:
 
     def reload(self, fp=None):
         """repack the module's current parameters into the target unconditionally"""
-        sd = self.module.state_dict()
-        self.target.load_weights(Engine.pack_state_dict(sd, self.target.vocab, device=self.target.device))
+        sd, t = self.module.state_dict(), self.target
+        # the target's block settings (an Engine's); a target that has none runs the default block
+        self.target.load_weights(Engine.pack_state_dict(sd, t.vocab, getattr(t, "timestep_type", "adalayernorm"), getattr(t, "diffusion_step", None),
+                                                        num_timesteps=t.T, device=t.device))
         self._fp = self._fingerprint() if fp is None else fp
         self.dirty = False
         self.reloads += 1
@@ -485,15 +487,18 @@ class LayoutDMB200:
     def from_state_dict(cls, sd, dataset: str = "rico25", num_timesteps: int = 100, q_type: str = "constrained",
                         operand_dtype: str = "fp16", device=None, tokenizer=None, bbox_centers=None, noise: str = "contract",
                         max_seq_length: Optional[int] = None, num_bin_bboxes: int = 32, shared_bbox_vocab: str = "x-y-w-h",
-                        var_order: str = "c-x-y-w-h") -> "LayoutDMB200":
+                        var_order: str = "c-x-y-w-h", timestep_type: Optional[str] = "adalayernorm", activation: str = "relu",
+                        diffusion_step: Optional[int] = None) -> "LayoutDMB200":
         """noise: "contract" (the project's Philox contract) or "torch" (torch's CUDA generator, FusedMaskAndReplaceDiffusion).
         The layout length comes from the tokenizer if given, else from the state_dict's positional table (`layout_length`);
         an explicit max_seq_length must agree with the table.  num_bin_bboxes / shared_bbox_vocab / var_order are the
         tokenizer settings (DataConfig, hydra_configs.py:64-83); a given tokenizer's own settings win.  A state_dict whose
-        cat_emb does not have the C rows these settings describe is a ValueError."""
+        cat_emb does not have the C rows these settings describe is a ValueError.  timestep_type / activation / diffusion_step
+        are the denoiser block's settings (backbone.encoder_layer.*, transformer_utils.py:103-170; `Engine.pack_state_dict`)."""
         vocab = Vocab.from_tokenizer(tokenizer) if tokenizer is not None else \
             cls.vocab_for(sd, dataset, max_seq_length, num_bin_bboxes, shared_bbox_vocab, var_order)
-        eng = Engine.from_state_dict(sd, vocab, num_timesteps=num_timesteps, q_type=q_type, operand_dtype=operand_dtype, device=device)
+        eng = Engine.from_state_dict(sd, vocab, num_timesteps=num_timesteps, q_type=q_type, operand_dtype=operand_dtype, device=device,
+                                     timestep_type=timestep_type, activation=activation, diffusion_step=diffusion_step)
         return cls(eng, tokenizer, bbox_centers, noise=noise)
 
     @staticmethod
@@ -557,6 +562,21 @@ class LayoutDMB200:
         return sampling_cfg
 
 
+def block_settings_of(layers) -> Tuple[Optional[str], str, int]:
+    """(timestep_type, activation, diffusion_step) of a live reference TransformerEncoder's Blocks (transformer_utils.py:103-170),
+    which must all agree.  The activation is known by identity: F.relu, F.gelu or the reference module's _gelu2."""
+    import importlib
+    found = set()
+    for layer in layers:
+        acts = {F.relu: "relu", F.gelu: "gelu", importlib.import_module(type(layer).__module__)._gelu2: "gelu2"}
+        if layer.activation not in acts:
+            raise NotImplementedError(f"Block activation {layer.activation!r}: the sm_90a kernels have relu, gelu and gelu2")
+        found.add((layer.timestep_type, acts[layer.activation], int(layer.diffusion_step)))
+    if len(found) != 1:
+        raise ValueError(f"the Blocks disagree on (timestep_type, activation, diffusion_step): {sorted(found, key=str)}")
+    return found.pop()
+
+
 def patch_reference_model(model, operand_dtype: str = "fp16", device=None, noise: str = "contract"):
     """Drop-in for a live reference `trainer.models.layoutdm.LayoutDM`: after `patch_reference_model(model)`,
     `model.sample(...)` (layoutdm.py:77) and `model.model.sample(...)` / `_sample_single_step(...)` run on the sm_90a library.
@@ -568,8 +588,10 @@ def patch_reference_model(model, operand_dtype: str = "fp16", device=None, noise
     tok = model.tokenizer
     vocab = Vocab.from_tokenizer(tok)
     q_type = "vanilla" if type(core).__name__.startswith("Vanilla") else "constrained"
+    timestep_type, activation, diffusion_step = block_settings_of(core.transformer.backbone.layers)
     eng = Engine.from_state_dict(model.state_dict(), vocab, num_timesteps=core.num_timesteps, q_type=q_type,
-                                 operand_dtype=operand_dtype, device=device)
+                                 operand_dtype=operand_dtype, device=device, timestep_type=timestep_type, activation=activation,
+                                 diffusion_step=diffusion_step)
     fused = FusedMaskAndReplaceDiffusion(eng, tok, noise=noise)
     fused.follow(core.transformer)
     # cond=relation: the reference's own gradient update (logit_adjustment.py:88-126) runs between the posterior and the draw.

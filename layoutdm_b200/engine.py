@@ -3,6 +3,7 @@ CUDA tensors.  PyTorch is only used for device memory and the current stream; al
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -34,6 +35,28 @@ def layout_length(sd) -> int:
     raise KeyError("state_dict has no positional table ('<prefix>pos_emb.elem_emb' or '<prefix>pos_emb.pos_emb')")
 
 
+def block_settings(timestep_type: Optional[str], activation: str) -> Tuple[int, int]:
+    """the denoiser block's timestep_type / activation (backbone.encoder_layer, transformer_utils.py:103-170) -> LdmModelDesc's
+    (norm1_kind, activation), refused as the reference refuses them"""
+    if isinstance(timestep_type, str) and timestep_type.endswith("_mlp"):
+        raise NotImplementedError(f"timestep_type={timestep_type!r}: the reference's LayoutDM raises for it when sampling (its _AdaNorm "
+                                  "MLP, nn.Linear(1, ...), is given the long timesteps base.py builds), so there is nothing to reproduce")
+    assert timestep_type in _lib.NORM1_KINDS, f"timestep_type={timestep_type!r} is not one of {list(_lib.NORM1_KINDS)} (transformer_utils.py:124-132)"
+    if activation not in _lib.ACTIVATIONS:
+        raise RuntimeError(f"activation should be relu/gelu/gelu2, not {activation}")        # transformer_utils.py:28-31
+    return _lib.NORM1_KINDS[timestep_type], _lib.ACTIVATIONS[activation]
+
+
+def sinusoidal_table(num_timesteps: int, diffusion_step: int, d: int) -> torch.Tensor:
+    """(T, d) fp32: SinusoidalPosEmb(diffusion_step, d)(t) for t = 0 .. T-1 (transformer_utils.py:34-49, rescale_steps 4000), the
+    reference's own float32 operations on its long timesteps"""
+    x = torch.arange(num_timesteps) / float(diffusion_step) * 4000.0
+    half = d // 2
+    e = torch.exp(torch.arange(half) * -(math.log(10000) / (half - 1)))
+    e = x[:, None] * e[None, :]
+    return torch.cat((e.sin(), e.cos()), dim=-1)
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
 
@@ -57,9 +80,14 @@ def sampling_struct(cfg) -> _lib.LdmSampling:
 class Engine:
     def __init__(self, vocab: Vocab, weights: Dict[str, torch.Tensor], num_timesteps: int = 100, q_type: str = "constrained",
                  operand_dtype: str = "fp16", device: Optional[int] = None, d_model: int = 464, n_heads: int = 8, d_ff: int = 1856,
-                 att_1=0.99999, att_T=0.000009, ctt_1=0.000009, ctt_T=0.99999):
+                 att_1=0.99999, att_T=0.000009, ctt_1=0.000009, ctt_T=0.99999, timestep_type: Optional[str] = "adalayernorm",
+                 activation: str = "relu", diffusion_step: Optional[int] = None):
+        """weights: the `pack_state_dict` arrays.  timestep_type / activation / diffusion_step: the denoiser block's settings
+        (backbone.encoder_layer.*); `load_state_dict` packs later checkpoints with them.  diffusion_step: what the sinusoidal
+        embedding of the *_abs types divides by (None: num_timesteps)."""
         if operand_dtype not in _lib.OPERAND_DTYPES:
             raise ValueError(f"operand_dtype must be one of {', '.join(_lib.OPERAND_DTYPES)}, got {operand_dtype!r}")
+        norm1_kind, act = block_settings(timestep_type, activation)
         if not torch.cuda.is_available():
             raise RuntimeError("layoutdm_b200 needs a CUDA (sm_90a, H100) device; there is no CPU fallback")
         self.lib = _lib.load()
@@ -67,13 +95,15 @@ class Engine:
         self.T = num_timesteps
         self.q_type = q_type
         self.operand_dtype = operand_dtype
+        self.timestep_type, self.activation, self.diffusion_step = timestep_type, activation, diffusion_step
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         self.device = torch.device("cuda", self.device_index)
         L = weights["in_proj_w"].shape[0]
         self.n_layers, self.d_model, self.d_ff = L, d_model, d_ff
         desc = _lib.LdmModelDesc(vocab.n_cat, vocab.n_bins, vocab.n_elem, vocab.n_attr, d_model, n_heads, d_ff, L, num_timesteps,
                                  {"constrained": 0, "vanilla": 1}[q_type], _lib.OPERAND_DTYPES[operand_dtype], self.device_index,
-                                 att_1, att_T, ctt_1, ctt_T, _lib.BBOX_VOCABS[vocab.shared_bbox_vocab], _lib.VAR_ORDERS[vocab.var_order])
+                                 att_1, att_T, ctt_1, ctt_T, norm1_kind, act, _lib.BBOX_VOCABS[vocab.shared_bbox_vocab],
+                                 _lib.VAR_ORDERS[vocab.var_order])
         w = _lib.LdmWeights()
         keep = []
         for name in _lib._W_FIELDS:
@@ -91,14 +121,28 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------------
     @classmethod
-    def from_state_dict(cls, sd: Dict[str, torch.Tensor], vocab: Vocab, num_timesteps: int = 100, **kw) -> "Engine":
-        """sd: the reference LayoutDM `state_dict()` (keys `model.module.transformer.*`, SURVEY.md 8a-a5)."""
-        return cls(vocab, cls.pack_state_dict(sd, vocab), num_timesteps=num_timesteps, **kw)
+    def from_state_dict(cls, sd: Dict[str, torch.Tensor], vocab: Vocab, num_timesteps: int = 100, timestep_type: Optional[str] = "adalayernorm",
+                        activation: str = "relu", diffusion_step: Optional[int] = None, **kw) -> "Engine":
+        """sd: the reference LayoutDM `state_dict()` (keys `model.module.transformer.*`, SURVEY.md 8a-a5), of a model whose blocks
+        have these timestep_type / activation / diffusion_step settings."""
+        block_settings(timestep_type, activation)
+        w = cls.pack_state_dict(sd, vocab, timestep_type, diffusion_step, num_timesteps=num_timesteps)
+        return cls(vocab, w, num_timesteps=num_timesteps, timestep_type=timestep_type, activation=activation, diffusion_step=diffusion_step, **kw)
 
     @staticmethod
-    def pack_state_dict(sd, vocab: Vocab, device=None) -> Dict[str, torch.Tensor]:
+    def pack_state_dict(sd, vocab: Vocab, timestep_type: Optional[str] = "adalayernorm", diffusion_step: Optional[int] = None,
+                        num_timesteps: Optional[int] = None, device=None) -> Dict[str, torch.Tensor]:
         """the reference's parameters in the LdmWeights layout, fp32, on `device` (default: the CPU).  Parameters already on
-        `device` are stacked there, with no host round trip."""
+        `device` are stacked there, with no host round trip.
+
+        norm1 of every timestep_type is a filling of the AdaLN arrays norm1_emb / norm1_w / norm1_b, whose table
+        Linear(SiLU(norm1_emb[t])) gives (scale_t, shift_t) and norm1 = norm(x) * (1 + scale_t) + shift_t:
+          adalayernorm / adainnorm          : the Embedding and Linear as they are
+          adalayernorm_abs / adainnorm_abs  : norm1_emb[l][t] = SinusoidalPosEmb(diffusion_step, d)(t) (`sinusoidal_table`)
+          None (nn.LayerNorm with affine)   : norm1_emb = 0, norm1_w = 0, norm1_b = [weight - 1, bias] -> (1 + scale, shift) = (w, b)
+        The table has num_timesteps rows; the types without an Embedding need num_timesteps (diffusion_step defaults to it).
+        norm1 keys that contradict timestep_type are a ValueError."""
+        block_settings(timestep_type, "relu")          # refuses *_mlp and unknown types
         p = _find_prefix(sd)
         device = torch.device("cpu") if device is None else torch.device(device)
         g = lambda k: sd[p + k].detach().to(device, torch.float32)
@@ -120,12 +164,36 @@ class Engine:
         if pos.shape[0] != vocab.S:
             raise ValueError(f"the state_dict's positional table covers {pos.shape[0]} tokens, the vocabulary has S = {vocab.S} "
                              f"({vocab.n_elem} elements): a model of another max_seq_length")
+        n1 = f"{p}backbone.layers.0.norm1."
+        kind = "None (nn.LayerNorm)" if n1 + "weight" in sd else "an Embedding timestep (adalayernorm / adainnorm)" \
+            if n1 + "emb.weight" in sd else "a sinusoidal timestep (*_abs)" if n1 + "linear.weight" in sd else "no norm1"
+        want = {None: "weight", "adalayernorm": "emb.weight", "adainnorm": "emb.weight"}.get(timestep_type, "linear.weight")
+        if n1 + want not in sd or (want == "linear.weight" and n1 + "emb.weight" in sd):
+            raise ValueError(f"timestep_type={timestep_type!r}, but the state_dict's norm1 keys are those of {kind}")
+        if timestep_type in (None, "adalayernorm_abs", "adainnorm_abs"):
+            if num_timesteps is None:
+                raise ValueError(f"timestep_type={timestep_type!r} has no timestep table in the state_dict: give num_timesteps")
+            d = sd[p + "cat_emb.weight"].shape[1]
+            if timestep_type is None:
+                norm1_emb = torch.zeros(L, num_timesteps, d, device=device)
+                norm1_w = torch.zeros(L, 2 * d, d, device=device)
+                norm1_b = torch.cat([st("norm1.weight") - 1.0, st("norm1.bias")], dim=1)
+            else:
+                sin = sinusoidal_table(num_timesteps, num_timesteps if diffusion_step is None else diffusion_step, d)
+                norm1_emb = sin.to(device)[None].expand(L, -1, -1).contiguous()
+                norm1_w, norm1_b = st("norm1.linear.weight"), st("norm1.linear.bias")
+        else:
+            norm1_emb, norm1_w, norm1_b = st("norm1.emb.weight"), st("norm1.linear.weight"), st("norm1.linear.bias")
+            if num_timesteps is not None:      # an Embedding of diffusion_step rows: the sampler reads rows t < num_timesteps
+                if norm1_emb.shape[1] < num_timesteps:
+                    raise ValueError(f"norm1.emb has {norm1_emb.shape[1]} rows (diffusion_step), fewer than num_timesteps = {num_timesteps}")
+                norm1_emb = norm1_emb[:, :num_timesteps].contiguous()
         return dict(
             cat_emb=g("cat_emb.weight"), pos_table=pos.contiguous(),
             in_proj_w=st("self_attn.in_proj_weight"), in_proj_b=st("self_attn.in_proj_bias"),
             out_proj_w=st("self_attn.out_proj.weight"), out_proj_b=st("self_attn.out_proj.bias"),
             linear1_w=st("linear1.weight"), linear1_b=st("linear1.bias"), linear2_w=st("linear2.weight"), linear2_b=st("linear2.bias"),
-            norm1_emb=st("norm1.emb.weight"), norm1_w=st("norm1.linear.weight"), norm1_b=st("norm1.linear.bias"),
+            norm1_emb=norm1_emb, norm1_w=norm1_w, norm1_b=norm1_b,
             norm2_w=st("norm2.weight"), norm2_b=st("norm2.bias"),
             head_ln_w=g("head.0.weight"), head_ln_b=g("head.0.bias"), head_w=g("head.1.weight"))
 
@@ -156,7 +224,7 @@ class Engine:
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
         """load_weights from a reference LayoutDM `state_dict()` (any of the key prefixes `from_state_dict` takes)"""
-        self.load_weights(self.pack_state_dict(sd, self.vocab, device=self.device))
+        self.load_weights(self.pack_state_dict(sd, self.vocab, self.timestep_type, self.diffusion_step, num_timesteps=self.T, device=self.device))
 
     def close(self):
         if getattr(self, "_h", None):

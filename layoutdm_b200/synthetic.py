@@ -13,9 +13,11 @@ PREFIX = "model.module.transformer."
 
 
 def random_state_dict(vocab: Vocab, num_timesteps: int = 100, d: int = 464, ff: int = 1856, layers: int = 4, seed: int = 0,
-                      std: float = 0.02) -> Dict[str, torch.Tensor]:
+                      std: float = 0.02, timestep_type: Optional[str] = "adalayernorm") -> Dict[str, torch.Tensor]:
     """Weights distributed like the reference's initialisation (base_model.py:108-116: N(0, 0.02) for Linear / Embedding,
-    pos-emb ~ U(0,1) nn_lib.py:109-110), with small non-zero biases / LN affine terms so no term is trivially zero."""
+    pos-emb ~ U(0,1) nn_lib.py:109-110), with small non-zero biases / LN affine terms so no term is trivially zero.
+    timestep_type: the blocks' norm1 keys (transformer_utils.py:151-157): the Embedding of adalayernorm / adainnorm, none for
+    the *_abs types, an affine nn.LayerNorm for None.  The other parameters are drawn as for the default."""
     g = torch.Generator().manual_seed(seed)
     n = lambda *shape, s=std: torch.randn(*shape, generator=g) * s
     sd = {PREFIX + "cat_emb.weight": n(vocab.C, d),
@@ -31,9 +33,13 @@ def random_state_dict(vocab: Vocab, num_timesteps: int = 100, d: int = 464, ff: 
         sd[p + "linear1.bias"] = n(ff)
         sd[p + "linear2.weight"] = n(d, ff)
         sd[p + "linear2.bias"] = n(d)
-        sd[p + "norm1.emb.weight"] = n(num_timesteps, d, s=1.0)
-        sd[p + "norm1.linear.weight"] = n(2 * d, d)
-        sd[p + "norm1.linear.bias"] = n(2 * d)
+        emb, w, b = n(num_timesteps, d, s=1.0), n(2 * d, d), n(2 * d)
+        if timestep_type is None:
+            sd[p + "norm1.weight"], sd[p + "norm1.bias"] = 1.0 + n(d, s=0.1), n(d, s=0.1)
+        else:
+            if not timestep_type.endswith("_abs"):
+                sd[p + "norm1.emb.weight"] = emb
+            sd[p + "norm1.linear.weight"], sd[p + "norm1.linear.bias"] = w, b
         sd[p + "norm2.weight"] = 1.0 + n(d, s=0.1)
         sd[p + "norm2.bias"] = n(d, s=0.1)
     sd[PREFIX + "head.0.weight"] = 1.0 + n(d, s=0.1)
