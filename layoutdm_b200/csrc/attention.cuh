@@ -58,7 +58,7 @@ attention_kernel(const __grid_constant__ OpMaps<MODE> map_qkv /*[M][1536], box 6
   using O = OpT<MODE>;
   using SM = AttSmem<R, SPLIT>;
   extern __shared__ uint8_t att_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(att_smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(att_smem_raw);
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + SM::kOffBar);
 
   // item = (layout * R + query tile) * n_heads + head; the R query tiles and n_heads heads of a layout are neighbours

@@ -18,6 +18,10 @@ constexpr float kLogEps = -69.07755278982137f;  // log(1e-30), T/models/categori
 // ------------------------------------------------------------------------------------------------------------
 LDM_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 LDM_DEVINL void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+// the dynamic shared memory `raw` (an extern __shared__ array) rounded up to 1024 bytes, the 128-byte swizzle's atom.  The
+// offset comes from the shared address, so the result is still `raw` plus an offset and keeps the shared state space: aligned
+// through a generic integer, every access through it compiled to a generic LD / ST
+LDM_DEVINL uint8_t* smem_align1024(uint8_t* raw) { return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u); }
 
 // ------------------------------------------------------------------------------------------------------------
 // programmatic dependent launch (every kernel of the step is launched with programmatic stream serialization): the

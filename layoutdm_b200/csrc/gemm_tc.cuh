@@ -231,7 +231,7 @@ gemm_tc_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box KB x 64 WG_M row
   static_assert(EPI == EPI_LN || WG_M == 2, "plain epilogues use 128-row tiles");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   typename SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
@@ -420,7 +420,7 @@ gemm_rowblock_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 r
   constexpr int kKB = SM::kKB, kCols = SM::kCols;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::kOffBars);
   R ring(smem + SM::kOffRing, bars);
   uint64_t* a_full = bars + 2 * R::kStages;                      // A k-block kb of the current item has landed
@@ -678,7 +678,7 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
   constexpr int kEpi = kGemmConsumers, kProducer = kEpi + kLnEpiThreads;   // first thread of the epilogue warps / producer warp
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   typename SM::R ring(smem, reinterpret_cast<uint64_t*>(smem + SM::kOffBars));
   uint64_t* res_full = ring.empty + SM::R::kStages;             // [2] row half w's residual rows have landed in the buffer
   uint64_t* buf_full = res_full + 2;                             // [2] MMA warpgroup w wrote y into row half w
@@ -728,9 +728,15 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
     const bool copier = et == 0;                             // the row halves' TMA loads and stores
     constexpr uint32_t kHalfBytes = kHalf * kCols * sizeof(float);
     const float inv_n = 1.0f / static_cast<float>(N);
-    constexpr int kVec = kCols / 4;                          // float4 columns of the CTA's part of a row (58)
-    constexpr int kTotal = kHalf * kVec;                     // float4 of a row half; element i = k * 96 + et
-    constexpr int kPerThread = (kTotal + kLnEpiThreads - 1) / kLnEpiThreads;
+    // normalise pass: lane l owns the float4 columns l and, for l < 26, l + 32 of the CTA's 58, so a warp's 16-bit stores of a
+    // row are its 464 contiguous bytes; epilogue warp ew takes the half's rows ew, ew + 3, .., kNormRows of them at a time
+    constexpr int kVec = kCols / 4;
+    constexpr int kEpiWarps = kLnEpiThreads / 32;
+    constexpr int kWarpRows = (kHalf + kEpiWarps - 1) / kEpiWarps;
+    constexpr int kNormRows = 4;
+    static_assert(kVec > 32 && kVec <= 64, "two float4 columns per lane");
+    const int ew = et >> 5;
+    const bool two = lane + 32 < kVec;
     const uint32_t px_var = map_peer(x_var, peer), pxv_full = map_peer(xv_full, peer);
     // the residual rows of row half w of tile t into the buffer (the half is free: every read of it and every store from it is
     // done)
@@ -749,7 +755,18 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
       const int m0 = tile_m0(t), b = it & 1;
       const uint32_t xph = (it >> 1) & 1;
       const LnAffine a = ln_affine(p.ln_scale, p.ln_shift, p.adaln, p.t_layout, p.n_layouts, p.layout_rows, m0, N);
-      const float *gam = a.gam + col0, *bet = a.bet + col0;
+      // gamma + gadd and beta of the lane's columns for the whole tile (one fp32 add, the same bits wherever it is done)
+      float4 gg[2], hh[2];
+#pragma unroll
+      for (int v = 0; v < 2; ++v) {
+        gg[v] = hh[v] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (v == 0 || two) {
+          const int c = col0 + 4 * (lane + 32 * v);
+          const float4 g = __ldg(reinterpret_cast<const float4*>(a.gam + c));
+          gg[v] = make_float4(g.x + a.gadd, g.y + a.gadd, g.z + a.gadd, g.w + a.gadd);
+          hh[v] = __ldg(reinterpret_cast<const float4*>(a.bet + c));
+        }
+      }
       typename O::T* out16 = static_cast<typename O::T*>(p.out) + col0;
       const bool keep32 = p.out32 != nullptr;
 #pragma unroll 1
@@ -790,19 +807,37 @@ gemm_ln_kernel(const __grid_constant__ OpMaps<MODE> map_a /*box 32 x 128 rows*/,
           }
         }
         named_bar_sync(1, kLnEpiThreads);
-        // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a TMA store
-#pragma unroll 6
-        for (int k = 0; k < kPerThread; ++k) {
-          const int i = k * kLnEpiThreads + et, r = h0 + i / kVec, c = (i - (r - h0) * kVec) * 4;
-          if (i >= kTotal) continue;
-          float4* bp = reinterpret_cast<float4*>(buf + r * kLd + c);
-          const float4 y = *bp;
-          const float4 g = __ldg(reinterpret_cast<const float4*>(gam + c)), h = __ldg(reinterpret_cast<const float4*>(bet + c));
-          const float piv = s_piv[r], s = s_sum[r], rstd = s_var[r];
-          const float4 v = make_float4(fmaf(fmaf(-s, inv_n, y.x - piv) * rstd, g.x + a.gadd, h.x), fmaf(fmaf(-s, inv_n, y.y - piv) * rstd, g.y + a.gadd, h.y),
-                                       fmaf(fmaf(-s, inv_n, y.z - piv) * rstd, g.z + a.gadd, h.z), fmaf(fmaf(-s, inv_n, y.w - piv) * rstd, g.w + a.gadd, h.w));
-          *reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N + c) = make_uint2(O::pack(v.x, v.y), O::pack(v.z, v.w));
-          if (keep32) *bp = v;
+        // normalise: 16-bit outputs stored here, the fp32 ones written back into the buffer for a TMA store.  A group's loads
+        // all come before its stores, which keeps them in flight together
+#pragma unroll 1
+        for (int k0 = 0; k0 < kWarpRows; k0 += kNormRows) {
+          float4 y[kNormRows][2];
+          float piv[kNormRows], s[kNormRows], rstd[kNormRows];
+#pragma unroll
+          for (int u = 0; u < kNormRows; ++u) {
+            const int r = h0 + ew + kEpiWarps * (k0 + u);
+            if (r - h0 >= kHalf) continue;
+            const float4* yr = reinterpret_cast<const float4*>(buf + r * kLd) + lane;
+            y[u][0] = yr[0];
+            if (two) y[u][1] = yr[32];
+            piv[u] = s_piv[r]; s[u] = s_sum[r]; rstd[u] = s_var[r];
+          }
+#pragma unroll
+          for (int u = 0; u < kNormRows; ++u) {
+            const int r = h0 + ew + kEpiWarps * (k0 + u);
+            if (r - h0 >= kHalf) continue;
+            uint2* o16 = reinterpret_cast<uint2*>(out16 + static_cast<size_t>(m0 + r) * N) + lane;
+            float4* o32 = reinterpret_cast<float4*>(buf + r * kLd) + lane;
+#pragma unroll
+            for (int v = 0; v < 2; ++v) {
+              if (v == 1 && !two) continue;
+              const float4 yv = y[u][v], g = gg[v], h = hh[v];
+              const float4 o = make_float4(fmaf(fmaf(-s[u], inv_n, yv.x - piv[u]) * rstd[u], g.x, h.x), fmaf(fmaf(-s[u], inv_n, yv.y - piv[u]) * rstd[u], g.y, h.y),
+                                           fmaf(fmaf(-s[u], inv_n, yv.z - piv[u]) * rstd[u], g.z, h.z), fmaf(fmaf(-s[u], inv_n, yv.w - piv[u]) * rstd[u], g.w, h.w));
+              o16[32 * v] = make_uint2(O::pack(o.x, o.y), O::pack(o.z, o.w));
+              if (keep32) o32[32 * v] = o;
+            }
+          }
         }
         if (keep32) fence_proxy_async_smem();                // the fp32 rows are visible to the TMA store
         named_bar_sync(1, kLnEpiThreads);

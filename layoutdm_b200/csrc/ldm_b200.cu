@@ -57,14 +57,14 @@ constexpr int kHeadBN = 160, kHeadStages = 4;     // vocabulary head: 128 x 160 
 // the fragment-epilogue kernel below, 64 x 464 tiles
 constexpr int kLnBN = 232, kLnStages = 3;
 constexpr int kLnSplitRows = 64;   // A box rows of the split mode's LN GEMMs (the one-plane kernel's: LnSmem<>::kRows)
-// ring stages of gemm_ln_kernel: FF2 (K = 1856) waits on its operand feed and takes the most that fit; the out-projection
-// (K = 512) waits on its epilogue, which measured faster beside the smaller shared-memory footprint of 3 stages (DESIGN §4)
-constexpr int kLnOutStages = 3, kLnFf2Stages = 4;
-using LnOut = LnSmem<kLnOutStages>;
-using LnFf2 = LnSmem<kLnFf2Stages>;
+// ring stages of gemm_ln_kernel, the most that fit beside the tile buffer, for both GEMMs: FF2 (K = 1856) waits on its operand
+// feed, and the out-projection (K = 512), which took 3 while it waited on its epilogue passes, is faster with 4 since those
+// passes run from shared memory (DESIGN §4)
+constexpr int kLnPairStages = 4;
+using LnPair = LnSmem<kLnPairStages>;
 // k-block of the LN GEMMs' operands (the TMA box columns) in every mode: the persistent kernel's, which is the split mode's
-constexpr int kLnKB = LnFf2::R::kKB;
-static_assert(LnOut::R::kKB == kLnKB && LnFf2::kCols == kLnBN && LnFf2::kPairCols == kDModel && kAttN % kLnKB == 0 &&
+constexpr int kLnKB = LnPair::R::kKB;
+static_assert(LnPair::kCols == kLnBN && LnPair::kPairCols == kDModel && kAttN % kLnKB == 0 &&
               4 * kDModel % kLnKB == 0 && gemm_kb(true) == kLnKB, "LN GEMM shapes");
 template <int EPI, int MODE> constexpr auto kGemmPlainSplit = gemm_tc_kernel<kPlainBN, 2, kPlainStages, EPI, MODE>;
 template <int MODE> constexpr auto kGemmHead = gemm_tc_kernel<kHeadBN, 2, kHeadStages, EPI_F32, MODE>;
@@ -405,20 +405,19 @@ int set_smem(LdmHandle* h) {
   CK(cudaFuncSetAttribute(kGemmHead<MODE>, attr, kHeadSmem));
   if constexpr (kOpSplit<MODE>) CK(cudaFuncSetAttribute(kGemmLn<MODE>, attr, kLnSmem));
   else {
-    CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnOutStages>, attr, LnOut::kBytes));
-    CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnFf2Stages>, attr, LnFf2::kBytes));
+    CK(cudaFuncSetAttribute(gemm_ln_kernel<MODE, kLnPairStages>, attr, LnPair::kBytes));
   }
   CK(cudaFuncSetAttribute(attention_kernel<MODE, 1>, attr, AttSmem<1, kOpSplit<MODE>>::kBytes));
   CK(cudaFuncSetAttribute(attention_kernel<MODE, 2>, attr, AttSmem<2, kOpSplit<MODE>>::kBytes));
   if constexpr (!kOpSplit<MODE>) {
-    // the larger of the two: the out-projection's pairs fit wherever FF2's do (the same threads and registers, less shared memory)
+    // the CTA pairs of the one gemm_ln_kernel that both LN GEMMs launch
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2); cfg.blockDim = dim3(kLnThreads); cfg.dynamicSmemBytes = LnFf2::kBytes;
+    cfg.gridDim = dim3(2); cfg.blockDim = dim3(kLnThreads); cfg.dynamicSmemBytes = LnPair::kBytes;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim = {2, 1, 1};
     cfg.attrs = at; cfg.numAttrs = 1;
-    CK(cudaOccupancyMaxActiveClusters(&h->ln_clusters, gemm_ln_kernel<MODE, kLnFf2Stages>, &cfg));
-    if (h->ln_clusters < 1) return fail(LDM_ERR_UNSUPPORTED, "gemm_ln_kernel: no CTA pair of %d bytes of shared memory fits the device", LnFf2::kBytes);
+    CK(cudaOccupancyMaxActiveClusters(&h->ln_clusters, gemm_ln_kernel<MODE, kLnPairStages>, &cfg));
+    if (h->ln_clusters < 1) return fail(LDM_ERR_UNSUPPORTED, "gemm_ln_kernel: no CTA pair of %d bytes of shared memory fits the device", LnPair::kBytes);
   }
   return LDM_OK;
 }
@@ -476,7 +475,7 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   const int kb = gemm_kb(h->split);
   if ((rc = make_op_maps(h, h->x16, M, d, kBM, kb))) return rc;
   if ((rc = make_op_maps(h, h->z16, M, d, kBM, kb))) return rc;
-  const int ln_rows = h->split ? kLnSplitRows : LnFf2::kRows;
+  const int ln_rows = h->split ? kLnSplitRows : LnPair::kRows;
   if ((rc = make_op_maps(h, h->att16, M, kAttN, ln_rows, kLnKB))) return rc;
   if ((rc = make_op_maps(h, h->hid16, M, ff, ln_rows, kLnKB))) return rc;
   // attention's Q / K / V head tiles: 128 rows x one padded head, in every mode
@@ -485,8 +484,8 @@ int ensure_workspace(LdmHandle* h, int n_layouts) {
   if (!h->split && (rc = make_map(&h->m_qkv16_st, h->qkv16.hi, M, kQkvN, kBM, 64, h->bf16))) return rc;
   if (!h->split && (rc = make_map(&h->m_hid16_st, h->hid16.hi, M, ff, kBM, 64, h->bf16))) return rc;
   // the persistent LN GEMMs' residual loads and fp32 stores: one row half of the CTA's columns per box
-  if (!h->split && (rc = make_map_f32(&h->m_x32, h->x32, M, d, LnFf2::kHalf, kLnBN))) return rc;
-  if (!h->split && (rc = make_map_f32(&h->m_y32, h->y32, M, d, LnFf2::kHalf, kLnBN))) return rc;
+  if (!h->split && (rc = make_map_f32(&h->m_x32, h->x32, M, d, LnPair::kHalf, kLnBN))) return rc;
+  if (!h->split && (rc = make_map_f32(&h->m_y32, h->y32, M, d, LnPair::kHalf, kLnBN))) return rc;
   return LDM_OK;
 }
 
@@ -526,8 +525,7 @@ int launch_denoiser(LdmHandle* h, int n, const long long* ids_in, int t_model, c
       return launch_step(h, kGemmLn<MODE>, grid(M / kLnSplitRows, false), kGemmThreads, kLnSmem, st, a, w, p);
     } else {
       const int pairs = std::min({nb, h->ln_clusters, h->gemm_ctas > 0 ? std::max(1, h->gemm_ctas / 2) : nb});
-      if (p.K == kAttN) return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnOutStages>, dim3(2 * pairs), kLnThreads, LnOut::kBytes, st, a, w, res, st32, p);
-      return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnFf2Stages>, dim3(2 * pairs), kLnThreads, LnFf2::kBytes, st, a, w, res, st32, p);
+      return launch_cluster(h, 2, gemm_ln_kernel<MODE, kLnPairStages>, dim3(2 * pairs), kLnThreads, LnPair::kBytes, st, a, w, res, st32, p);
     }
   };
   // instance-norm blocks (norm1_kind 1): norm1 of layer l is its own pass over the fp32 rows x32 (instance_norm_kernel); layer 0's
